@@ -60,7 +60,6 @@ static void free_cloud(Cloud &c) {
   if (c.d_sorted) cudaFree(c.d_sorted);
   if (c.d_rel) cudaFree(c.d_rel);
   if (c.d_cell_off) cudaFree(c.d_cell_off);
-  if (c.d_cell_id) cudaFree(c.d_cell_id);
   if (c.d_coarse) cudaFree(c.d_coarse);
   if (c.d_hkey) cudaFree(c.d_hkey);
   if (c.d_hval) cudaFree(c.d_hval);
@@ -235,6 +234,7 @@ void me_destroy(me_ctx *ctx) {
   if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
   if (ctx->d_work) cudaFree(ctx->d_work);
   if (ctx->d_scan_tmp) cudaFree(ctx->d_scan_tmp);
+  if (ctx->d_rank) cudaFree(ctx->d_rank);
   if (ctx->d_rs_hist) cudaFree(ctx->d_rs_hist);
   for (int i = 0; i < 2 * ME_N_STAGE_TIMES; ++i) if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
   if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);

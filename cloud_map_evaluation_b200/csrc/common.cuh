@@ -88,8 +88,6 @@ struct Cloud {
   long long cap_hash = 0;
   uint32_t hmask = 0;
   long long n_seg = 0;
-  uint32_t *d_cell_id = nullptr;    // scratch: cell of each point (caller order)
-  long long cap_cell_id = 0;
   uint32_t *d_tiles = nullptr;      // non-empty query tiles (tile id = (bz*nb[1]+by)*nb[0]+bx)
   long long cap_tiles = 0;
   long long n_tiles = 0;
@@ -177,8 +175,10 @@ struct me_ctx {
   // large device scratch (scan partials, far list, voxel tables)
   void *d_work = nullptr;
   size_t work_bytes = 0;
-  uint32_t *d_scan_tmp = nullptr;   // per-tile partials of exclusive_scan_inplace
+  unsigned long long *d_scan_tmp = nullptr;   // tile status words of exclusive_scan_inplace
   long long cap_scan_tmp = 0;
+  uint32_t *d_rank = nullptr;       // dense build: in-cell rank of every point of the cloud being laid out (caller order)
+  long long cap_rank = 0;
   uint32_t *d_rs_hist = nullptr;    // radix sort: digit histograms of every tile
   long long cap_rs_hist = 0;
   cudaEvent_t ev[2 * ME_N_STAGE_TIMES];
@@ -274,7 +274,7 @@ double density_edge(const Cloud &c);
 int build_both(me_ctx *ctx);
 int build_tiles(me_ctx *ctx, int which);
 int query_shard(me_ctx *ctx, int which, long long *b, long long *e);
-int exclusive_scan_inplace(me_ctx *ctx, uint32_t *a, long long n);
+int exclusive_scan_inplace(me_ctx *ctx, uint32_t *a, long long n, unsigned long long *stats = nullptr);
 int voxel_downsample(me_ctx *ctx, int which, double voxel_size, int64_t *n_out);
 int radix_sort_pairs(me_ctx *ctx, unsigned long long *keys, uint32_t *vals, unsigned long long *keys_tmp, uint32_t *vals_tmp,
                      long long n, int key_bits, unsigned long long **keys_sorted, uint32_t **vals_sorted);

@@ -114,135 +114,167 @@ int compute_bbox(me_ctx *ctx, int which) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// cell histogram
+// dense build: cell histogram -> exclusive scan -> scatter -> fp32 screening copy.  Both point passes read the
+// caller-order fp64 cloud through shared memory, one tile of kThreads points at a time: the block loads the tile's
+// 3 * kThreads coordinates with consecutive 16-byte loads (8-byte loads if the cloud is only 8-byte aligned), so every
+// load instruction is fully used, and each thread then takes its point from shared memory.  The histogram keeps the
+// value its atomic returned, the point's rank in its cell; the scatter recomputes the cell from the coordinates and
+// writes the point to off[cell] + rank with plain loads of the scanned table.  (The atomics in the histogram meet a
+// count table that lives in L2; taking the slots with atomics in the scatter instead, against 320 MB of random record
+// writes, made the scatter 1.2x slower on C3.)
 // ---------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void stage_tile(const double *__restrict__ xyz, long long n, bool aligned16, long long p0,
+                                           double *__restrict__ s) {
+  const long long nd = 3 * (n - p0 < kThreads ? n - p0 : kThreads);      // coordinates in this tile
+  const double *src = xyz + 3 * p0;
+  if (aligned16 && nd == 3 * kThreads) {       // a tile starts 16-byte aligned: 3 * kThreads * 8 B is a multiple of 16
+    const double2 *q = reinterpret_cast<const double2 *>(src);
+    double2 *d = reinterpret_cast<double2 *>(s);
+    for (int k = threadIdx.x; k < 3 * kThreads / 2; k += kThreads) d[k] = __ldg(q + k);
+  } else {
+    for (int k = threadIdx.x; k < nd; k += kThreads) s[k] = __ldg(src + k);
+  }
+}
+
+// lattice cell of a point; points define the lattice, so the coordinates are in range by construction: clamp against
+// surprises
+__device__ __forceinline__ void point_cell(double x, double y, double z, const Lattice &L, int &ix, int &iy, int &iz) {
+  long long cx = cell_coord(x, L, 0), cy = cell_coord(y, L, 1), cz = cell_coord(z, L, 2);
+  ix = (int)(cx < 0 ? 0 : (cx >= L.dims[0] ? L.dims[0] - 1 : cx));
+  iy = (int)(cy < 0 ? 0 : (cy >= L.dims[1] ? L.dims[1] - 1 : cy));
+  iz = (int)(cz < 0 ? 0 : (cz >= L.dims[2] ? L.dims[2] - 1 : cz));
+}
+
 __global__ void __launch_bounds__(kThreads) cell_count_kernel(const double *__restrict__ xyz, long long n, Lattice L,
-                                                              uint32_t *__restrict__ cell_id,
-                                                              uint32_t *__restrict__ count) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    double x = __ldg(xyz + 3 * i), y = __ldg(xyz + 3 * i + 1), z = __ldg(xyz + 3 * i + 2);
-    long long ix = cell_coord(x, L, 0), iy = cell_coord(y, L, 1), iz = cell_coord(z, L, 2);
-    // points define the lattice, so the coordinates are in range by construction; clamp against surprises
-    ix = ix < 0 ? 0 : (ix >= L.dims[0] ? L.dims[0] - 1 : ix);
-    iy = iy < 0 ? 0 : (iy >= L.dims[1] ? L.dims[1] - 1 : iy);
-    iz = iz < 0 ? 0 : (iz >= L.dims[2] ? L.dims[2] - 1 : iz);
-    long long c = (iz * L.dims[1] + iy) * (long long)L.dims[0] + ix;
-    cell_id[i] = (uint32_t)c;
-    atomicAdd(count + c, 1u);
+                                                              uint32_t *__restrict__ count, uint32_t *__restrict__ rank) {
+  __shared__ __align__(16) double s[3 * kThreads];
+  const bool aligned16 = ((uintptr_t)xyz & 15) == 0;
+  for (long long p0 = (long long)blockIdx.x * kThreads; p0 < n; p0 += (long long)gridDim.x * kThreads) {
+    __syncthreads();
+    stage_tile(xyz, n, aligned16, p0, s);
+    __syncthreads();
+    if (p0 + threadIdx.x < n) {
+      int ix, iy, iz;
+      point_cell(s[3 * threadIdx.x], s[3 * threadIdx.x + 1], s[3 * threadIdx.x + 2], L, ix, iy, iz);
+      rank[p0 + threadIdx.x] = atomicAdd(count + ((long long)iz * L.dims[1] + iy) * (long long)L.dims[0] + ix, 1u);
+    }
   }
-}
-
-// occupancy statistics of the histogram: [0] occupied cells, [1] max count
-__global__ void __launch_bounds__(kThreads) occupancy_kernel(const uint32_t *__restrict__ count, long long ncells,
-                                                             unsigned long long *__restrict__ stats) {
-  unsigned long long occ = 0, mx = 0;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < ncells;
-       i += (long long)gridDim.x * blockDim.x) {
-    uint32_t c = __ldg(count + i);
-    occ += c != 0;
-    mx = c > mx ? c : mx;
-  }
-  occ = (unsigned long long)warp_sum_ll((long long)occ);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) { unsigned long long t = __shfl_xor_sync(0xffffffffu, mx, o); mx = t > mx ? t : mx; }
-  if ((threadIdx.x & 31) == 0) { atomicAdd(stats, occ); atomicMax(stats + 1, mx); }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// in-place exclusive scan over the cell counts (3 phases: tile sums, scan of tile sums, tile scan + offset)
+// in-place exclusive scan, single pass (decoupled look-back): every block scans its tile of kScanTile values, publishes
+// the tile's sum, and takes its offset from the published sums / inclusive prefixes of the tiles before it.  Blocks start
+// in blockIdx order, so a tile only ever waits on tiles that are running or done.  Optionally it also reduces the
+// statistics of the values: stats[0] += number of non-zero values, stats[1] = max(stats[1], largest value).
 // ---------------------------------------------------------------------------------------------------------------
 static constexpr int kScanItems = 8;                       // per thread
-static constexpr int kScanTile = kThreads * kScanItems;    // 2048 cells per block
+static constexpr int kScanTile = kThreads * kScanItems;    // 2048 values per block
+// tile status word: flag in the high 32 bits (0: nothing yet, 1: tile sum, 2: inclusive prefix), the value in the low 32
+static constexpr unsigned long long kTileSum = 1ull << 32, kTilePrefix = 2ull << 32;
 
-__global__ void __launch_bounds__(kThreads) scan_tile_sum_kernel(const uint32_t *__restrict__ a, long long n,
-                                                                 uint32_t *__restrict__ tile_sum) {
+__global__ void __launch_bounds__(kThreads) scan_kernel(uint32_t *__restrict__ a, long long n,
+                                                        unsigned long long *__restrict__ status,
+                                                        unsigned long long *__restrict__ stats) {
+  __shared__ uint32_t s[kScanTile + kScanTile / 32];      // padded: conflict-free in both the striped and blocked order
   __shared__ uint32_t ws[kThreads / 32];
-  long long base = (long long)blockIdx.x * kScanTile;
-  uint32_t s = 0;
+  __shared__ uint32_t tile_off;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long tile = blockIdx.x, base = tile * kScanTile;
+  // coalesced loads (a need not be 16-byte aligned), then every thread takes kScanItems consecutive values
 #pragma unroll
   for (int k = 0; k < kScanItems; ++k) {
-    long long i = base + (long long)k * kThreads + threadIdx.x;
-    if (i < n) s += __ldg(a + i);
+    const int j = k * kThreads + threadIdx.x;
+    s[j + (j >> 5)] = base + j < n ? a[base + j] : 0u;
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = s;
   __syncthreads();
-  if (threadIdx.x == 0) {
-    uint32_t t = 0;
-    for (int w = 0; w < kThreads / 32; ++w) t += ws[w];
-    tile_sum[blockIdx.x] = t;
+  uint32_t v[kScanItems], sum = 0, occ = 0, mx = 0;
+#pragma unroll
+  for (int k = 0; k < kScanItems; ++k) {
+    const int j = threadIdx.x * kScanItems + k;
+    v[k] = s[j + (j >> 5)];
+    sum += v[k]; occ += v[k] != 0u; mx = max(mx, v[k]);
   }
-}
-
-// single block: exclusive scan of the tile sums, in place
-__global__ void __launch_bounds__(1024) scan_tile_offsets_kernel(uint32_t *__restrict__ tile_sum, long long ntiles) {
-  __shared__ uint32_t ws[32];
-  __shared__ uint32_t carry_s;
-  if (threadIdx.x == 0) carry_s = 0;
+  uint32_t inc = sum;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
+  if (lane == 31) ws[warp] = inc;
+  if (stats) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { occ += __shfl_xor_sync(0xffffffffu, occ, o); mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o)); }
+    if (lane == 0 && (occ || mx)) { atomicAdd(stats, (unsigned long long)occ); atomicMax(stats + 1, (unsigned long long)mx); }
+  }
   __syncthreads();
-  for (long long base = 0; base < ntiles; base += 1024) {
-    long long i = base + threadIdx.x;
-    uint32_t v = i < ntiles ? tile_sum[i] : 0u;
-    uint32_t inc = v;
+  if (warp == 0) {
+    uint32_t w = lane < kThreads / 32 ? ws[lane] : 0u, winc = w;
 #pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, inc, o); if ((threadIdx.x & 31) >= o) inc += t; }
-    if ((threadIdx.x & 31) == 31) ws[threadIdx.x >> 5] = inc;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      uint32_t w = ws[threadIdx.x];
-      uint32_t winc = w;
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, winc, o); if (lane >= o) winc += t; }
+    if (lane < kThreads / 32) ws[lane] = winc - w;                       // exclusive prefix of the warp sums
+    const uint32_t total = __shfl_sync(0xffffffffu, winc, 31);
+    volatile unsigned long long *st = status;
+    uint32_t off = 0;
+    if (tile == 0) {
+      if (lane == 0) st[0] = kTilePrefix | total;
+    } else {
+      if (lane == 0) st[tile] = kTileSum | total;
+      // look back over windows of 32 predecessors (lane l: tile - 1 - l) until one holds an inclusive prefix
+      for (long long w0 = tile - 1;; w0 -= 32) {
+        const long long t = w0 - lane;
+        unsigned long long x;
+        do {
+          x = kTilePrefix;      // before tile 0: an inclusive prefix of 0
+          if (t >= 0) x = st[t];
+        } while (__any_sync(0xffffffffu, (x >> 32) == 0ull));
+        const unsigned pre = __ballot_sync(0xffffffffu, (x >> 32) == 2ull);
+        const int stop = pre ? __ffs(pre) - 1 : 32;                    // nearest predecessor with its inclusive prefix
+        uint32_t part = lane <= stop ? (uint32_t)x : 0u;
 #pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, winc, o); if (threadIdx.x >= o) winc += t; }
-      ws[threadIdx.x] = winc - w;   // exclusive prefix of warp sums
+        for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+        off += part;
+        if (pre) break;
+      }
+      if (lane == 0) st[tile] = kTilePrefix | (off + total);
     }
-    __syncthreads();
-    uint32_t carry = carry_s;
-    uint32_t excl = carry + ws[threadIdx.x >> 5] + inc - v;
-    if (i < ntiles) tile_sum[i] = excl;
-    __syncthreads();
-    if (threadIdx.x == 1023) carry_s = excl + v;
-    __syncthreads();
+    if (lane == 0) tile_off = off;
+  }
+  __syncthreads();
+  uint32_t run = tile_off + ws[warp] + inc - sum;
+#pragma unroll
+  for (int k = 0; k < kScanItems; ++k) {
+    const int j = threadIdx.x * kScanItems + k;
+    s[j + (j >> 5)] = run;
+    run += v[k];
+  }
+  __syncthreads();
+#pragma unroll
+  for (int k = 0; k < kScanItems; ++k) {
+    const int j = k * kThreads + threadIdx.x;
+    if (base + j < n) a[base + j] = s[j + (j >> 5)];
   }
 }
 
-// per tile: exclusive scan + tile offset, written in place (count[c] -> start[c])
-__global__ void __launch_bounds__(kThreads) scan_apply_kernel(uint32_t *__restrict__ a, long long n,
-                                                              const uint32_t *__restrict__ tile_off) {
-  __shared__ uint32_t ws[kThreads / 32];
-  long long base = (long long)blockIdx.x * kScanTile + (long long)threadIdx.x * kScanItems;
-  uint32_t v[kScanItems];
-  uint32_t s = 0;
-#pragma unroll
-  for (int k = 0; k < kScanItems; ++k) { long long i = base + k; v[k] = i < n ? a[i] : 0u; s += v[k]; }
-  uint32_t inc = s;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, inc, o); if ((threadIdx.x & 31) >= o) inc += t; }
-  if ((threadIdx.x & 31) == 31) ws[threadIdx.x >> 5] = inc;
-  __syncthreads();
-  uint32_t woff = 0;
-  for (int w = 0; w < (int)(threadIdx.x >> 5); ++w) woff += ws[w];
-  uint32_t run = tile_off[blockIdx.x] + woff + inc - s;
-#pragma unroll
-  for (int k = 0; k < kScanItems; ++k) { long long i = base + k; if (i < n) a[i] = run; run += v[k]; }
-}
-
 // ---------------------------------------------------------------------------------------------------------------
-// scatter: slot = start[c]++ on off[c+1]; afterwards off[c+1] = end of cell c = start of cell c+1 (CSR)
+// scatter: point i of cell c goes to slot off[c] + rank[i]; off[] is the CSR offset array of the scan and stays as it is
 // ---------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kThreads) scatter_kernel(const double *__restrict__ xyz, long long n,
-                                                           const uint32_t *__restrict__ cell_id,
-                                                           uint32_t *__restrict__ cell_cursor,
-                                                           P4 *__restrict__ sorted, int axis, int dimx, int dimy, int c_lo, int c_hi) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    uint32_t c = __ldg(cell_id + i);
+__global__ void __launch_bounds__(kThreads) scatter_kernel(const double *__restrict__ xyz, long long n, Lattice L,
+                                                           const uint32_t *__restrict__ off, const uint32_t *__restrict__ rank,
+                                                           P4 *__restrict__ sorted, int axis, int c_lo, int c_hi) {
+  __shared__ __align__(16) double s[3 * kThreads];
+  const bool aligned16 = ((uintptr_t)xyz & 15) == 0;
+  for (long long p0 = (long long)blockIdx.x * kThreads; p0 < n; p0 += (long long)gridDim.x * kThreads) {
+    __syncthreads();
+    stage_tile(xyz, n, aligned16, p0, s);
+    __syncthreads();
+    const long long i = p0 + threadIdx.x;
+    if (i >= n) continue;
+    const double x = s[3 * threadIdx.x], y = s[3 * threadIdx.x + 1], z = s[3 * threadIdx.x + 2];
+    int ix, iy, iz;
+    point_cell(x, y, z, L, ix, iy, iz);
     if (axis) {      // slab layout: points outside this rank's planes are not laid out
-      const uint32_t row = c / (uint32_t)dimx;
-      const int a = axis == 2 ? (int)(row / (uint32_t)dimy) : (int)(row % (uint32_t)dimy);
+      const int a = axis == 2 ? iz : iy;
       if (a < c_lo || a >= c_hi) continue;
     }
-    uint32_t slot = atomicAdd(cell_cursor + c, 1u);
-    double x = __ldg(xyz + 3 * i), y = __ldg(xyz + 3 * i + 1), z = __ldg(xyz + 3 * i + 2);
+    const uint32_t c = (uint32_t)(((long long)iz * L.dims[1] + iy) * (long long)L.dims[0] + ix);
+    const uint32_t slot = __ldg(off + c) + __ldg(rank + i);
     double2 *o = reinterpret_cast<double2 *>(sorted + slot);
     o[0] = make_double2(x, y);
     o[1] = make_double2(z, __longlong_as_double((long long)(((unsigned long long)c << 32) | (unsigned long long)i)));
@@ -251,7 +283,9 @@ __global__ void __launch_bounds__(kThreads) scatter_kernel(const double *__restr
 
 // fp32 screening copy of the sorted cloud (streaming pass, coalesced both ways): offset of every point from the origin
 // of its own cell (|offset| < ~h, so the fp32 rounding error is ~3e-8 h whatever the world extent) and the cell's x
-// index.  The sweeps rebuild the offset between two points as (ix_a - ix_b) * h + (rel_a - rel_b).
+// index.  The sweeps rebuild the offset between two points as (ix_a - ix_b) * h + (rel_a - rel_b).  A pass of its own:
+// written from the scatter, as a random 16-byte write next to each record, it made the scatter 2.3x slower on C3, far
+// more than this pass costs.
 __global__ void __launch_bounds__(kThreads) rel_kernel(const P4 *__restrict__ sorted, long long n, Lattice L,
                                                        float4 *__restrict__ rel) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
@@ -403,25 +437,24 @@ static bool make_lattice(const Cloud &c, double v, int m, long long budget, Latt
 
 static int histogram(me_ctx *ctx, Cloud &c, const Lattice &L) {
   ME_TRY(ensure(ctx, (void **)&c.d_cell_off, &c.cap_cells, L.ncells + 1, sizeof(uint32_t)));
-  ME_TRY(ensure(ctx, (void **)&c.d_cell_id, &c.cap_cell_id, c.n, sizeof(uint32_t)));
-  // counts live at off[1..ncells]; off[0] stays 0, so after scan + scatter off[] is a CSR offset array
+  // counts live at off[0..ncells-1] and off[ncells] stays 0, so the exclusive scan of all ncells + 1 entries turns off[]
+  // into the CSR offset array; the in-cell rank of every point goes to ctx->d_rank
   ME_CUDA(ctx, cudaMemsetAsync(c.d_cell_off, 0, (size_t)(L.ncells + 1) * sizeof(uint32_t), ctx->stream));
+  ME_TRY(ensure(ctx, (void **)&ctx->d_rank, &ctx->cap_rank, c.n, sizeof(uint32_t)));
   int blocks = (int)std::min<long long>((c.n + kThreads - 1) / kThreads, (long long)ctx->sm_count * 16);
-  cell_count_kernel<<<blocks, kThreads, 0, ctx->stream>>>(c.d_xyz, c.n, L, c.d_cell_id, c.d_cell_off + 1);
+  cell_count_kernel<<<blocks, kThreads, 0, ctx->stream>>>(c.d_xyz, c.n, L, c.d_cell_off, ctx->d_rank);
   ME_LAUNCH_CHECK(ctx);
   return ME_OK;
 }
 
-static int occupancy(me_ctx *ctx, Cloud &c, const Lattice &L, long long *occupied, long long *max_count) {
-  unsigned long long *s = (unsigned long long *)ctx->d_scratch;
-  ME_CUDA(ctx, cudaMemsetAsync(s, 0, 2 * sizeof(unsigned long long), ctx->stream));
-  int blocks = (int)std::min<long long>((L.ncells + kThreads - 1) / kThreads, (long long)ctx->sm_count * 16);
-  occupancy_kernel<<<blocks, kThreads, 0, ctx->stream>>>(c.d_cell_off + 1, L.ncells, s);
-  ME_LAUNCH_CHECK(ctx);
-  unsigned long long *h = (unsigned long long *)ctx->h_pinned;
-  ME_CUDA(ctx, cudaMemcpyAsync(h, s, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
-  ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  *occupied = (long long)h[0]; *max_count = (long long)h[1];
+// exclusive scan of the cell counts, in place, with their statistics on the way: pinned slots [9] occupied cells, [10]
+// points in the fullest cell (bounds the run lengths of the sweeps), valid once the stream is synchronized
+static int scan_cells(me_ctx *ctx, Cloud &c, const Lattice &L) {
+  unsigned long long *d = (unsigned long long *)ctx->d_scratch + 9;
+  ME_CUDA(ctx, cudaMemsetAsync(d, 0, 2 * sizeof(unsigned long long), ctx->stream));
+  ME_TRY(exclusive_scan_inplace(ctx, c.d_cell_off, L.ncells + 1, d));
+  ME_CUDA(ctx, cudaMemcpyAsync((unsigned long long *)ctx->h_pinned + 9, d, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                               ctx->stream));
   return ME_OK;
 }
 
@@ -495,17 +528,13 @@ bool plan_lattice_host(const double bmin[3], const double bmax[3], long long n, 
   return choose_lattice(c, o.bbox_valid ? &o : nullptr, v_req, h_target, budget, allow_sparse, &v, &m, out);
 }
 
-// in-place exclusive scan of n uint32 (3 phases; the per-tile partials live in a small buffer of their own, so callers
-// may keep data in the work buffer across the scan)
-int exclusive_scan_inplace(me_ctx *ctx, uint32_t *a, long long n) {
+// in-place exclusive scan of n uint32, one pass (scan_kernel; the tile status words live in a small buffer of their own,
+// so callers may keep data in the work buffer across the scan).  stats: see scan_kernel; the caller clears them.
+int exclusive_scan_inplace(me_ctx *ctx, uint32_t *a, long long n, unsigned long long *stats) {
   const long long ntiles = (n + kScanTile - 1) / kScanTile;
-  ME_TRY(ensure(ctx, (void **)&ctx->d_scan_tmp, &ctx->cap_scan_tmp, ntiles, sizeof(uint32_t)));
-  uint32_t *tile = ctx->d_scan_tmp;
-  scan_tile_sum_kernel<<<(unsigned)ntiles, kThreads, 0, ctx->stream>>>(a, n, tile);
-  ME_LAUNCH_CHECK(ctx);
-  scan_tile_offsets_kernel<<<1, 1024, 0, ctx->stream>>>(tile, ntiles);
-  ME_LAUNCH_CHECK(ctx);
-  scan_apply_kernel<<<(unsigned)ntiles, kThreads, 0, ctx->stream>>>(a, n, tile);
+  ME_TRY(ensure(ctx, (void **)&ctx->d_scan_tmp, &ctx->cap_scan_tmp, ntiles, sizeof(unsigned long long)));
+  ME_CUDA(ctx, cudaMemsetAsync(ctx->d_scan_tmp, 0, (size_t)ntiles * sizeof(unsigned long long), ctx->stream));
+  scan_kernel<<<(unsigned)ntiles, kThreads, 0, ctx->stream>>>(a, n, ctx->d_scan_tmp, stats);
   ME_LAUNCH_CHECK(ctx);
   return ME_OK;
 }
@@ -636,15 +665,9 @@ static int build_sparse(me_ctx *ctx, Cloud &c, const Lattice &L, long long *occu
   ME_LAUNCH_CHECK(ctx);
   unsigned long long *d_nt = (unsigned long long *)ctx->d_scratch + 8;
   ME_CUDA(ctx, cudaMemsetAsync(d_nt, 0, 3 * sizeof(unsigned long long), ctx->stream));
-  {
-    const long long ncomp = nseg * kSegCells;
-    const int ob = (int)std::min<long long>((ncomp + kThreads - 1) / kThreads, (long long)ctx->sm_count * 16);
-    occupancy_kernel<<<ob, kThreads, 0, ctx->stream>>>(c.d_cell_off, ncomp, d_nt + 1);
-    ME_LAUNCH_CHECK(ctx);
-  }
+  ME_TRY(exclusive_scan_inplace(ctx, c.d_cell_off, nseg * kSegCells + 1, d_nt + 1));      // [9] occupied cells, [10] fullest cell
   unsigned long long *h_nt = (unsigned long long *)ctx->h_pinned + 8;
   ME_CUDA(ctx, cudaMemcpyAsync(h_nt, d_nt, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
-  ME_TRY(exclusive_scan_inplace(ctx, c.d_cell_off, nseg * kSegCells + 1));
   ME_TRY(ensure(ctx, (void **)&c.d_sorted, &c.cap_sorted, n, sizeof(P4)));
   ME_TRY(ensure(ctx, (void **)&c.d_rel, &c.cap_rel, n, sizeof(float4)));
   sparse_gather_kernel<<<blocks, kThreads, 0, ctx->stream>>>(c.d_xyz, keys, vals, n, L, c.d_sorted, c.d_rel);
@@ -786,7 +809,7 @@ void slab_cut(const unsigned long long *planes_y, int n_planes_y, const unsigned
   if (best_axis) for (int r = 0; r <= W; ++r) bounds[r] = best_b[r];
 }
 
-// plan the owned voxel layers of every rank from the layer histograms of cloud c (histogram in c.d_cell_off + 1); the same
+// plan the owned voxel layers of every rank from the layer histograms of cloud c (histogram in c.d_cell_off); the same
 // arithmetic on the same (replicated) cloud on every rank gives the same plan
 static int plan_slabs(me_ctx *ctx, Cloud &c, const Lattice &L) {
   ctx->slab_planned = true;
@@ -795,9 +818,9 @@ static int plan_slabs(me_ctx *ctx, Cloud &c, const Lattice &L) {
   const int np = L.dims[1] + L.dims[2];
   ME_TRY(ensure_work(ctx, (size_t)np * sizeof(unsigned long long)));
   unsigned long long *d_pl = (unsigned long long *)ctx->d_work;
-  plane_count_kernel<<<std::min(L.dims[1], ctx->sm_count * 8), kThreads, 0, ctx->stream>>>(c.d_cell_off + 1, L.dims[0], L.dims[1], L.dims[2], 1, d_pl);
+  plane_count_kernel<<<std::min(L.dims[1], ctx->sm_count * 8), kThreads, 0, ctx->stream>>>(c.d_cell_off, L.dims[0], L.dims[1], L.dims[2], 1, d_pl);
   ME_LAUNCH_CHECK(ctx);
-  plane_count_kernel<<<std::min(L.dims[2], ctx->sm_count * 8), kThreads, 0, ctx->stream>>>(c.d_cell_off + 1, L.dims[0], L.dims[1], L.dims[2], 2, d_pl + L.dims[1]);
+  plane_count_kernel<<<std::min(L.dims[2], ctx->sm_count * 8), kThreads, 0, ctx->stream>>>(c.d_cell_off, L.dims[0], L.dims[1], L.dims[2], 2, d_pl + L.dims[1]);
   ME_LAUNCH_CHECK(ctx);
   std::vector<unsigned long long> h((size_t)np);
   ME_CUDA(ctx, cudaMemcpyAsync(h.data(), d_pl, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
@@ -858,6 +881,7 @@ int build_grid(me_ctx *ctx, int which, double solo_h) {
   // (occupied row segments only) instead of coarser cells.
   Lattice L;
   bool built = false;      // the sparse build lays the cloud out while planning
+  bool scanned = false;    // the dense table already holds the scan of the histogram (planning measured the occupancy)
   long long occupied = 0;
   if (solo) {
     double v; int m;
@@ -901,15 +925,19 @@ int build_grid(me_ctx *ctx, int which, double solo_h) {
       L = cand; have = true;
       h_used = h_target;
       ctx->spec_v = v; ctx->spec_m = m;
-      long long max_count = 0;
       if (L.sparse) { ME_TRY(build_sparse(ctx, c, L, &occupied)); built = true; }
-      else { built = false; ME_TRY(histogram(ctx, c, L)); }
+      else { built = false; scanned = false; ME_TRY(histogram(ctx, c, L)); }
       if (ctx->nn_cell_size > 0) break;   // caller fixed the cell size
       if (hit && L.sparse == pc.lat.sparse && L.m == pc.lat.m && L.v == pc.lat.v && L.dims[0] == pc.lat.dims[0] &&
           L.dims[1] == pc.lat.dims[1] && L.dims[2] == pc.lat.dims[2])
         break;                            // the remembered lattice: no need to measure the occupancy again
       hit = false;
-      if (!L.sparse) ME_TRY(occupancy(ctx, c, L, &occupied, &max_count));
+      if (!L.sparse) {
+        ME_TRY(scan_cells(ctx, c, L));
+        ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        scanned = true;
+        occupied = (long long)((unsigned long long *)ctx->h_pinned)[9];
+      }
       const double mean_occ = (double)c.n / (double)std::max<long long>(1, occupied);
       if (mean_occ <= 4.0 || iter == 3) break;
       // surface-like data: occupancy of occupied cells scales ~h^2; aim at ~2 points per occupied cell
@@ -940,6 +968,7 @@ int build_grid(me_ctx *ctx, int which, double solo_h) {
   c.ns = c.n;
   c.n_owned = c.n;
   if (!built && !solo && slab_wanted(ctx)) {
+    if (scanned) { ME_TRY(histogram(ctx, c, L)); scanned = false; }      // the slab cut and mask work on the counts
     if (!ctx->slab_planned) ME_TRY(plan_slabs(ctx, c, L));
     {
       PlanCache &pc = ctx->plan_cache[which];
@@ -954,7 +983,7 @@ int build_grid(me_ctx *ctx, int which, double solo_h) {
       unsigned long long *d_own = (unsigned long long *)ctx->d_scratch + 11;
       ME_CUDA(ctx, cudaMemsetAsync(d_own, 0, sizeof(unsigned long long), ctx->stream));
       const int mb = (int)std::min<long long>((L.ncells + kThreads - 1) / kThreads, (long long)ctx->sm_count * 16);
-      slab_mask_kernel<<<mb, kThreads, 0, ctx->stream>>>(c.d_cell_off + 1, L.ncells, L.dims[0], L.dims[1], c.sl_axis, c.sc_lo, c.sc_hi,
+      slab_mask_kernel<<<mb, kThreads, 0, ctx->stream>>>(c.d_cell_off, L.ncells, L.dims[0], L.dims[1], c.sl_axis, c.sc_lo, c.sc_hi,
                                                         c.so_lo, c.so_hi, d_own);
       ME_LAUNCH_CHECK(ctx);
       c.slab = true;
@@ -969,28 +998,15 @@ int build_grid(me_ctx *ctx, int which, double solo_h) {
     }
   }
   if (!built) {
-    // scratch slots: [9] occupied cells, [10] largest cell (bounds the run lengths of the sweeps)
-    unsigned long long *d_nt = (unsigned long long *)ctx->d_scratch + 8;
-    ME_CUDA(ctx, cudaMemsetAsync(d_nt, 0, 3 * sizeof(unsigned long long), ctx->stream));
-    {
-      const int blocks = (int)std::min<long long>((L.ncells + kThreads - 1) / kThreads, (long long)ctx->sm_count * 16);
-      occupancy_kernel<<<blocks, kThreads, 0, ctx->stream>>>(c.d_cell_off + 1, L.ncells, d_nt + 1);
-      ME_LAUNCH_CHECK(ctx);
-    }
-    unsigned long long *h_nt = (unsigned long long *)ctx->h_pinned + 8;
-    ME_CUDA(ctx, cudaMemcpyAsync(h_nt, d_nt, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
-
-    // exclusive scan of the histogram, in place
-    ME_TRY(exclusive_scan_inplace(ctx, c.d_cell_off + 1, L.ncells));
-
+    if (!scanned) ME_TRY(scan_cells(ctx, c, L));
     ME_TRY(ensure(ctx, (void **)&c.d_sorted, &c.cap_sorted, c.n, sizeof(P4)));
     ME_TRY(ensure(ctx, (void **)&c.d_rel, &c.cap_rel, c.n, sizeof(float4)));
     int blocks = (int)std::min<long long>((c.n + kThreads - 1) / kThreads, (long long)ctx->sm_count * 16);
-    scatter_kernel<<<blocks, kThreads, 0, ctx->stream>>>(c.d_xyz, c.n, c.d_cell_id, c.d_cell_off + 1, c.d_sorted, c.slab ? c.sl_axis : 0,
-                                                        L.dims[0], L.dims[1], c.sc_lo, c.sc_hi);
+    scatter_kernel<<<blocks, kThreads, 0, ctx->stream>>>(c.d_xyz, c.n, L, c.d_cell_off, ctx->d_rank, c.d_sorted,
+                                                        c.slab ? c.sl_axis : 0, c.sc_lo, c.sc_hi);
     ME_LAUNCH_CHECK(ctx);
     if (c.slab) {
-      // the scatter leaves off[] a CSR array: its last entry = the points laid out here
+      // the last entry of the CSR array = the points laid out here
       uint32_t *h_sl = (uint32_t *)((unsigned long long *)ctx->h_pinned + 16);
       unsigned long long *h_own = (unsigned long long *)ctx->h_pinned + 11;
       ME_CUDA(ctx, cudaMemcpyAsync(h_sl, c.d_cell_off + L.ncells, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1005,7 +1021,7 @@ int build_grid(me_ctx *ctx, int which, double solo_h) {
       ME_LAUNCH_CHECK(ctx);
     }
     ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    c.max_cell_count = (long long)h_nt[2];
+    c.max_cell_count = (long long)((unsigned long long *)ctx->h_pinned)[10];
   }
   ME_TRY(build_coarse(ctx, c));
   c.tiles_valid = false;
