@@ -119,6 +119,10 @@ class MapEvalB200:
     def estimate_normals(self, which, knn=20):
         """PointCloud::EstimateNormals(KDTreeSearchParamKNN(knn)); returns the (N, 3) normals in caller order."""
         self._check(self._L.me_estimate_normals(self._ctx, which, int(knn)))
+        return self.get_normals(which)
+
+    def get_normals(self, which):
+        """The normals of the held cloud, (N, 3) in the order of get_cloud; an error when the cloud has none."""
         out = np.empty((self.n[which], 3), np.float64)
         self._check(self._L.me_get_normals(self._ctx, which, out.ctypes.data_as(C.POINTER(C.c_double))))
         return out

@@ -440,7 +440,7 @@ int me_set_normals(me_ctx *ctx, int which, const double *normals_host, int64_t n
 int me_estimate_normals(me_ctx *ctx, int which, int32_t knn) {
   ME_ENTER(ctx);
   if (which != ME_CLOUD_EST && which != ME_CLOUD_GT) return fail(ctx, ME_ERR_INVALID, "bad cloud id");
-  return estimate_normals(ctx, which, knn, 0);
+  return estimate_normals(ctx, which, knn);
 }
 
 int me_get_normals(me_ctx *ctx, int which, double *normals_host) {

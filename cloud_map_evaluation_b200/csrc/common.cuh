@@ -112,8 +112,8 @@ struct Cloud {
   double *d_entropy_caller = nullptr;   // caller order, kept when the sweep ran on a solo lattice (which the next build replaces)
   long long cap_entropy_caller = 0;
   bool entropy_caller_valid = false;
-  double *d_normal = nullptr;           // caller order, 3 fp64 per point: normals (me_set_normals / me_estimate_normals); during
-  long long cap_normal = 0;             // generalized ICP the unit vector that carries the point's covariance (icp.cu)
+  double *d_normal = nullptr;           // caller order, 3 fp64 per point: normals (me_set_normals / me_estimate_normals, averaged
+  long long cap_normal = 0;             // by me_voxel_downsample); the working k-NN normals of generalized ICP when !normal_valid
   bool normal_valid = false;
 };
 
@@ -305,7 +305,7 @@ int voxel_finish_block(me_ctx *ctx, int scs_radius);
 int transform_cloud(me_ctx *ctx, int which, const double T[16]);
 int run_icp(me_ctx *ctx, int method, double max_dist, int max_iter, double rel_fitness, double rel_rmse, const double T_init[16],
             me_icp_result *out);
-int estimate_normals(me_ctx *ctx, int which, int knn, int gicp);
+int estimate_normals(me_ctx *ctx, int which, int knn);
 void invalidate_cloud(Cloud &c);      // the cloud's coordinates changed: bbox, lattice, NN and entropy results are stale
 int run_awd_rows(me_ctx *ctx, const double *rows27, int64_t n_rows, double voxel_size, int scs_radius, double *w_out,
                  me_awd_result *out);

@@ -5,9 +5,12 @@
 //   voxel_min_bound = GetMinBound() - 0.5 * voxel_size
 //   voxel index     = int(floor((p - voxel_min_bound) / voxel_size))   per axis, fp64, IEEE division
 //   output point    = (sum of the voxel's points, accumulated in INPUT order) / double(count)
+//   output normal   = (sum of the voxel's normals without a NaN component, INPUT order) / double(count), not re-normalised;
+//                     only when the cloud holds normals (me_set_normals / me_estimate_normals), otherwise there are none
 // Open3D emits the voxels in std::unordered_map iteration order (implementation-defined); here they come out in
-// increasing (ix, iy, iz).  The SET of output points is bit-identical to the CPU path: the 64-bit voxel keys are sorted
-// with a STABLE radix sort (points of a voxel stay in input order) and each voxel is summed sequentially by one thread.
+// increasing (ix, iy, iz).  The SET of output points (and of point-normal pairs) is bit-identical to the CPU path: the
+// 64-bit voxel keys are sorted with a STABLE radix sort (points of a voxel stay in input order) and each voxel is summed
+// sequentially by one thread.
 //
 // The sort is the library's own LSD radix sort (sort.cu); key building, run detection and the ordered sums follow.
 #include "common.cuh"
@@ -45,23 +48,32 @@ __global__ void __launch_bounds__(kThreads) vds_head_kernel(const unsigned long 
     head[i] = (i < n && (i == 0 || key[i] != key[i - 1])) ? 1u : 0u;
 }
 
-// one thread per voxel start: sequential sum in input order (the sort is stable), then the division by the count
+// one thread per voxel start: sequential sum in input order (the sort is stable), then the division by the count.
+// kNormals: AccumulatedPoint's normal sum in the same walk — a normal is added only when none of its components is NaN,
+// the division is by the count of ALL the voxel's points, and the result is not re-normalised (GetAverageNormal)
+template <bool kNormals>
 __global__ void __launch_bounds__(kThreads) vds_mean_kernel(const double *__restrict__ xyz, const unsigned long long *__restrict__ key,
                                                             const uint32_t *__restrict__ val, const uint32_t *__restrict__ pos,
-                                                            long long n, double *__restrict__ out) {
+                                                            long long n, double *__restrict__ out, const double *__restrict__ nrm,
+                                                            double *__restrict__ out_nrm) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const uint32_t p = pos[i];
     if (pos[i + 1] == p) continue;                    // not the first point of its voxel
     const unsigned long long k = key[i];
-    double sx = 0.0, sy = 0.0, sz = 0.0;
+    double sx = 0.0, sy = 0.0, sz = 0.0, nx = 0.0, ny = 0.0, nz = 0.0;
     long long cnt = 0;
     for (long long j = i; j < n && key[j] == k; ++j) {
       const long long o = val[j];
       sx = __dadd_rn(sx, __ldg(xyz + 3 * o)); sy = __dadd_rn(sy, __ldg(xyz + 3 * o + 1)); sz = __dadd_rn(sz, __ldg(xyz + 3 * o + 2));
+      if (kNormals) {
+        const double a = __ldg(nrm + 3 * o), b = __ldg(nrm + 3 * o + 1), c = __ldg(nrm + 3 * o + 2);
+        if (!isnan(a) && !isnan(b) && !isnan(c)) { nx = __dadd_rn(nx, a); ny = __dadd_rn(ny, b); nz = __dadd_rn(nz, c); }
+      }
       ++cnt;
     }
     const double c = (double)cnt;
     out[3ll * p] = __ddiv_rn(sx, c); out[3ll * p + 1] = __ddiv_rn(sy, c); out[3ll * p + 2] = __ddiv_rn(sz, c);
+    if (kNormals) { out_nrm[3ll * p] = __ddiv_rn(nx, c); out_nrm[3ll * p + 1] = __ddiv_rn(ny, c); out_nrm[3ll * p + 2] = __ddiv_rn(nz, c); }
   }
 }
 
@@ -115,14 +127,23 @@ int voxel_downsample(me_ctx *ctx, int which, double voxel_size, int64_t *n_out) 
   ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (h[0] != 0) return fail(ctx, ME_ERR_RANGE, "voxel_size is too small for the extent of the cloud (more than 2^21 voxels per axis)");
   const long long nv = (long long)h[1];
-  double *out = nullptr;
-  long long cap_out = 0;
+  double *out = nullptr, *out_nrm = nullptr;
+  long long cap_out = 0, cap_nrm = 0;
   ME_TRY(ensure(ctx, (void **)&out, &cap_out, 3 * nv, sizeof(double)));
-  vds_mean_kernel<<<blocks, kThreads, 0, ctx->stream>>>(c.d_xyz, key1, val1, pos, n, out);
+  if (c.normal_valid) {
+    if (ensure(ctx, (void **)&out_nrm, &cap_nrm, 3 * nv, sizeof(double)) != ME_OK) { cudaFree(out); return ME_ERR_NOMEM; }
+    vds_mean_kernel<true><<<blocks, kThreads, 0, ctx->stream>>>(c.d_xyz, key1, val1, pos, n, out, c.d_normal, out_nrm);
+  } else {
+    vds_mean_kernel<false><<<blocks, kThreads, 0, ctx->stream>>>(c.d_xyz, key1, val1, pos, n, out, nullptr, nullptr);
+  }
   ME_LAUNCH_CHECK(ctx);
-  ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // the old buffer may be released (or handed back) now
+  ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // the old buffers may be released (or handed back) now
   if (c.owned && c.d_xyz) cudaFree(c.d_xyz);
   c.d_xyz = out; c.cap_xyz = cap_out; c.owned = true; c.n = nv;
+  if (c.normal_valid) {                               // the normals follow the points: averaged, in the output order
+    cudaFree(c.d_normal);
+    c.d_normal = out_nrm; c.cap_normal = cap_nrm;
+  }
   c.grid_valid = false; c.bbox_valid = false; c.nn_valid = false; c.entropy_valid = false; c.entropy_caller_valid = false;
   if (n_out) *n_out = nv;
   return ME_OK;

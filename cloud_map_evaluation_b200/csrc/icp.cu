@@ -13,11 +13,14 @@
 //   point-to-point:  Eigen::umeyama without scaling — icp_accum_kernel reduces count, sum p, sum q, sum q p^T, sum d2
 //                    (17 doubles); the 3x3 algebra runs on the host.
 //   point-to-plane:  r = (vs - vt) . nt, J = [vs x nt, nt]; needs target normals (me_set_normals / me_estimate_normals).
-//   generalized:     InitializePointCloudForGeneralizedICP = EstimateNormals(KNN 20) on both clouds (knn_normals_kernel:
-//                    exact k-NN by ring expansion over the lattice, covariance, Eberly's robust 3x3 eigenvector =
-//                    Open3D's FastEigen3x3), covariance_i = Rx diag(1e-3, 1, 1) Rx^T = I + (eps - 1) n n^T with n := e1
-//                    where Open3D's GetRotationFromE1ToX falls back to the identity (n.x < -0.99, sic) — so a unit vector
-//                    per point carries the covariance, and PointCloud::Transform's R C R^T is a rotation of that vector;
+//   generalized:     InitializePointCloudForGeneralizedICP, per cloud: the cloud's normals when it has them (me_set_normals,
+//                    me_estimate_normals, averaged by me_voxel_downsample), else EstimateNormals(KNN 20) into a working
+//                    buffer (knn_normals_kernel: exact k-NN by ring expansion over the lattice, covariance, Eberly's robust
+//                    3x3 eigenvector = Open3D's FastEigen3x3); covariance_i = Rx diag(1e-3, 1, 1) Rx^T with
+//                    Rx = GetRotationFromE1ToX(n_i), n_i as given (not normalised; Rx = I when n.x < -0.99, sic), built per
+//                    correspondence from the 3 doubles of the normal (gicp_cov); PointCloud::Transform's R C R^T of the
+//                    source is R_T C(n_i) R_T^T with R_T the rotation block of the accumulated transformation (T_init
+//                    included): the source normals themselves stay as handed in during the loop.
 //                    ComputeTransformation: M = Cs + Ct, J = M^-1/2 [-skew(vs) | I], r = M^-1/2 d, i.e. the 6x6 normal
 //                    equations sum A^T M^-1 A, sum A^T M^-1 d, reduced on the device (icp_ne_accum_kernel, 28 doubles);
 //                    the 6x6 solve and TransformVector6dToMatrix4d run on the host.
@@ -254,13 +257,12 @@ __device__ void fast_eigen3x3_normal(const double cov[9], double nrm[3]) {
 // included), their covariance, the eigenvector of its smallest eigenvalue.  One thread per point; the k best (d2,
 // position) pairs sit sorted in shared memory ([slot][thread]); the lattice is searched shell by shell (Chebyshev rings)
 // until the k-th distance beats the distance to the border of the searched block.  Ties go to the smaller caller index.
-// gicp != 0: store e1 where Open3D's GetRotationFromE1ToX falls back to the identity (n.x < -0.99).
 // ---------------------------------------------------------------------------------------------------------------
 static constexpr int kKnnThreads = 128;
 
 __global__ void __launch_bounds__(kKnnThreads)
 knn_normals_kernel(const P4 *__restrict__ S, long long n, CellIndex I, Lattice L, CoarseGrid CG, int k, double slack,
-                   int gicp, double *__restrict__ normals) {
+                   double *__restrict__ normals) {
   extern __shared__ __align__(16) unsigned char knn_smem[];
   double *dk = reinterpret_cast<double *>(knn_smem) + threadIdx.x;                                     // dk[t * kKnnThreads]
   uint32_t *ik = reinterpret_cast<uint32_t *>(knn_smem + (size_t)k * kKnnThreads * sizeof(double)) + threadIdx.x;
@@ -384,13 +386,12 @@ knn_normals_kernel(const P4 *__restrict__ S, long long n, CellIndex I, Lattice L
     double nr[3];
     fast_eigen3x3_normal(cov, nr);
     if (sqrt(nr[0] * nr[0] + nr[1] * nr[1] + nr[2] * nr[2]) == 0.0) { nr[0] = 0; nr[1] = 0; nr[2] = 1; }
-    if (gicp && nr[0] < -0.99) { nr[0] = 1; nr[1] = 0; nr[2] = 0; }
     const long long o = orig_of(q.idx);
     normals[3 * o] = nr[0]; normals[3 * o + 1] = nr[1]; normals[3 * o + 2] = nr[2];
   }
 }
 
-int estimate_normals(me_ctx *ctx, int which, int knn, int gicp) {
+int estimate_normals(me_ctx *ctx, int which, int knn) {
   Cloud &c = ctx->cloud[which];
   if (c.n <= 0) return fail(ctx, ME_ERR_EMPTY, "cloud is empty");
   if (knn < 1 || knn > 64) return fail(ctx, ME_ERR_INVALID, "knn must be in 1..64");
@@ -405,7 +406,7 @@ int estimate_normals(me_ctx *ctx, int which, int knn, int gicp) {
   for (int a = 0; a < 3; ++a) maxabs = std::max(maxabs, std::max(std::fabs(c.bbox_min[a]), std::fabs(c.bbox_max[a])));
   const double slack = 1e-9 * c.lat.h + 4e-14 * maxabs;
   const int blocks = (int)std::min<long long>((c.n + kKnnThreads - 1) / kKnnThreads, (long long)ctx->sm_count * 32);
-  knn_normals_kernel<<<blocks, kKnnThreads, smem, ctx->stream>>>(c.d_sorted, c.n, index_of(c), c.lat, coarse_of(c), k, slack, gicp, c.d_normal);
+  knn_normals_kernel<<<blocks, kKnnThreads, smem, ctx->stream>>>(c.d_sorted, c.n, index_of(c), c.lat, coarse_of(c), k, slack, c.d_normal);
   ME_LAUNCH_CHECK(ctx);
   c.normal_valid = true;
   return ME_OK;
@@ -419,11 +420,39 @@ struct NeAcc {
   unsigned long long n;
   double v[28];
 };
+struct Mat9 { double r[9]; };
+
+// GetRotationFromE1ToX(x) diag(eps, 1, 1) GetRotationFromE1ToX(x)^T with x as given (Open3D does not normalise it):
+// Rx = I + [v]x + [v]x^2 / (1 + c), v = e1 x x = (0, -x2, x1), c = x0, written out; Rx = I when c < -0.99.  When R is
+// given, the covariance is rotated: (R Rx) diag(eps, 1, 1) (R Rx)^T.  C: upper triangle xx xy xz yy yz zz.
+__device__ __forceinline__ void gicp_cov(const double x[3], double eps, const double *R, double C[6]) {
+  double Q[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0};
+  if (!(x[0] < -0.99)) {
+    const double f = 1.0 / (1.0 + x[0]), fxy = f * x[1] * x[2];
+    Q[0] = 1.0 - f * (x[1] * x[1] + x[2] * x[2]); Q[1] = -x[1];                 Q[2] = -x[2];
+    Q[3] = x[1];                                  Q[4] = 1.0 - f * x[1] * x[1]; Q[5] = -fxy;
+    Q[6] = x[2];                                  Q[7] = -fxy;                  Q[8] = 1.0 - f * x[2] * x[2];
+  }
+  if (R) {
+    double P[9];
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+      for (int col = 0; col < 3; ++col) P[r * 3 + col] = R[r * 3] * Q[col] + R[r * 3 + 1] * Q[3 + col] + R[r * 3 + 2] * Q[6 + col];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) Q[k] = P[k];
+  }
+  int t = 0;
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = a; b < 3; ++b) C[t++] = eps * Q[a * 3] * Q[b * 3] + Q[a * 3 + 1] * Q[b * 3 + 1] + Q[a * 3 + 2] * Q[b * 3 + 2];
+}
 
 __global__ void __launch_bounds__(kThreads)
 icp_ne_accum_kernel(const P4 *__restrict__ Q, long long n, const int32_t *__restrict__ nn_idx, const double *__restrict__ nn_d2,
                     const double *__restrict__ gt_xyz, const double *__restrict__ gt_nrm, const double *__restrict__ est_nrm,
-                    double r2, double eps, int method, NeAcc *__restrict__ acc) {
+                    Mat9 Rs, double r2, double eps, int method, NeAcc *__restrict__ acc) {
   double v[28];
 #pragma unroll
   for (int k = 0; k < 28; ++k) v[k] = 0.0;
@@ -454,10 +483,12 @@ icp_ne_accum_kernel(const P4 *__restrict__ Q, long long n, const int32_t *__rest
     } else {
       const long long o = orig_of(p.idx);
       const double ns[3] = {__ldg(est_nrm + 3 * o), __ldg(est_nrm + 3 * o + 1), __ldg(est_nrm + 3 * o + 2)};
-      // M = Cs + Ct = 2 I + (eps - 1)(ns ns^T + nt nt^T); B = M^-1 (symmetric, by cofactors)
-      const double w = eps - 1.0;
-      const double m00 = 2.0 + w * (ns[0] * ns[0] + nt[0] * nt[0]), m01 = w * (ns[0] * ns[1] + nt[0] * nt[1]), m02 = w * (ns[0] * ns[2] + nt[0] * nt[2]);
-      const double m11 = 2.0 + w * (ns[1] * ns[1] + nt[1] * nt[1]), m12 = w * (ns[1] * ns[2] + nt[1] * nt[2]), m22 = 2.0 + w * (ns[2] * ns[2] + nt[2] * nt[2]);
+      // M = Cs + Ct with Cs = Rs C(ns) Rs^T; B = M^-1 (symmetric, by cofactors)
+      double cs[6], ct[6];
+      gicp_cov(ns, eps, Rs.r, cs);
+      gicp_cov(nt, eps, nullptr, ct);
+      const double m00 = cs[0] + ct[0], m01 = cs[1] + ct[1], m02 = cs[2] + ct[2];
+      const double m11 = cs[3] + ct[3], m12 = cs[4] + ct[4], m22 = cs[5] + ct[5];
       const double c00 = m11 * m22 - m12 * m12, c01 = m02 * m12 - m01 * m22, c02 = m01 * m12 - m02 * m11;
       const double c11 = m00 * m22 - m02 * m02, c12 = m01 * m02 - m00 * m12, c22 = m00 * m11 - m01 * m01;
       const double idet = 1.0 / (m00 * c00 + m01 * c01 + m02 * c02);
@@ -552,23 +583,30 @@ int run_icp(me_ctx *ctx, int method, double max_dist, int max_iter, double rel_f
                                      "PointCloud (me_set_normals / me_estimate_normals on the ground-truth cloud)");
   ME_TRY(wait_upload(ctx, ME_CLOUD_EST));
   const double eps = 1e-3;      // TransformationEstimationForGeneralizedICP() default epsilon
+  const bool est_had_normals = E.normal_valid, gt_had_normals = G.normal_valid;
+  int rc = ME_OK;
   if (method == ME_ICP_GENERALIZED) {
-    // InitializePointCloudForGeneralizedICP on both clouds (before the initial transform, as Open3D does)
-    ME_TRY(build_both(ctx));
-    ME_TRY(estimate_normals(ctx, ME_CLOUD_EST, 20, 1));
-    ME_TRY(estimate_normals(ctx, ME_CLOUD_GT, 20, 1));
+    // InitializePointCloudForGeneralizedICP per cloud (before the initial transform, as Open3D does): the cloud's own
+    // normals, else EstimateNormals(KNN 20) into the cloud's normal buffer as a working copy that stays invalid afterwards
+    if (!est_had_normals || !gt_had_normals) rc = build_both(ctx);
+    if (rc == ME_OK && !est_had_normals) rc = estimate_normals(ctx, ME_CLOUD_EST, 20);
+    if (rc == ME_OK && !gt_had_normals) rc = estimate_normals(ctx, ME_CLOUD_GT, 20);
+    E.normal_valid = est_had_normals; G.normal_valid = gt_had_normals;
+    if (rc != ME_OK) return rc;
   }
   // the original cloud: RegistrationICP iterates on a copy, the caller's cloud is transformed once at the end (:1392)
   double *orig = nullptr;
   long long cap_orig = 0;
   ME_TRY(ensure(ctx, (void **)&orig, &cap_orig, 3 * E.n, sizeof(double)));
-  int rc = ME_OK;
+  // the estimated cloud's normals stay as they came in while the copy moves (generalized ICP rotates the covariances
+  // with the accumulated R instead); the final transformation rotates them once, as PointCloud::Transform does
+  E.normal_valid = false;
   if (cudaMemcpyAsync(orig, E.d_xyz, (size_t)E.n * 3 * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess)
     rc = fail(ctx, ME_ERR_CUDA, "copy of the estimated cloud failed");
 
   double T[16];
   std::memcpy(T, T_init, sizeof(T));
-  if (rc == ME_OK) rc = transform_cloud(ctx, ME_CLOUD_EST, T);      // rotates the (effective) normals along
+  if (rc == ME_OK) rc = transform_cloud(ctx, ME_CLOUD_EST, T);
   me_nn_params p;
   std::memset(&p, 0, sizeof(p));
   p.icp_max_distance = max_dist;
@@ -600,9 +638,12 @@ int run_icp(me_ctx *ctx, int method, double max_dist, int max_iter, double rel_f
       res = *h_acc;
       n_corr = res.n; err2 = res.err2;
     } else {
+      Mat9 R;      // rotation block of the accumulated transformation: the source covariances are R C(n) R^T
+      for (int r = 0; r < 3; ++r)
+        for (int col = 0; col < 3; ++col) R.r[r * 3 + col] = T[r * 4 + col];
       ME_CUDA(ctx, cudaMemsetAsync(d_ne, 0, sizeof(NeAcc), ctx->stream));
       icp_ne_accum_kernel<<<blocks, kThreads, 0, ctx->stream>>>(E.d_sorted, E.n, E.d_nn_idx, E.d_nn_d2, G.d_xyz, G.d_normal,
-                                                               E.d_normal, max_dist * max_dist, eps, method, d_ne);
+                                                               E.d_normal, R, max_dist * max_dist, eps, method, d_ne);
       ME_LAUNCH_CHECK(ctx);
       ME_CUDA(ctx, cudaMemcpyAsync(h_ne, d_ne, sizeof(NeAcc), cudaMemcpyDeviceToHost, ctx->stream));
       ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -640,17 +681,16 @@ int run_icp(me_ctx *ctx, int method, double max_dist, int max_iter, double rel_f
     if (rc != ME_OK) break;
     if (std::fabs(f0 - fitness) < rel_fitness && std::fabs(r0 - rmse) < rel_rmse) { ++it; converged = 1; break; }
   }
-  // est := Transform(original, T) (map_eval.cpp:1392).  On an error the original cloud comes back untouched; either way
-  // every derived structure of the estimated cloud is stale now.
+  // est := Transform(original, T) (map_eval.cpp:1392), normals handed in included.  On an error the original cloud (and
+  // its normals) come back untouched; either way every derived structure of the estimated cloud is stale now.
   int rc2 = ME_OK;
   if (cudaMemcpyAsync(E.d_xyz, orig, (size_t)E.n * 3 * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess)
     rc2 = fail(ctx, ME_ERR_CUDA, "restoring the estimated cloud failed");
   invalidate_cloud(E);
-  E.normal_valid = false;                         // the working normals of generalized ICP do not outlive the call
+  E.normal_valid = est_had_normals;               // the working normals of generalized ICP do not outlive the call
   if (rc == ME_OK && rc2 == ME_OK) rc2 = transform_cloud(ctx, ME_CLOUD_EST, T);
   if (cudaStreamSynchronize(ctx->stream) != cudaSuccess && rc2 == ME_OK) rc2 = fail(ctx, ME_ERR_CUDA, "synchronize after ICP failed");
   cudaFree(orig);
-  if (method == ME_ICP_GENERALIZED) G.normal_valid = false;      // they hold the e1 substitution: not plain normals
   if (rc != ME_OK) return rc;
   if (rc2 != ME_OK) return rc2;
   std::memcpy(out->transformation, T, sizeof(T));

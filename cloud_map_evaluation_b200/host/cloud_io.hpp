@@ -4,8 +4,9 @@
 // ReadPointCloudOption("auto", remove_nan = true, remove_infinite = true, print_progress = true), map_eval.cpp:6-21),
 // which is not available here.  Only the x/y/z fields are consumed by the metric path; points with a non-finite
 // coordinate are dropped, as that option does.  Coordinates are widened to double — the type of Open3D's
-// PointCloud::points_.  Normals (PCD normal_x / normal_y / normal_z, PLY nx / ny / nz) are read on request: point-to-plane ICP
-// (registration_methods: 1) needs them on the ground-truth cloud, as Open3D's PointCloud::normals_.
+// PointCloud::points_.  Normals (PCD normal_x / normal_y / normal_z, PLY nx / ny / nz) are read on request, as Open3D's
+// PointCloud::normals_: point-to-plane ICP (registration_methods: 1) needs them on the ground-truth cloud, generalized ICP
+// (2) uses those of either cloud.
 #pragma once
 #include <cmath>
 #include <cstdint>

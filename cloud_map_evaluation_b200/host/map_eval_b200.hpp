@@ -17,9 +17,11 @@
 //   performRegistration / performICPRegistration :191-237, 1366-1394   performRegistration -> me_icp (§8f N2: point-to-point,
 //                                                         point-to-plane and generalized ICP) + calculateMetrics(reg)
 //   rendered clouds                  :485-499, 568-736    render.hpp (§8f N3): entropy maps, raw / inlier NN-distance maps
-// Limits of this driver: point-to-plane ICP (registration_methods: 1) needs normals in the ground-truth FILE, as in the
-// reference (Open3D raises without them), and no down-sampling (VoxelDownSample's normal averaging is not built);
-// validate() rejects such a configuration before anything is written.
+// Normals: on path B (evaluate_using_initial: false) with point-to-plane or generalized ICP (registration_methods: 1 / 2)
+// the normals that either FILE carries are read and handed to every context before VoxelDownSample, which averages them
+// as Open3D does; generalized ICP builds a cloud's covariances from them and estimates normals (KNN 20) only for a cloud
+// without any.  Point-to-plane ICP needs them in the ground-truth file, as in the reference (Open3D raises without them).
+// Path A and point-to-point ICP never read normals.
 #pragma once
 #include <algorithm>
 #include <chrono>
@@ -191,12 +193,6 @@ class MapEvalB200 {
              "; 0 = point-to-point, 1 = point-to-plane, 2 = generalized ICP, map_eval.cpp:1368-1390)";
       return false;
     }
-    if (p.evaluation_method_ == 1 && p.downsample_size > 0) {
-      *why = "registration_methods: 1 (point-to-plane ICP) takes the target normals from the ground-truth file; with "
-             "downsample_size > 0 they would have to be averaged per voxel (Open3D VoxelDownSample), which this driver does "
-             "not do: set downsample_size: 0, or use registration_methods: 0 / 2";
-      return false;
-    }
     return true;
   }
 
@@ -258,7 +254,7 @@ class MapEvalB200 {
   GpuGroup gpus_;            // one context per GPU; rank r evaluates the r-th shard of every sweep's query range
   me_ctx *ctx_ = nullptr;    // = gpus_.ctx(0): the voxel stage and the single-GPU calls
   std::vector<double> map_3d_, gt_3d_;   // N x 3 fp64, the layout of open3d PointCloud::points_ (as loaded)
-  std::vector<double> gt_normals_;       // PointCloud::normals_ of the ground truth (point-to-plane ICP only)
+  std::vector<double> map_normals_, gt_normals_;   // PointCloud::normals_ as loaded (path B, point-to-plane / generalized ICP)
   int64_t n_est_ = 0, n_gt_ = 0;         // point counts after VoxelDownSample (the clouds the metrics see)
   double t1, t2, t3, t4, t5, t6, t7, t_fcd = 0.0, t_acc = 0.0;
   double t_vmd = 0.0, t_v = 0.0, t_cdf = 0.0, t_scs = 0.0;
@@ -273,18 +269,20 @@ inline int MapEvalB200::process() {
     std::cerr << "ERROR: " << err << std::endl;
     return -1;
   }
-  // point-to-plane ICP: Open3D needs normals on the target cloud; they can only come from the ground-truth file
-  std::vector<double> *want_normals = (!param_.evaluate_using_initial_ && param_.evaluation_method_ == 1) ? &gt_normals_ : nullptr;
+  // point-to-plane ICP needs normals on the target cloud, which can only come from the ground-truth file; generalized ICP
+  // uses the normals of either file when it carries them (InitializePointCloudForGeneralizedICP)
+  const bool load_normals = !param_.evaluate_using_initial_ && (param_.evaluation_method_ == 1 || param_.evaluation_method_ == 2);
   std::string file_extension = param_.map_gt_path_.substr(param_.map_gt_path_.find_last_of(".") + 1);
   bool gt_ok = false;
-  if (file_extension == "pcd") gt_ok = cloud_io::read_pcd(param_.map_gt_path_, gt_3d_, &err, want_normals);
-  else if (file_extension == "ply") gt_ok = cloud_io::read_ply(param_.map_gt_path_, gt_3d_, &err, want_normals);
+  if (file_extension == "pcd") gt_ok = cloud_io::read_pcd(param_.map_gt_path_, gt_3d_, &err, load_normals ? &gt_normals_ : nullptr);
+  else if (file_extension == "ply") gt_ok = cloud_io::read_ply(param_.map_gt_path_, gt_3d_, &err, load_normals ? &gt_normals_ : nullptr);
   else {
     std::cerr << "ERROR: Unsupported ground truth file format: " << param_.map_gt_path_ << std::endl;
     return -1;
   }
   if (!gt_ok && param_.enable_debug) std::cerr << "WARNING: " << err << std::endl;   // the reference ignores this return value
-  bool success = cloud_io::read_pcd(param_.evaluation_map_pcd_path_ + param_.pcd_file_name_, map_3d_, &err);
+  bool success = cloud_io::read_pcd(param_.evaluation_map_pcd_path_ + param_.pcd_file_name_, map_3d_, &err,
+                                    load_normals ? &map_normals_ : nullptr);
   if (param_.enable_debug)
     std::cout << "INFO: Loading map point cloud from: " << param_.evaluation_map_pcd_path_ + param_.pcd_file_name_ << std::endl;
   if (!success) {
@@ -295,7 +293,7 @@ inline int MapEvalB200::process() {
     std::cerr << "ERROR: One or both point clouds are empty!" << std::endl;
     return -1;
   }
-  if (want_normals && gt_normals_.size() != gt_3d_.size()) {
+  if (load_normals && param_.evaluation_method_ == 1 && gt_normals_.size() != gt_3d_.size()) {
     std::cerr << "ERROR: TransformationEstimationPointToPlane requires pre-computed normal vectors for the target PointCloud: "
               << param_.map_gt_path_ << " carries none (registration_methods: 1)." << std::endl;
     return -1;
@@ -305,10 +303,15 @@ inline int MapEvalB200::process() {
   if (gpus_.size() > 1) std::cout << "INFO: sharding the sweeps over " << gpus_.size() << " GPUs (NCCL all-reduce of the accumulators)" << std::endl;
   // every GPU holds both clouds (the lattices are replicated); VoxelDownSample (map_eval.cpp:38-39) runs on each of them.
   // The reference calls it unconditionally (Open3D raises for voxel_size <= 0); a non-positive value skips the step here.
+  // Normals loaded from a file go with their cloud, so that VoxelDownSample averages them.
   std::vector<int64_t> ne(gpus_.size(), (int64_t)(map_3d_.size() / 3)), ng(gpus_.size(), (int64_t)(gt_3d_.size() / 3));
+  const bool map_has_normals = !map_normals_.empty() && map_normals_.size() == map_3d_.size();
+  const bool gt_has_normals = !gt_normals_.empty() && gt_normals_.size() == gt_3d_.size();
   if (gpus_.for_each([&](int r, me_ctx *c) {
         int rc = me_set_cloud(c, ME_CLOUD_EST, map_3d_.data(), (int64_t)(map_3d_.size() / 3));
         if (rc == ME_OK) rc = me_set_cloud(c, ME_CLOUD_GT, gt_3d_.data(), (int64_t)(gt_3d_.size() / 3));
+        if (rc == ME_OK && map_has_normals) rc = me_set_normals(c, ME_CLOUD_EST, map_normals_.data(), (int64_t)(map_normals_.size() / 3));
+        if (rc == ME_OK && gt_has_normals) rc = me_set_normals(c, ME_CLOUD_GT, gt_normals_.data(), (int64_t)(gt_normals_.size() / 3));
         if (rc == ME_OK && param_.downsample_size > 0) {
           rc = me_voxel_downsample(c, ME_CLOUD_EST, param_.downsample_size, &ne[r]);
           if (rc == ME_OK) rc = me_voxel_downsample(c, ME_CLOUD_GT, param_.downsample_size, &ng[r]);
@@ -486,11 +489,9 @@ inline int MapEvalB200::performRegistration() {
   // ICP needs all correspondences on one GPU: run it on a single-shard context, then hand every GPU the aligned cloud
   me_icp_result reg{};
   me_set_shard(ctx_, 0, 1);
-  int rc = ME_OK;
-  if (param_.evaluation_method_ == ME_ICP_POINT_TO_PLANE)
-    rc = me_set_normals(ctx_, ME_CLOUD_GT, gt_normals_.data(), (int64_t)(gt_normals_.size() / 3));
-  // performICPRegistration (:1366-1394): ICPConvergenceCriteria() = {1e-6, 1e-6, 30}
-  if (rc == ME_OK) rc = me_icp(ctx_, param_.evaluation_method_, param_.icp_max_distance_, 30, 1e-6, 1e-6, param_.initial_matrix_, &reg);
+  // performICPRegistration (:1366-1394): ICPConvergenceCriteria() = {1e-6, 1e-6, 30}; the normals loaded with the
+  // clouds (down-sampled along with them) are already on the context
+  const int rc = me_icp(ctx_, param_.evaluation_method_, param_.icp_max_distance_, 30, 1e-6, 1e-6, param_.initial_matrix_, &reg);
   me_set_shard(ctx_, 0, gpus_.size());
   if (rc != ME_OK) return fail("me_icp");
   t4 = tic_toc.toc();

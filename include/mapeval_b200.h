@@ -218,7 +218,9 @@ ME_API int  me_transform(me_ctx *ctx, int which, const double T[16]);
  * open3d::geometry::PointCloud::VoxelDownSample: voxel index floor((p - (min_bound - s/2)) / s), output = mean of the
  * voxel's points accumulated in input order).  The cloud held by the context is replaced by its down-sampled version;
  * *n_out (nullable) receives the new point count.  The output points are bit-identical to the CPU path as a set; they
- * are ordered by increasing voxel index (Open3D: std::unordered_map iteration order, implementation-defined). */
+ * are ordered by increasing voxel index (Open3D: std::unordered_map iteration order, implementation-defined).  A cloud
+ * that holds normals keeps them: per voxel the sum, in input order, of the normals without a NaN component, divided by
+ * the voxel's point count and not re-normalised (Open3D AccumulatedPoint::GetAverageNormal), in the output order. */
 ME_API int  me_voxel_downsample(me_ctx *ctx, int which, double voxel_size, int64_t *n_out);
 /* the cloud currently held by the context (after me_transform / me_voxel_downsample), caller order, N x 3 fp64.
  * xyz_host == NULL: size query only (*n).  capacity_points < N is an error. */
@@ -234,8 +236,11 @@ ME_API int  me_icp_point_to_point(me_ctx *ctx, double max_correspondence_distanc
  * (ME_ICP_*).  ME_ICP_POINT_TO_PLANE = RegistrationICP with TransformationEstimationPointToPlane: the ground-truth cloud
  * needs normals (me_set_normals, e.g. from a PCD that carries them, or me_estimate_normals) — without them the call fails
  * like Open3D does.  ME_ICP_GENERALIZED = RegistrationGeneralizedICP with TransformationEstimationForGeneralizedICP()
- * (epsilon 1e-3): per-point covariances from EstimateNormals(KNN 20) on both clouds, computed inside.  Same post-condition
- * as me_icp_point_to_point.  Normals handed in or estimated before the call do not survive ME_ICP_GENERALIZED. */
+ * (epsilon 1e-3): per-point covariances Rx diag(eps, 1, 1) Rx^T, Rx = GetRotationFromE1ToX(normal) of the normal as held
+ * (not normalised), as InitializePointCloudForGeneralizedICP builds them — from the cloud's own normals when it has them
+ * (me_set_normals, me_estimate_normals, averaged by me_voxel_downsample), else from EstimateNormals(KNN 20) computed
+ * inside, which do not outlive the call (the cloud still has no normals afterwards).  Same post-condition as
+ * me_icp_point_to_point; normals the estimated cloud held are rotated by the result, the ground truth's are unchanged. */
 ME_API int  me_icp(me_ctx *ctx, int32_t method, double max_correspondence_distance, int32_t max_iteration,
                    double relative_fitness, double relative_rmse, const double T_init[16], me_icp_result *out);
 /* normals of a cloud held by the context, caller order, N x 3 fp64 (open3d PointCloud::normals_): upload / estimate as
