@@ -31,6 +31,39 @@ ME_ICP_POINT_TO_POINT = 0
 ME_ICP_POINT_TO_PLANE = 1
 ME_ICP_GENERALIZED = 2
 
+# enum me_kernel_bit: bit (1 << value) of the me_kernel_trace mask
+ME_KBIT_NN_ROWS_DENSE = 0
+ME_KBIT_NN_ROWS_SPARSE = 1
+ME_KBIT_NN_FLAT = 2
+ME_KBIT_NN_TILE = 3
+ME_KBIT_NN_FAR = 4
+ME_KBIT_NN_FAR_COARSE = 5
+ME_KBIT_NN_BRUTE = 6
+ME_KBIT_MME_FLAT1_DENSE = 7
+ME_KBIT_MME_FLAT2_DENSE = 8
+ME_KBIT_MME_FLAT3_DENSE = 9
+ME_KBIT_MME_FLAT1_SPARSE = 10
+ME_KBIT_MME_FLAT2_SPARSE = 11
+ME_KBIT_MME_FLAT3_SPARSE = 12
+ME_KBIT_MME_ROWS1 = 13
+ME_KBIT_MME_ROWS2 = 14
+ME_KBIT_MME_ROWS3 = 15
+ME_KBIT_MME_PLANE = 16
+ME_KBIT_MME_GENERIC = 17
+ME_KBIT_MME_SOLO = 18
+ME_KBIT_SCS_R5 = 19
+ME_KBIT_SCS_RT_CACHED = 20
+ME_KBIT_SCS_RT_UNCACHED = 21
+ME_KBIT_COUNT = 22
+# name -> value of every kernel bit (ME_KBIT_COUNT excluded)
+KERNEL_BITS = {k: v for k, v in dict(globals()).items() if k.startswith("ME_KBIT_") and k != "ME_KBIT_COUNT"}
+
+
+def kernel_bit_names(mask):
+    """the ME_KBIT_* names set in a me_kernel_trace mask"""
+    return {k for k, v in KERNEL_BITS.items() if mask >> v & 1}
+
+
 ME_N_STAGE_TIMES = 9
 STAGE_NAMES = ("grid_est", "grid_gt", "nn_est_to_gt", "nn_gt_to_est", "mme_est", "mme_gt",
                "voxel_moments", "awd", "scs")

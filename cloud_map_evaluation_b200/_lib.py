@@ -20,7 +20,7 @@ SYMBOLS = (
     "me_eval_awd", "me_awd_from_rows", "me_free", "me_get_stage_times", "me_launch_count",
     "me_accum_reset", "me_eval_nn_accum_device", "me_eval_mme_accum_device", "me_accum_block", "me_accum_fetch",
     "me_set_layout", "me_layout_active", "me_voxel_begin", "me_voxel_w_table", "me_voxel_finish_accum_device", "me_accum_fetch_awd",
-    "me_plan_slab_cut", "me_plan_lattice",
+    "me_plan_slab_cut", "me_plan_lattice", "me_kernel_trace",
 )
 
 _lib = None
@@ -94,6 +94,7 @@ def load():
     L.me_get_stage_times.argtypes = [ctx, dp]
     L.me_launch_count.argtypes = [ctx]
     L.me_launch_count.restype = C.c_int64
+    L.me_kernel_trace.argtypes = [ctx, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.c_int32]
     if L.me_abi_version() != A.ME_ABI_VERSION:
         raise RuntimeError("libmapeval_b200.so ABI version mismatch")
     _lib = L

@@ -209,6 +209,8 @@ int me_create(const me_options *opt, me_ctx **out) {
   }
   bool ok = cudaMalloc(&ctx->d_scratch, kScratchBytes) == cudaSuccess && cudaMallocHost(&ctx->h_pinned, kScratchBytes) == cudaSuccess;
   ok = ok && cudaMalloc((void **)&ctx->d_block, kBlkTotal * sizeof(double)) == cudaSuccess;
+  ok = ok && cudaMalloc((void **)&ctx->d_trace, sizeof(unsigned int)) == cudaSuccess &&
+       cudaMemsetAsync(ctx->d_trace, 0, sizeof(unsigned int), ctx->stream) == cudaSuccess;
   ok = ok && cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking) == cudaSuccess;
   ok = ok && cudaEventCreateWithFlags(&ctx->compute_mark, cudaEventDisableTiming) == cudaSuccess;
   for (int w = 0; ok && w < 2; ++w) ok = cudaEventCreateWithFlags(&ctx->cloud[w].upload_done, cudaEventDisableTiming) == cudaSuccess;
@@ -231,6 +233,7 @@ void me_destroy(me_ctx *ctx) {
   stage_pool_free(ctx);
   if (ctx->d_scratch) cudaFree(ctx->d_scratch);
   if (ctx->d_block) cudaFree(ctx->d_block);
+  if (ctx->d_trace) cudaFree(ctx->d_trace);
   if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
   if (ctx->d_work) cudaFree(ctx->d_work);
   if (ctx->d_scan_tmp) cudaFree(ctx->d_scan_tmp);
@@ -695,5 +698,20 @@ int me_get_stage_times(me_ctx *ctx, double ms[ME_N_STAGE_TIMES]) {
 }
 
 int64_t me_launch_count(const me_ctx *ctx) { return ctx ? ctx->launches : 0; }
+
+int me_kernel_trace(me_ctx *ctx, uint64_t *mask, int32_t *mme_rows_cfg, int32_t reset) {
+  ME_ENTER(ctx);
+  unsigned int dev = 0;      // the bits the far / brute kernels set
+  ME_CUDA(ctx, cudaMemcpyAsync(&dev, ctx->d_trace, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
+  ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (mask) *mask = (uint64_t)(ctx->kernel_mask | dev);
+  if (mme_rows_cfg) *mme_rows_cfg = ctx->mme_rows_cfg;
+  if (reset) {
+    ctx->kernel_mask = 0;
+    ctx->mme_rows_cfg = 0;
+    ME_CUDA(ctx, cudaMemsetAsync(ctx->d_trace, 0, sizeof(unsigned int), ctx->stream));
+  }
+  return ME_OK;
+}
 
 }  // extern "C"

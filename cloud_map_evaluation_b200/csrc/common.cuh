@@ -185,6 +185,11 @@ struct me_ctx {
   bool ev_used[ME_N_STAGE_TIMES];
   int sm_count = 132;
   long long launches = 0;
+  // me_kernel_trace: sweep paths chosen on the host (1 << ME_KBIT_*), the last mme_rows_kernel configuration, and a device
+  // word the far / brute kernels OR their bits into when a query reaches them
+  unsigned long long kernel_mask = 0;
+  int mme_rows_cfg = 0;
+  unsigned int *d_trace = nullptr;
   std::string err;
 };
 
@@ -214,6 +219,9 @@ int ensure_work(me_ctx *ctx, size_t bytes);
     if (e__ != cudaSuccess)                                                                        \
       return me::fail((ctx), ME_ERR_CUDA, std::string("kernel launch: ") + cudaGetErrorString(e__)); \
   } while (0)
+
+// me_kernel_trace: the sweep path `bit` (ME_KBIT_*) was launched
+inline void trace_kernel(me_ctx *ctx, int bit) { ctx->kernel_mask |= 1ull << bit; }
 
 // contiguous range r of W over n items (tile lists; the point ranges of the sweeps come from query_shard, which snaps
 // them to cell boundaries)

@@ -430,6 +430,8 @@ static int launch_rows_v(me_ctx *ctx, Cloud &c, long long qb, long long qe, cons
   const int blocks = (int)std::min<long long>((qe - qb + kRowsThreads - 1) / kRowsThreads, (long long)ctx->sm_count * 192);
   mme_rows_kernel<R, CAP, U><<<blocks, kRowsThreads, smem, ctx->stream>>>(c.d_sorted, c.d_rel, qb, qe, index_of(c), C, c.d_entropy, acc);
   ME_LAUNCH_CHECK(ctx);
+  trace_kernel(ctx, ME_KBIT_MME_ROWS1 + R - 1);
+  ctx->mme_rows_cfg = (CAP << 8) | U;
   return ME_OK;
 }
 
@@ -538,6 +540,7 @@ static int launch_plane(me_ctx *ctx, Cloud &c, long long qb, long long qe, const
   const int blocks = (int)std::min<long long>((qe - qb + kFlatThreads - 1) / kFlatThreads, (long long)ctx->sm_count * 64);
   mme_plane_kernel<<<blocks, kFlatThreads, smem, ctx->stream>>>(c.d_sorted, c.d_rel, qb, qe, index_of(c), C, rings, c.d_entropy, acc);
   ME_LAUNCH_CHECK(ctx);
+  trace_kernel(ctx, ME_KBIT_MME_PLANE);
   return ME_OK;
 }
 
@@ -561,6 +564,7 @@ static int launch_flat(me_ctx *ctx, Cloud &c, long long qb, long long qe, const 
   else
     mme_flat_kernel<R, E16, U2, 0><<<blocks, kFlatThreads, smem, ctx->stream>>>(c.d_sorted, c.d_rel, qb, qe, index_of(c), C, c.d_entropy, acc);
   ME_LAUNCH_CHECK(ctx);
+  trace_kernel(ctx, (c.lat.sparse ? ME_KBIT_MME_FLAT1_SPARSE : ME_KBIT_MME_FLAT1_DENSE) + R - 1);
   return ME_OK;
 }
 
@@ -600,6 +604,7 @@ int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors, me_mme_acc
     }
   }
   ME_TRY(build_grid(ctx, which, solo ? 0.5 * radius : 0.0));
+  if (c.grid_solo) trace_kernel(ctx, ME_KBIT_MME_SOLO);
   StageTimer timer(ctx, which == ME_CLOUD_EST ? 4 : 5);
   long long qb, qe;
   ME_TRY(query_shard(ctx, which, &qb, &qe));     // contiguous, cell-aligned range of the cell-sorted order
@@ -657,6 +662,7 @@ int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors, me_mme_acc
       mme_kernel<<<blocks, kThreads, 0, ctx->stream>>>(c.d_sorted, qb, qe, index_of(c), c.lat, radius * radius, rc2, rings,
                                                       min_neighbors, owned_of(c), c.d_entropy, acc);
       ME_LAUNCH_CHECK(ctx);
+      trace_kernel(ctx, ME_KBIT_MME_GENERIC);
     }
   }
   if (to_block) {

@@ -619,12 +619,14 @@ __global__ void __launch_bounds__(kThreads)
 nn_far_kernel(const P4 *__restrict__ Q, const P4 *__restrict__ R, CellIndex I, Lattice L, CoarseGrid CG,
               NNConst C, int32_t *__restrict__ nn_idx, double *__restrict__ nn_d2,
               const uint32_t *__restrict__ far_list, const unsigned int *__restrict__ far_count,
-              uint32_t *__restrict__ unres_list, unsigned int *__restrict__ unres_count, AccBlock *__restrict__ acc) {
+              uint32_t *__restrict__ unres_list, unsigned int *__restrict__ unres_count, AccBlock *__restrict__ acc,
+              unsigned int *__restrict__ trace) {
   const unsigned FULL = 0xffffffffu;
   const int lane = threadIdx.x & 31;
   const long long warp = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
   const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
   const unsigned int nfar = *far_count;
+  if (blockIdx.x == 0 && threadIdx.x == 0 && nfar > 0) atomicOr(trace, 1u << ME_KBIT_NN_FAR);
   // with a coarse grid the cell-by-cell rings stop after kFineRings and blocks of f^3 cells take over
   const int fine_rings = CG.cnt ? 4 : 0x7fffffff;
   for (long long w = warp; w < nfar; w += nwarps) {
@@ -690,6 +692,7 @@ nn_far_kernel(const P4 *__restrict__ Q, const P4 *__restrict__ R, CellIndex I, L
       // coarse phase: Chebyshev rings of blocks of f^3 cells around the query's block; empty blocks cost one count load,
       // occupied blocks that can still hold a closer point are scanned by the whole warp (lanes over the block's f^2 rows)
       const int f = CG.f;
+      if (lane == 0) atomicOr(trace, 1u << ME_KBIT_NN_FAR_COARSE);
       const long long cqx = min(max(ix, 0ll), (long long)L.dims[0] - 1) / f, cqy = min(max(iy, 0ll), (long long)L.dims[1] - 1) / f,
                       cqz = min(max(iz, 0ll), (long long)L.dims[2] - 1) / f;
       for (int rc = 0; !done; ++rc) {
@@ -718,9 +721,11 @@ nn_far_kernel(const P4 *__restrict__ Q, const P4 *__restrict__ R, CellIndex I, L
               mask &= mask - 1;
               const long long sbx = __shfl_sync(FULL, bx, src), sby = __shfl_sync(FULL, by, src), sbz = __shfl_sync(FULL, bz, src);
               const int xa = (int)(sbx * f), xb = (int)min(sbx * f + f - 1, (long long)L.dims[0] - 1);
-              for (int row = lane; row < f * f; row += 32) {
-                const long long z = sbz * f + row / f, y = sby * f + row % f;
-                if (z >= L.dims[2] || y >= L.dims[1]) continue;
+              // the block's rows inside the lattice only: on a lattice long along x (f = 2^17 for 1.8e7 cells) the f^2 rows
+              // of a full block would overflow an int, and nearly all of them lie outside a thin lattice
+              const long long ny = min((long long)f, (long long)L.dims[1] - sby * f), nz = min((long long)f, (long long)L.dims[2] - sbz * f);
+              for (long long row = lane; row < ny * nz; row += 32) {
+                const long long z = sbz * f + row / ny, y = sby * f + row % ny;
                 uint32_t s, e;
                 cell_range(I, (int)z, (int)y, xa, xb, s, e);
                 for (uint32_t j = s; j < e; ++j) {
@@ -757,11 +762,12 @@ nn_far_kernel(const P4 *__restrict__ Q, const P4 *__restrict__ R, CellIndex I, L
 __global__ void __launch_bounds__(kThreads)
 nn_brute_kernel(const P4 *__restrict__ Q, const double *__restrict__ ref_xyz, long long n_ref, NNConst C,
                 int32_t *__restrict__ nn_idx, double *__restrict__ nn_d2, const uint32_t *__restrict__ unres_list,
-                const unsigned int *__restrict__ unres_count) {
+                const unsigned int *__restrict__ unres_count, unsigned int *__restrict__ trace) {
   const int lane = threadIdx.x & 31;
   const long long warp = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
   const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
   const unsigned int nu = *unres_count;
+  if (blockIdx.x == 0 && threadIdx.x == 0 && nu > 0) atomicOr(trace, 1u << ME_KBIT_NN_BRUTE);
   for (long long w = warp; w < nu; w += nwarps) {
     const long long i = unres_list[w];
     const P4 q = load_p4(Q + i);
@@ -945,6 +951,7 @@ static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, me_nn_a
       nn_tile_kernel<<<grid, kTileThreads, dyn_smem, ctx->stream>>>(
           Qc.d_sorted, Qc.d_cell_off, Qc.lat, Qc.d_tiles, tb, te, Rc.d_sorted, Rc.d_cell_off, Rc.lat, C, Qc.d_nn_idx,
           Qc.d_nn_d2, Qc.d_nn_sq, far_list, far_count);
+      trace_kernel(ctx, ME_KBIT_NN_TILE);
     } else {
       FlatGeom G;
       G.qdimx = Qc.lat.dims[0]; G.qdimy = Qc.lat.dims[1];
@@ -964,26 +971,31 @@ static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, me_nn_a
       // default: the warp-synchronous row walk, 4 candidates per iteration (C3 on one H100: 1.6 / 2.3 ms per direction
       // against 1.7 / 2.4 ms for the run-table walk, which stays behind ME_NN_KERNEL=flat)
       const char *kv = getenv("ME_NN_KERNEL");
-      if (kv && !strcmp(kv, "flat"))
+      if (kv && !strcmp(kv, "flat")) {
         nn_flat_kernel<true, 0><<<grid, kFlatThreads, 0, ctx->stream>>>(Qc.d_sorted, Qc.d_rel, qb, qe, Rc.d_sorted, Rc.d_rel,
                                                                         index_of(Rc), Rc.lat, G, C, Qc.d_nn_idx, Qc.d_nn_d2,
                                                                         Qc.d_nn_sq, far_list, far_count);
-      else if (Rc.lat.sparse)
+        trace_kernel(ctx, ME_KBIT_NN_FLAT);
+      } else if (Rc.lat.sparse) {
         nn_rows_kernel<4, 1><<<grid, kFlatThreads, 0, ctx->stream>>>(Qc.d_sorted, Qc.d_rel, qb, qe, Rc.d_sorted, Rc.d_rel,
                                                                      index_of(Rc), Rc.lat, G, C, Qc.d_nn_idx, Qc.d_nn_d2,
                                                                      Qc.d_nn_sq, far_list, far_count);
-      else
+        trace_kernel(ctx, ME_KBIT_NN_ROWS_SPARSE);
+      } else {
         nn_rows_kernel<4, 0><<<grid, kFlatThreads, 0, ctx->stream>>>(Qc.d_sorted, Qc.d_rel, qb, qe, Rc.d_sorted, Rc.d_rel,
                                                                      index_of(Rc), Rc.lat, G, C, Qc.d_nn_idx, Qc.d_nn_d2,
                                                                      Qc.d_nn_sq, far_list, far_count);
+        trace_kernel(ctx, ME_KBIT_NN_ROWS_DENSE);
+      }
     }
     ME_LAUNCH_CHECK(ctx);
     nn_far_kernel<<<ctx->sm_count * 4, kThreads, 0, ctx->stream>>>(Qc.d_sorted, Rc.d_sorted, index_of(Rc), Rc.lat, coarse_of(Rc), C,
-                                                                  Qc.d_nn_idx, Qc.d_nn_d2, far_list, far_count, unres_list, unres_count, acc);
+                                                                  Qc.d_nn_idx, Qc.d_nn_d2, far_list, far_count, unres_list, unres_count, acc,
+                                                                  ctx->d_trace);
     ME_LAUNCH_CHECK(ctx);
     if (Rc.slab) {
       nn_brute_kernel<<<ctx->sm_count * 4, kThreads, 0, ctx->stream>>>(Qc.d_sorted, Rc.d_xyz, Rc.n, C, Qc.d_nn_idx, Qc.d_nn_d2,
-                                                                      unres_list, unres_count);
+                                                                      unres_list, unres_count, ctx->d_trace);
       ME_LAUNCH_CHECK(ctx);
     }
     if (C.accumulate) {

@@ -292,6 +292,15 @@ awd_kernel(Lattice Le, Lattice Lg, const int32_t *__restrict__ cnt_e, const doub
 }
 
 // ---- SCS: one warp per paired voxel, lanes over the (2R+1)^3 - 1 neighbour offsets (map_eval.cpp:351-387) -------
+static constexpr int kScsMaxPerLane = 48;      // neighbour values a lane keeps in registers (radius <= 5: 1331 / 32 = 42)
+
+// me_kernel_trace: which scs_kernel path a radius takes
+static void trace_scs(me_ctx *ctx, int radius) {
+  const int side = 2 * radius + 1;
+  trace_kernel(ctx, radius == 5 ? ME_KBIT_SCS_R5
+                    : ((side * side * side + 31) / 32 <= kScsMaxPerLane ? ME_KBIT_SCS_RT_CACHED : ME_KBIT_SCS_RT_UNCACHED));
+}
+
 template <int RADIUS>      // RADIUS > 0: compile-time neighbourhood (the reference hard-codes 5, map_eval.cpp:353); 0: run time
 __global__ void __launch_bounds__(kThreads)
 scs_kernel(Lattice Le, const double *__restrict__ w_vox, const uint32_t *__restrict__ pair_list, int radius_rt,
@@ -311,7 +320,7 @@ scs_kernel(Lattice Le, const double *__restrict__ w_vox, const uint32_t *__restr
     const int vz = (int)(vox / ((long long)Le.nvox[0] * Le.nvox[1]));
     // the lane's share of the (2R+1)^3 - 1 neighbour values is fetched once (all loads in flight together) and kept for
     // both passes of the reference's mean / population-variance computation (map_eval.cpp:364-381)
-    constexpr int kMaxPerLane = 48;                  // radius <= 5: 1331 / 32 = 42 values per lane
+    constexpr int kMaxPerLane = kScsMaxPerLane;
     double wv[kMaxPerLane];
     const int per_lane = (total + 31) / 32;
     const bool cached = per_lane <= kMaxPerLane;
@@ -466,6 +475,7 @@ static int voxel_scs_impl(me_ctx *ctx, int scs_radius) {
   if (scs_radius == 5) scs_kernel<5><<<ctx->sm_count * 4, kThreads, 0, ctx->stream>>>(Le, w_vox, pair_list, scs_radius, acc);
   else scs_kernel<0><<<ctx->sm_count * 4, kThreads, 0, ctx->stream>>>(Le, w_vox, pair_list, scs_radius, acc);
   ME_LAUNCH_CHECK(ctx);
+  trace_scs(ctx, scs_radius);
   return ME_OK;
 }
 
@@ -607,6 +617,7 @@ int run_awd_rows(me_ctx *ctx, const double *rows27, int64_t n_rows, double voxel
   if (scs_radius == 5) scs_kernel<5><<<ctx->sm_count * 4, kThreads, 0, ctx->stream>>>(L, d_wv, d_pl, scs_radius, acc);
   else scs_kernel<0><<<ctx->sm_count * 4, kThreads, 0, ctx->stream>>>(L, d_wv, d_pl, scs_radius, acc);
   ME_LAUNCH_CHECK(ctx);
+  trace_scs(ctx, scs_radius);
   AwdAcc *h = (AwdAcc *)ctx->h_pinned;
   ME_CUDA(ctx, cudaMemcpyAsync(h, acc, sizeof(AwdAcc), cudaMemcpyDeviceToHost, ctx->stream));
   if (w_out) ME_CUDA(ctx, cudaMemcpyAsync(w_out, d_w, (size_t)n_rows * 8, cudaMemcpyDeviceToHost, ctx->stream));

@@ -318,6 +318,40 @@ ME_API int  me_get_stage_times(me_ctx *ctx, double ms[ME_N_STAGE_TIMES]);
 /* kernels launched by this context since creation (bench.py's gpu_launches) */
 ME_API int64_t me_launch_count(const me_ctx *ctx);
 
+/* Which sweep kernels a context has run: bit (1 << ME_KBIT_x) of the trace mask is set once the path ran.  The kernel
+ * choice depends on the lattice, the cell occupancy, the radius-to-cell ratio and the ME_* environment hooks; the trace
+ * lets a caller (tests, A/B tools) check which one produced a result.  NN_FAR, NN_FAR_COARSE and NN_BRUTE are set only when
+ * at least one query reached that path (recorded on the device); every other bit when its kernel was launched. */
+enum me_kernel_bit {
+  ME_KBIT_NN_ROWS_DENSE = 0,       /* nn_rows_kernel, dense reference table (default)                      */
+  ME_KBIT_NN_ROWS_SPARSE = 1,      /* nn_rows_kernel, sparse reference table                               */
+  ME_KBIT_NN_FLAT = 2,             /* nn_flat_kernel, run-table walk (ME_NN_KERNEL=flat)                   */
+  ME_KBIT_NN_TILE = 3,             /* nn_tile_kernel (>= 2^24 cells along x, crowded cells, ME_NN_TILE)    */
+  ME_KBIT_NN_FAR = 4,              /* nn_far_kernel resolved queries with cell rings                       */
+  ME_KBIT_NN_FAR_COARSE = 5,       /* ... and some went on to its coarse-block phase                       */
+  ME_KBIT_NN_BRUTE = 6,            /* nn_brute_kernel finished queries that left this rank's slab          */
+  ME_KBIT_MME_FLAT1_DENSE = 7,     /* mme_flat_kernel at 1 / 2 / 3 rings, dense table                      */
+  ME_KBIT_MME_FLAT2_DENSE = 8,
+  ME_KBIT_MME_FLAT3_DENSE = 9,
+  ME_KBIT_MME_FLAT1_SPARSE = 10,   /* mme_flat_kernel at 1 / 2 / 3 rings, sparse table                     */
+  ME_KBIT_MME_FLAT2_SPARSE = 11,
+  ME_KBIT_MME_FLAT3_SPARSE = 12,
+  ME_KBIT_MME_ROWS1 = 13,          /* mme_rows_kernel at 1 / 2 / 3 rings (ME_MME_KERNEL=rows)              */
+  ME_KBIT_MME_ROWS2 = 14,
+  ME_KBIT_MME_ROWS3 = 15,
+  ME_KBIT_MME_PLANE = 16,          /* mme_plane_kernel, 4 .. 15 rings                                      */
+  ME_KBIT_MME_GENERIC = 17,        /* mme_kernel, the fp64 row walk                                        */
+  ME_KBIT_MME_SOLO = 18,           /* the MME sweep laid the cloud out on a lattice of its own (h = r / 2) */
+  ME_KBIT_SCS_R5 = 19,             /* scs_kernel with the compiled radius 5                                */
+  ME_KBIT_SCS_RT_CACHED = 20,      /* scs_kernel, run-time radius, neighbour values cached per lane        */
+  ME_KBIT_SCS_RT_UNCACHED = 21,    /* scs_kernel, run-time radius too large for the per-lane cache         */
+  ME_KBIT_COUNT = 22
+};
+/* *mask (nullable) = the trace since creation or the last reset; *mme_rows_cfg (nullable) = (CAP << 8) | U of the last
+ * mme_rows_kernel<R, CAP, U> launched (ring slots, candidates per iteration), 0 if none.  reset != 0 clears both.
+ * Synchronises the context's stream. */
+ME_API int me_kernel_trace(me_ctx *ctx, uint64_t *mask, int32_t *mme_rows_cfg, int32_t reset);
+
 #ifdef __cplusplus
 }
 #endif

@@ -51,6 +51,20 @@ def test_struct_sizes_match_the_header(tmp_path):
     assert C.sizeof(A.me_nn_accum) == 8 * (A.ME_NN_ACCUM_I64 + A.ME_NN_ACCUM_F64)
 
 
+def test_kernel_bit_enum_mirror_matches_the_header():
+    """enum me_kernel_bit of the header and its ctypes mirror: the same names with the same values, one bit each, dense
+    from 0 to ME_KBIT_COUNT - 1 (the kernel-path tests generate their cases from the mirror)."""
+    text = open(os.path.join(ROOT, "include", "mapeval_b200.h")).read()
+    body = re.search(r"enum\s+me_kernel_bit\s*\{(.*?)\};", text, flags=re.S).group(1)
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    declared = {k: int(v) for k, v in re.findall(r"\b(ME_KBIT_\w+)\s*=\s*(\d+)", body)}
+    assert len(declared) == body.count("=")      # every entry carries an explicit value
+    count = declared.pop("ME_KBIT_COUNT")
+    assert declared == A.KERNEL_BITS
+    assert sorted(declared.values()) == list(range(count)) and count == A.ME_KBIT_COUNT
+    assert A.kernel_bit_names((1 << A.ME_KBIT_NN_TILE) | (1 << A.ME_KBIT_SCS_R5)) == {"ME_KBIT_NN_TILE", "ME_KBIT_SCS_R5"}
+
+
 def test_no_cpu_fallback_without_a_device(L):
     import torch
     if torch.cuda.is_available():

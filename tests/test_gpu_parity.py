@@ -108,6 +108,9 @@ def test_nn_far_queries_clusters_and_outliers(api, O):
         e, g = ctx.eval_nn_accum(p)
         got = ctx.nn_finalize(p, e, g)
         idx_e, d2_e = ctx.get_nn(A.ME_CLOUD_EST)
+        # the ground truth's lattice stays below 257 cells per axis here, so the far kernel has no coarse-block phase to
+        # enter; tests/test_gpu_kernel_paths.py ("clusters") reaches it
+        assert "ME_KBIT_NN_FAR" in ctx.kernel_trace()[0]
     assert e.n_far > 1000
     exp = O.eval_nn(est, gt, p)
     _cmp_nn(got, exp)
@@ -168,9 +171,18 @@ def test_mme_radius_to_cell_ratios(api, O, cells_per_radius, shared_lattice):
     p = A.make_nn_params(cfg["tau"], 1.0, pairing=A.ME_PAIRING_GEOMETRIC)
     if shared_lattice:
         os.environ["ME_MME_SHARED_LATTICE"] = "1"
+    rings = int(np.ceil(cells_per_radius - 1e-9))
+    table = "SPARSE" if os.environ.get("ME_FORCE_SPARSE") else "DENSE"
+    if rings <= 3:
+        kernels = {f"ME_KBIT_MME_FLAT{rings}_{table}"}
+    elif not shared_lattice:
+        kernels = {"ME_KBIT_MME_SOLO", f"ME_KBIT_MME_FLAT2_{table}"}      # h = r / 2 on the cloud's own lattice
+    else:
+        kernels = {"ME_KBIT_MME_PLANE" if rings <= 15 else "ME_KBIT_MME_GENERIC"}
     try:
         with _ctx(api, est, gt, nn_cell_size=r / cells_per_radius) as ctx:
             got = ctx.computeMME(A.ME_CLOUD_EST, r, 10)
+            assert ctx.kernel_trace()[0] == kernels
             nn = ctx.calculateMetricsWithInitialMatrix(p)
             ent = ctx.get_entropies(A.ME_CLOUD_EST)       # after the NN stage re-laid the cloud out
     finally:
@@ -307,9 +319,13 @@ def test_shard_count_invariance(api, O, world, tile):
     p = A.make_nn_params(cfg["tau"], 1.0, pairing=A.ME_PAIRING_AS_WRITTEN)
     if tile:
         os.environ["ME_NN_TILE"] = "1"
+    # the tile sweep needs a dense cell table; on a sparse one ME_NN_TILE falls back to the row walk
+    sweep = ("ME_KBIT_NN_ROWS_SPARSE" if os.environ.get("ME_FORCE_SPARSE")
+             else ("ME_KBIT_NN_TILE" if tile else "ME_KBIT_NN_ROWS_DENSE"))
     try:
         with _ctx(api, est, gt) as ctx:
             ref = ctx.calculateMetricsWithInitialMatrix(p)
+            assert sweep in ctx.kernel_trace()[0]
             ref_m = ctx.eval_mme_accum(A.ME_CLOUD_EST, 0.1, 10)
         tot_e, tot_g, tot_m = A.me_nn_accum(), A.me_nn_accum(), A.me_mme_accum()
         tot_m.min_entropy, tot_m.max_entropy = np.inf, -np.inf
@@ -318,6 +334,7 @@ def test_shard_count_invariance(api, O, world, tile):
             perm_e = np.random.RandomState(100 + r).permutation(len(est))
             with _ctx(api, est[perm_e], gt, rank=r, world=world) as ctx:
                 e, g = ctx.eval_nn_accum(p_geo := A.make_nn_params(cfg["tau"], 1.0, pairing=A.ME_PAIRING_GEOMETRIC))
+                assert sweep in ctx.kernel_trace()[0]
                 m = ctx.eval_mme_accum(A.ME_CLOUD_EST, 0.1, 10)
             for tot, part in ((tot_e, e), (tot_g, g)):
                 for name, ctype in A.me_nn_accum._fields_:

@@ -79,6 +79,8 @@ def test_sparse_table_far_queries_normals_and_shards(api, O):
         e, g = ctx.eval_nn_accum(p)
         nn = ctx.nn_finalize(p, e, g)
         idx, d2 = ctx.get_nn(A.ME_CLOUD_EST)
+        # the outliers lie beyond the far kernel's cell rings: its coarse-block phase (> 256 cells per axis) finds them
+        assert {"ME_KBIT_NN_FAR", "ME_KBIT_NN_FAR_COARSE", "ME_KBIT_NN_ROWS_SPARSE"} <= ctx.kernel_trace()[0]
         nrm = ctx.estimate_normals(A.ME_CLOUD_GT, 20)
     assert e.n_far > 500
     oi, od2 = O.knn1(est, gt)
