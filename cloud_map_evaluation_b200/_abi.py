@@ -1,7 +1,7 @@
 """ctypes mirror of include/mapeval_b200.h (struct layouts and constants only — no library is loaded here)."""
 import ctypes as C
 
-ME_ABI_VERSION = 1
+ME_ABI_VERSION = 2
 
 ME_OK = 0
 ME_ERR_INVALID = -1
@@ -80,15 +80,18 @@ class me_nn_params(C.Structure):
                 ("pairing", C.c_int32), ("want_full_cd", C.c_int32), ("directions", C.c_int32)]
 
 
+ME_MAX_WORLD = 64
 ME_NN_ACCUM_I64 = 9
-ME_NN_ACCUM_F64 = 13
+ME_NN_ACCUM_F64 = 13 + 3 * ME_MAX_WORLD
 
 
 class me_nn_accum(C.Structure):
     _fields_ = [("n_query", C.c_int64), ("n_corr", C.c_int64), ("n_inlier", C.c_int64 * 5), ("n_ub", C.c_int64),
                 ("n_far", C.c_int64),
                 ("sum_d", C.c_double * 5), ("sum_d2", C.c_double * 5), ("sum_d_all", C.c_double),
-                ("sum_d2_all", C.c_double), ("sum_nn_dist", C.c_double)]
+                ("sum_d2_all", C.c_double), ("sum_nn_dist", C.c_double),
+                ("rank_n", C.c_double * ME_MAX_WORLD), ("rank_mean", C.c_double * ME_MAX_WORLD),
+                ("rank_m2", C.c_double * ME_MAX_WORLD)]
 
 
 class me_dir_result(C.Structure):

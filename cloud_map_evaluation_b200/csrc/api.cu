@@ -79,7 +79,7 @@ static void free_cloud(Cloud &c) {
 
 using namespace me;
 
-static constexpr size_t kScratchBytes = 4096;
+static constexpr size_t kScratchBytes = 8192;   // h_pinned: up to 4 KB of per-stage scratch, then the accumulator block
 
 // ---- upload from PAGEABLE host memory ------------------------------------------------------------------------------
 // cudaMemcpyAsync from pageable memory goes through the driver's single staging buffer, which for the 480 MB of the
@@ -180,6 +180,8 @@ int me_create(const me_options *opt, me_ctx **out) {
   *out = nullptr;
   if (!opt || opt->abi_version != ME_ABI_VERSION) return fail(nullptr, ME_ERR_INVALID, "me_options.abi_version mismatch");
   if (opt->world < 1 || opt->rank < 0 || opt->rank >= opt->world) return fail(nullptr, ME_ERR_INVALID, "bad rank/world");
+  if (opt->world > ME_MAX_WORLD)
+    return fail(nullptr, ME_ERR_INVALID, "world " + std::to_string(opt->world) + " > ME_MAX_WORLD = " + std::to_string(ME_MAX_WORLD));
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
   if (e != cudaSuccess || ndev <= 0) {
@@ -261,6 +263,8 @@ int me_set_stream(me_ctx *ctx, void *cuda_stream) {
 int me_set_shard(me_ctx *ctx, int32_t rank, int32_t world) {
   ME_ENTER(ctx);
   if (world < 1 || rank < 0 || rank >= world) return fail(ctx, ME_ERR_INVALID, "bad rank/world");
+  if (world > ME_MAX_WORLD)
+    return fail(ctx, ME_ERR_INVALID, "world " + std::to_string(world) + " > ME_MAX_WORLD = " + std::to_string(ME_MAX_WORLD));
   ctx->rank = rank; ctx->world = world;
   ctx->slab_planned = false; ctx->slab_on = false; ctx->vox_open = false;
   ctx->cloud[0].grid_valid = ctx->cloud[1].grid_valid = false;      // slab lattices belong to one (rank, world)
@@ -475,16 +479,14 @@ int me_eval_nn_accum(me_ctx *ctx, const me_nn_params *p, me_nn_accum *est_to_gt,
 
 // ---- device-resident accumulators: sweep -> (all-reduce on the device by the caller) -> one fetch per pass ----------------
 __global__ void block_init_kernel(double *blk) {
-  const int t = threadIdx.x;
-  if (t < me::kBlkSumCount) blk[t] = 0.0;
-  else if (t < me::kBlkTotal) blk[t] = -INFINITY;
+  for (int t = threadIdx.x; t < me::kBlkTotal; t += blockDim.x) blk[t] = t < me::kBlkSumCount ? 0.0 : -INFINITY;
 }
 
 extern "C" {
 
 int me_accum_reset(me_ctx *ctx) {
   ME_ENTER(ctx);
-  block_init_kernel<<<1, 64, 0, ctx->stream>>>(ctx->d_block);
+  block_init_kernel<<<1, 256, 0, ctx->stream>>>(ctx->d_block);
   ME_LAUNCH_CHECK(ctx);
   return ME_OK;
 }
@@ -530,7 +532,7 @@ int me_voxel_finish_accum_device(me_ctx *ctx, int32_t scs_radius) {
 int me_accum_fetch_awd(me_ctx *ctx, me_awd_result *out) {
   ME_ENTER(ctx);
   if (!out) return fail(ctx, ME_ERR_INVALID, "null result");
-  double *h = (double *)((char *)ctx->h_pinned + 3072);
+  double *h = (double *)((char *)ctx->h_pinned + 4096);
   ME_CUDA(ctx, cudaMemcpyAsync(h, ctx->d_block + kBlkAwd, 8 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   auto i64 = [](double v) { return (int64_t)std::llround(v); };
@@ -546,7 +548,8 @@ int me_accum_fetch_awd(me_ctx *ctx, me_awd_result *out) {
 
 int me_accum_fetch(me_ctx *ctx, me_nn_accum *est_to_gt, me_nn_accum *gt_to_est, me_mme_accum *mme_est, me_mme_accum *mme_gt) {
   ME_ENTER(ctx);
-  double *h = (double *)((char *)ctx->h_pinned + 3072);
+  static_assert(4096 + kBlkTotal * sizeof(double) <= kScratchBytes, "the accumulator block fits the pinned scratch");
+  double *h = (double *)((char *)ctx->h_pinned + 4096);
   ME_CUDA(ctx, cudaMemcpyAsync(h, ctx->d_block, kBlkTotal * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   auto i64 = [](double v) { return (int64_t)std::llround(v); };
@@ -560,6 +563,10 @@ int me_accum_fetch(me_ctx *ctx, me_nn_accum *est_to_gt, me_nn_accum *gt_to_est, 
     a->n_ub = i64(b[7]); a->n_far = i64(b[8]);
     for (int k = 0; k < 5; ++k) { a->sum_d[k] = b[9 + k]; a->sum_d2[k] = b[14 + k]; }
     a->sum_d_all = b[19]; a->sum_d2_all = b[20]; a->sum_nn_dist = b[21];
+    for (int r = 0; r < ME_MAX_WORLD; ++r) {
+      a->rank_n[r] = b[kBlkMoments + r]; a->rank_mean[r] = b[kBlkMoments + ME_MAX_WORLD + r];
+      a->rank_m2[r] = b[kBlkMoments + 2 * ME_MAX_WORLD + r];
+    }
   }
   me_mme_accum *mm[2] = {mme_est, mme_gt};
   for (int w = 0; w < 2; ++w) {
@@ -582,15 +589,27 @@ static void finalize_dir(const me_nn_accum *a, int64_t n_source, me_dir_result *
   r->sum_nn_dist = a->sum_nn_dist;
   const double nc = (double)a->n_corr;
   const int target_num = (int)n_source;                       // map_eval.cpp:1128
+  double n_all = 0, mean_all = 0, m2_all = 0;                  // moments of d over all kept pairs, ranks merged in order
+  for (int s = 0; s < ME_MAX_WORLD; ++s) chan_merge(n_all, mean_all, m2_all, a->rank_n[s], a->rank_mean[s], a->rank_m2[s]);
+  // every sweep of the library fills the moments; an accumulator built from the sums only (its slots do not account for
+  // its pairs) has nothing better than the closed form, which cancels when the spread of d is small against its mean
+  const bool moments = n_all == nc;
   for (int k = 0; k < 5; ++k) {
     r->n_inlier[k] = a->n_inlier[k];
     const double mean = a->sum_d[k] / nc;                      // :1125
     r->mean[k] = mean;
     r->rmse[k] = std::sqrt(a->sum_d2[k] / nc);                 // :1126,1131
     r->fitness[k] = (double)a->n_inlier[k] * 1.0 / target_num; // :1130
-    // :1132-1138, sum over ALL kept pairs of (d - mean_k)^2, in closed form
-    double ss = a->sum_d2_all - 2.0 * mean * a->sum_d_all + nc * mean * mean;
-    if (ss < 0 && ss > -1e-9 * a->sum_d2_all) ss = 0;
+    // :1132-1138, the sum over ALL kept pairs of (d - mean_k)^2 = M2 + n (mean_all - mean_k)^2: both terms are >= 0, so
+    // nothing cancels however small the spread of d is against its mean
+    double ss;
+    if (moments) {
+      const double dm = mean_all - mean;
+      ss = m2_all + nc * dm * dm;
+    } else {
+      ss = a->sum_d2_all - 2.0 * mean * a->sum_d_all + nc * mean * mean;
+      if (ss < 0 && ss > -1e-9 * a->sum_d2_all) ss = 0;
+    }
     r->sigma[k] = std::sqrt(ss / nc);
   }
 }

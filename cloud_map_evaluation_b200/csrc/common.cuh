@@ -292,10 +292,14 @@ int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors, me_mme_acc
 
 // layout of me_ctx::d_block (fp64): the SUM-reducible part first, then the MAX-reducible part.  Counts ride as fp64 (exact
 // below 2^53, so their sums are exact and order-independent).
-static constexpr int kBlkNN = 22;                    // per direction: n_query n_corr n_inlier[5] n_ub n_far | sum_d[5] sum_d2[5] sum_d_all sum_d2_all sum_nn
+// per direction: n_query n_corr n_inlier[5] n_ub n_far | sum_d[5] sum_d2[5] sum_d_all sum_d2_all sum_nn |
+// rank_n[W] rank_mean[W] rank_m2[W]
+// (me_nn_accum; a rank fills only its own moment slot, so the SUM all-reduce gathers the slots)
+static constexpr int kBlkNN = ME_NN_ACCUM_I64 + ME_NN_ACCUM_F64;
+static constexpr int kBlkMoments = 22;               // offset of rank_n within a direction
 static constexpr int kBlkMmeSum = 2 * kBlkNN;        // per cloud: n_query n_valid sum_entropy
 static constexpr int kBlkAwd = kBlkMmeSum + 6;       // voxel stage: n_pairs n_scs n_voxels_est n_voxels_gt n_active n_new sum_w sum_scs
-static constexpr int kBlkSumCount = kBlkAwd + 8;     // = 58 SUM values
+static constexpr int kBlkSumCount = kBlkAwd + 8;     // = 442 SUM values
 static constexpr int kBlkMax = kBlkSumCount;         // per cloud: max_entropy, -min_entropy
 static constexpr int kBlkMaxCount = 4;
 static constexpr int kBlkTotal = kBlkSumCount + kBlkMaxCount;
@@ -437,6 +441,15 @@ __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+// Chan, Golub & LeVeque's pairwise update: (na, ma, m2a) <- the count, mean and sum of squared deviations of the union of
+// two sets given those of each.  No cancellation: m2 only ever adds non-negative terms.
+__host__ __device__ __forceinline__ void chan_merge(double &na, double &ma, double &m2a, double nb, double mb, double m2b) {
+  if (nb == 0) return;
+  const double n = na + nb, delta = mb - ma;
+  ma += delta * (nb / n);
+  m2a += m2b + delta * delta * (na * (nb / n));
+  na = n;
 }
 __device__ __forceinline__ long long warp_sum_ll(long long v) {
 #pragma unroll

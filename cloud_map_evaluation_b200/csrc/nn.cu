@@ -49,21 +49,31 @@ __device__ __forceinline__ double cover_dist_cells(const NNConst &C, double uy, 
   return fmin(C.cov_lo > 0 ? ua - (double)C.cov_lo : INFINITY, C.cov_hi < C.cov_dim ? (double)C.cov_hi - ua : INFINITY);
 }
 
-// device accumulator block: 8 x int64 then 13 x fp64 (see me_nn_accum)
+// device accumulator block of one direction: 8 x int64, 11 fp64 summed with atomics, then what merge_moments_kernel
+// derives from the blocks' (n, mean, M2) of the kept d: their mean and M2, and sum(d), sum(d^2) (= n mean, M2 + n mean^2)
 struct AccBlock {
   unsigned long long n_corr, n_inl[5], n_ub, n_far;
-  double sum_d[5], sum_d2[5], sum_d_all, sum_d2_all, sum_nn;
+  double sum_d[5], sum_d2[5], sum_nn;
+  double mean_all, m2_all, sum_d_all, sum_d2_all;
 };
 
 struct LocalAcc {
   unsigned int n_corr, n_inl[5], n_ub;
-  double sum_d[5], sum_d2[5], sum_d_all, sum_d2_all, sum_nn;
+  double sum_d[5], sum_d2[5], sum_nn;
+  // this thread's kept d as sums of (d - shift) and (d - shift)^2, shift = its first kept d: the sums then cancel by at
+  // most a factor n_corr + 1 when they are turned into (mean, M2), since n (mean - shift)^2 <= n M2
+  double shift, s1, s2;
   __device__ void clear() {
-    n_corr = 0; n_ub = 0; sum_d_all = 0; sum_d2_all = 0; sum_nn = 0;
+    n_corr = 0; n_ub = 0; sum_nn = 0; shift = 0; s1 = 0; s2 = 0;
 #pragma unroll
     for (int k = 0; k < 5; ++k) { n_inl[k] = 0; sum_d[k] = 0; sum_d2[k] = 0; }
   }
-  __device__ __forceinline__ void pair(double nd, double sq) { n_corr++; sum_d_all += nd; sum_d2_all += sq; }
+  __device__ __forceinline__ void pair(double nd, double) {
+    if (n_corr++ == 0) shift = nd;
+    const double t = nd - shift;
+    s1 += t;
+    s2 += t * t;
+  }
   __device__ __forceinline__ void inlier(int k, double nd, double sq) { sum_d[k] += nd; sum_d2[k] += sq; n_inl[k]++; }
   __device__ __forceinline__ void nn_dist(double d) { sum_nn += d; }
   __device__ __forceinline__ void ub() { n_ub++; }
@@ -89,29 +99,51 @@ __device__ __forceinline__ void accum_pair(double dx, double dy, double dz, cons
   accum_sq(sqnorm_eigen(dx, dy, dz), c, a);
 }
 
-__device__ void flush_acc(LocalAcc &a, AccBlock *g) {
-  __shared__ double sh_d[kThreads / 32][13];
-  __shared__ unsigned long long sh_i[kThreads / 32][7];
+// (n, mean, M2) of the whole block from every thread's (n, mean, M2), valid in thread 0; every thread of the block calls it
+__device__ void block_moments(double &n, double &m, double &m2) {
+  __shared__ double sh[kThreads / 32][3];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const double nb = __shfl_xor_sync(0xffffffffu, n, o), mb = __shfl_xor_sync(0xffffffffu, m, o),
+                 m2b = __shfl_xor_sync(0xffffffffu, m2, o);
+    chan_merge(n, m, m2, nb, mb, m2b);
+  }
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  double dv[13];
+  if (lane == 0) { sh[warp][0] = n; sh[warp][1] = m; sh[warp][2] = m2; }
+  __syncthreads();
+  if (threadIdx.x == 0)
+    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) chan_merge(n, m, m2, sh[w][0], sh[w][1], sh[w][2]);
+}
+
+// the sums and counts go to g with atomics; the block's (n, mean, M2) of the kept d to mom[3 * blockIdx.x ..] (nullable:
+// the kernel keeps no pairs), which merge_moments_kernel folds in block order
+__device__ void flush_acc(LocalAcc &a, AccBlock *g, double *mom) {
+  __shared__ double sh_d[kThreads / 32][11];
+  __shared__ unsigned long long sh_i[kThreads / 32][7];
+  double mn = (double)a.n_corr, mm = 0, m2 = 0;
+  if (a.n_corr) { mm = a.shift + a.s1 / mn; m2 = fmax(0.0, a.s2 - a.s1 * (a.s1 / mn)); }
+  block_moments(mn, mm, m2);
+  if (mom && threadIdx.x == 0) { mom[3 * blockIdx.x] = mn; mom[3 * blockIdx.x + 1] = mm; mom[3 * blockIdx.x + 2] = m2; }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double dv[11];
   long long iv[7];
 #pragma unroll
   for (int k = 0; k < 5; ++k) { dv[k] = a.sum_d[k]; dv[5 + k] = a.sum_d2[k]; iv[1 + k] = a.n_inl[k]; }
-  dv[10] = a.sum_d_all; dv[11] = a.sum_d2_all; dv[12] = a.sum_nn;
+  dv[10] = a.sum_nn;
   iv[0] = a.n_corr; iv[6] = a.n_ub;
 #pragma unroll
-  for (int k = 0; k < 13; ++k) dv[k] = warp_sum(dv[k]);
+  for (int k = 0; k < 11; ++k) dv[k] = warp_sum(dv[k]);
 #pragma unroll
   for (int k = 0; k < 7; ++k) iv[k] = warp_sum_ll(iv[k]);
   if (lane == 0) {
 #pragma unroll
-    for (int k = 0; k < 13; ++k) sh_d[warp][k] = dv[k];
+    for (int k = 0; k < 11; ++k) sh_d[warp][k] = dv[k];
 #pragma unroll
     for (int k = 0; k < 7; ++k) sh_i[warp][k] = (unsigned long long)iv[k];
   }
   __syncthreads();
   const int nwarps = blockDim.x >> 5;
-  if (threadIdx.x < 13) {
+  if (threadIdx.x < 11) {
     double s = 0;
     for (int w = 0; w < nwarps; ++w) s += sh_d[w][threadIdx.x];
     double *dst = &g->sum_d[0];
@@ -808,9 +840,9 @@ nn_far_sq_kernel(const P4 *__restrict__ Q, const double *__restrict__ ref_xyz, c
 
 // streaming pass over the per-query results of a sweep: the five-threshold accumulators (map_eval.cpp:1095-1123) and the
 // full-Chamfer sum (:1416).  Entries < 0 are queries without a neighbour within reach (-1) or owned by another rank (-2).
-__global__ void __launch_bounds__(kThreads)
+__global__ void __launch_bounds__(kThreads, 4)      // 4 blocks per SM, as before the moments: the grid is 8 per SM
 nn_stats_kernel(long long i_begin, long long i_end, const int32_t *__restrict__ nn_idx, const double *__restrict__ nn_d2,
-                const double *__restrict__ nn_sq, NNConst C, AccBlock *__restrict__ acc) {
+                const double *__restrict__ nn_sq, NNConst C, AccBlock *__restrict__ acc, double *__restrict__ mom) {
   LocalAcc a;
   a.clear();
   for (long long i = i_begin + blockIdx.x * (long long)blockDim.x + threadIdx.x; i < i_end;
@@ -820,7 +852,7 @@ nn_stats_kernel(long long i_begin, long long i_end, const int32_t *__restrict__ 
     if (C.want_full_cd) a.nn_dist(__dsqrt_rn(d2));
     if (C.accumulate && keep_pair(d2, C)) accum_sq(__ldg(nn_sq + i), C, a);
   }
-  flush_acc(a, acc);
+  flush_acc(a, acc, mom);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -828,10 +860,11 @@ nn_stats_kernel(long long i_begin, long long i_end, const int32_t *__restrict__ 
 // :1093-1094 reads gt[nn_est] and est[i_gt].  Reproduced verbatim; out-of-range (UB in the reference) is counted.
 // Walks every gt point; points this rank did not evaluate carry the marker -2.
 // ---------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kThreads)
+__global__ void __launch_bounds__(kThreads, 4)      // as nn_stats_kernel
 pair_as_written_kernel(const P4 *__restrict__ Qgt, long long n, const int32_t *__restrict__ nn_idx,
                        const double *__restrict__ nn_d2, const double *__restrict__ gt_xyz, long long n_gt,
-                       const double *__restrict__ est_xyz, long long n_est, NNConst C, AccBlock *__restrict__ acc) {
+                       const double *__restrict__ est_xyz, long long n_est, NNConst C, AccBlock *__restrict__ acc,
+                       double *__restrict__ mom) {
   LocalAcc a;
   a.clear();
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
@@ -846,7 +879,7 @@ pair_as_written_kernel(const P4 *__restrict__ Qgt, long long n, const int32_t *_
     const double dz = __dsub_rn(__ldg(gt_xyz + 3 * s + 2), __ldg(est_xyz + 3 * t + 2));
     accum_pair(dx, dy, dz, C, a);
   }
-  flush_acc(a, acc);
+  flush_acc(a, acc, mom);
 }
 
 __global__ void fill_i32_kernel(int32_t *p, long long n, int32_t v) {
@@ -873,9 +906,24 @@ __global__ void count_marked_kernel(const int32_t *__restrict__ idx, long long n
   if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, c);
 }
 
-// accumulator block of one direction -> the context's fp64 block (me_eval_nn_accum_device): no host round trip
+// the per-block (n, mean, M2) of a stats pass, merged in block order into acc (one block)
+__global__ void __launch_bounds__(kThreads) merge_moments_kernel(const double *__restrict__ mom, int n_slots, AccBlock *__restrict__ acc) {
+  double n = 0, m = 0, m2 = 0;
+  for (int s = threadIdx.x; s < n_slots; s += blockDim.x) chan_merge(n, m, m2, mom[3 * s], mom[3 * s + 1], mom[3 * s + 2]);
+  block_moments(n, m, m2);
+  if (threadIdx.x == 0) { acc->mean_all = m; acc->m2_all = m2; acc->sum_d_all = n * m; acc->sum_d2_all = m2 + n * m * m; }
+}
+
+// accumulator block of one direction -> the context's fp64 block (me_eval_nn_accum_device): no host round trip.  The
+// moments go to this rank's slot; the other ranks' slots are zeroed, so that the SUM all-reduce gathers them.
 __global__ void pack_nn_kernel(const AccBlock *__restrict__ a, const unsigned long long *__restrict__ n_eval, long long n_query,
-                               double *__restrict__ blk) {
+                               int rank, double *__restrict__ blk) {
+  for (int r = threadIdx.x; r < ME_MAX_WORLD; r += blockDim.x) {
+    const bool mine = r == rank;
+    blk[kBlkMoments + r] = mine ? (double)a->n_corr : 0.0;
+    blk[kBlkMoments + ME_MAX_WORLD + r] = mine ? a->mean_all : 0.0;
+    blk[kBlkMoments + 2 * ME_MAX_WORLD + r] = mine ? a->m2_all : 0.0;
+  }
   if (threadIdx.x != 0) return;
   blk[0] = (double)(n_eval ? (long long)*n_eval : n_query);
   blk[1] = (double)a->n_corr;
@@ -925,13 +973,16 @@ static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, me_nn_a
   ME_TRY(ensure(ctx, (void **)&Qc.d_nn_idx, &Qc.cap_nn, Qc.n, sizeof(int32_t)));
   ME_TRY(ensure(ctx, (void **)&Qc.d_nn_d2, &Qc.cap_nn_d2, Qc.n, sizeof(double)));
   ME_TRY(ensure(ctx, (void **)&Qc.d_nn_sq, &Qc.cap_nn_sq, Qc.n, sizeof(double)));
-  // work buffer: far list and unresolved list (n uint32 each) after a 256-byte header holding the counters
-  ME_TRY(ensure_work(ctx, 256 + 2 * (size_t)Qc.n * sizeof(uint32_t)));
+  // work buffer: far list and unresolved list (n uint32 each) after a 256-byte header holding the counters, then the
+  // per-block moments of the stats pass (3 fp64 per block, at most sm_count * 16 blocks)
+  const int max_mom_slots = ctx->sm_count * 16;
+  ME_TRY(ensure_work(ctx, 256 + 2 * (size_t)Qc.n * sizeof(uint32_t) + 3 * sizeof(double) * (size_t)max_mom_slots));
   unsigned int *far_count = (unsigned int *)ctx->d_work;
   unsigned long long *n_eval = (unsigned long long *)((char *)ctx->d_work + 64);
   unsigned int *unres_count = (unsigned int *)((char *)ctx->d_work + 128);
   uint32_t *far_list = (uint32_t *)((char *)ctx->d_work + 256);
   uint32_t *unres_list = far_list + Qc.n;
+  double *mom = (double *)(unres_list + Qc.n);
   AccBlock *acc = (AccBlock *)ctx->d_scratch;
   ME_CUDA(ctx, cudaMemsetAsync(acc, 0, sizeof(AccBlock), ctx->stream));
   ME_CUDA(ctx, cudaMemsetAsync(ctx->d_work, 0, 256, ctx->stream));
@@ -1003,15 +1054,23 @@ static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, me_nn_a
                                                                     far_count);
       ME_LAUNCH_CHECK(ctx);
     }
+    int mom_slots = 0;     // blocks of the kernel that kept the pairs
     if (C.accumulate || C.want_full_cd) {
       const long long sb = use_tile ? 0 : qb, se = use_tile ? Qc.n : qe;
-      const int sblocks = (int)std::min<long long>((se - sb + kThreads - 1) / kThreads, (long long)ctx->sm_count * 8);
-      nn_stats_kernel<<<std::max(1, sblocks), kThreads, 0, ctx->stream>>>(sb, se, Qc.d_nn_idx, Qc.d_nn_d2, Qc.d_nn_sq, C, acc);
+      const int sblocks = std::max(1, (int)std::min<long long>((se - sb + kThreads - 1) / kThreads, (long long)ctx->sm_count * 8));
+      nn_stats_kernel<<<sblocks, kThreads, 0, ctx->stream>>>(sb, se, Qc.d_nn_idx, Qc.d_nn_d2, Qc.d_nn_sq, C, acc,
+                                                             C.accumulate ? mom : nullptr);
       ME_LAUNCH_CHECK(ctx);
+      if (C.accumulate) mom_slots = sblocks;
     }
     if (as_written) {
       pair_as_written_kernel<<<fill_blocks, kThreads, 0, ctx->stream>>>(Qc.d_sorted, Qc.ns, Qc.d_nn_idx, Qc.d_nn_d2,
-                                                                       Qc.d_xyz, Qc.n, Rc.d_xyz, Rc.n, C, acc);
+                                                                       Qc.d_xyz, Qc.n, Rc.d_xyz, Rc.n, C, acc, mom);
+      ME_LAUNCH_CHECK(ctx);
+      mom_slots = fill_blocks;
+    }
+    if (mom_slots) {
+      merge_moments_kernel<<<1, kThreads, 0, ctx->stream>>>(mom, mom_slots, acc);
       ME_LAUNCH_CHECK(ctx);
     }
   }
@@ -1021,7 +1080,7 @@ static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, me_nn_a
   }
   if (to_block) {      // the accumulators stay on the device (all-reduced there, fetched once per pass)
     pack_nn_kernel<<<1, 32, 0, ctx->stream>>>(acc, (sharded && use_tile) ? n_eval : nullptr, Qc.slab ? Qc.n_owned : (sharded ? qe - qb : Qc.n),
-                                              ctx->d_block + (qwhich == ME_CLOUD_EST ? 0 : kBlkNN));
+                                              ctx->rank, ctx->d_block + (qwhich == ME_CLOUD_EST ? 0 : kBlkNN));
     ME_LAUNCH_CHECK(ctx);
     Qc.nn_valid = true;
     return ME_OK;
@@ -1038,6 +1097,7 @@ static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, me_nn_a
   out->n_ub = (int64_t)h->n_ub;
   out->n_far = (int64_t)h->n_far;
   out->sum_d_all = h->sum_d_all; out->sum_d2_all = h->sum_d2_all; out->sum_nn_dist = h->sum_nn;
+  out->rank_n[ctx->rank] = (double)h->n_corr; out->rank_mean[ctx->rank] = h->mean_all; out->rank_m2[ctx->rank] = h->m2_all;
   Qc.nn_valid = true;
   return ME_OK;
 }

@@ -18,7 +18,7 @@ def pack(nn_e, nn_g, mme_list):
     ints, flts, mins, maxs = [], [], [], []
     for a in (nn_e, nn_g):
         ints += [a.n_query, a.n_corr] + list(a.n_inlier) + [a.n_ub, a.n_far]
-        flts += list(a.sum_d) + list(a.sum_d2) + [a.sum_d_all, a.sum_d2_all, a.sum_nn_dist]
+        flts += list(a.sum_d) + list(a.sum_d2) + [a.sum_d_all, a.sum_d2_all, a.sum_nn_dist] + list(a.rank_n) + list(a.rank_mean) + list(a.rank_m2)
     for m in mme_list:
         ints += [m.n_query, m.n_valid]
         flts += [m.sum_entropy]
@@ -39,6 +39,11 @@ def unpack(ints, flts, mins, maxs, nn_e, nn_g, mme_list):
             a.sum_d[k] = float(flts[fi + k])
             a.sum_d2[k] = float(flts[fi + 5 + k])
         a.sum_d_all, a.sum_d2_all, a.sum_nn_dist = float(flts[fi + 10]), float(flts[fi + 11]), float(flts[fi + 12])
+        W = A.ME_MAX_WORLD
+        for r in range(W):
+            a.rank_n[r] = float(flts[fi + 13 + r])
+            a.rank_mean[r] = float(flts[fi + 13 + W + r])
+            a.rank_m2[r] = float(flts[fi + 13 + 2 * W + r])
         fi += _NN_F
     for j, m in enumerate(mme_list):
         m.n_query, m.n_valid = int(ints[ii]), int(ints[ii + 1])

@@ -136,7 +136,7 @@ class GpuGroup {
   }
 
  private:
-  static constexpr int kMaxValues = 128;
+  static constexpr int kMaxValues = 2 * (ME_NN_ACCUM_I64 + ME_NN_ACCUM_F64);
   static void pack(const me_nn_accum &a, std::vector<double> &v) {
     v.push_back((double)a.n_query); v.push_back((double)a.n_corr);
     for (int k = 0; k < 5; ++k) v.push_back((double)a.n_inlier[k]);
@@ -144,6 +144,9 @@ class GpuGroup {
     for (int k = 0; k < 5; ++k) v.push_back(a.sum_d[k]);
     for (int k = 0; k < 5; ++k) v.push_back(a.sum_d2[k]);
     v.push_back(a.sum_d_all); v.push_back(a.sum_d2_all); v.push_back(a.sum_nn_dist);
+    v.insert(v.end(), a.rank_n, a.rank_n + ME_MAX_WORLD);
+    v.insert(v.end(), a.rank_mean, a.rank_mean + ME_MAX_WORLD);
+    v.insert(v.end(), a.rank_m2, a.rank_m2 + ME_MAX_WORLD);
   }
   static void unpack(const std::vector<double> &v, size_t &k, me_nn_accum &a) {
     auto i64 = [&](void) { return (int64_t)std::llround(v[k++]); };
@@ -153,6 +156,9 @@ class GpuGroup {
     for (int j = 0; j < 5; ++j) a.sum_d[j] = v[k++];
     for (int j = 0; j < 5; ++j) a.sum_d2[j] = v[k++];
     a.sum_d_all = v[k++]; a.sum_d2_all = v[k++]; a.sum_nn_dist = v[k++];
+    for (int j = 0; j < ME_MAX_WORLD; ++j) a.rank_n[j] = v[k++];
+    for (int j = 0; j < ME_MAX_WORLD; ++j) a.rank_mean[j] = v[k++];
+    for (int j = 0; j < ME_MAX_WORLD; ++j) a.rank_m2[j] = v[k++];
   }
 
   std::vector<me_ctx *> ctx_;

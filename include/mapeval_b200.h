@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define ME_ABI_VERSION 1
+#define ME_ABI_VERSION 2
 
 #if defined(__GNUC__)
 #define ME_API __attribute__((visibility("default")))
@@ -89,9 +89,17 @@ typedef struct {
   int32_t directions;        /* bit0: est->gt, bit1: gt->est; 0 = both                     */
 } me_nn_params;
 
-/* sum-reducible partial accumulators of one direction (int64 block first, then fp64 block) */
+/* Largest world size of a sharded pass (me_create / me_set_shard refuse more): every rank owns one slot of the per-rank
+ * moments below, so that the single SUM all-reduce of the accumulators gathers them. */
+#define ME_MAX_WORLD 64
+
+/* sum-reducible partial accumulators of one direction (int64 block first, then fp64 block).  sigma needs the spread of d
+ * over ALL kept pairs; sum(d) and sum(d^2) lose u (mean / spread)^2 of it to cancellation, so every rank also reports the
+ * count, mean and sum of squared deviations (M2) of its kept d in its own slot [rank], zeros elsewhere, and
+ * me_nn_finalize merges the slots (Chan et al.).  Accumulators whose slots do not account for all n_corr pairs (filled by
+ * a caller that sets the sums only) are finalised from sum_d_all / sum_d2_all instead. */
 #define ME_NN_ACCUM_I64 9
-#define ME_NN_ACCUM_F64 13
+#define ME_NN_ACCUM_F64 (13 + 3 * ME_MAX_WORLD)
 typedef struct {
   int64_t n_query;           /* queries evaluated by this rank                             */
   int64_t n_corr;            /* kept pairs |C|                                             */
@@ -100,9 +108,12 @@ typedef struct {
   int64_t n_far;             /* queries resolved by the far (ring-expansion) kernel        */
   double  sum_d[5];          /* sum of d   over pairs with d <= tau_k (mean_vec)           */
   double  sum_d2[5];         /* sum of d^2 over pairs with d <= tau_k (rmse_vec)           */
-  double  sum_d_all;         /* sum of d   over all kept pairs  (sigma closed form)        */
+  double  sum_d_all;         /* sum of d   over all kept pairs                             */
   double  sum_d2_all;        /* sum of d^2 over all kept pairs                             */
   double  sum_nn_dist;       /* sum of sqrt(d2_nn) over ALL queries (full CD)              */
+  double  rank_n[ME_MAX_WORLD];     /* kept pairs of rank r (= n_corr of that rank)        */
+  double  rank_mean[ME_MAX_WORLD];  /* mean of d over them                                 */
+  double  rank_m2[ME_MAX_WORLD];    /* sum of (d - rank_mean)^2 over them                  */
 } me_nn_accum;
 
 typedef struct {             /* == est_gt_results / gt_est_results (map_eval.cpp:1140-1144) */

@@ -128,3 +128,35 @@ def test_finalizers_match_the_reference_formulas(L):
     m.n_valid, m.sum_entropy, m.min_entropy, m.max_entropy = 0, 0.0, np.inf, -np.inf
     assert L.me_mme_finalize(C.byref(m), 10, C.byref(r)) == 0
     assert r.mme == 0.0 and np.isnan(r.min_abs_entropy)
+
+
+def test_finalizer_merges_the_rank_moments(L):
+    """me_nn_finalize on per-rank (n, mean, M2) slots: sigma from the merged moments, to the exact two-pass value, where the
+    closed form on sum(d) and sum(d^2) of the same distances loses it to cancellation (a cluster 1e-9 m wide around
+    2.6 cm, split over three ranks)"""
+    from fractions import Fraction
+    rng = np.random.RandomState(4)
+    nd = 0.026 + 1e-9 * rng.rand(3000)
+    tau = [1.0, 0.026 + 5e-10, 0.02, 1.0, 1.0]
+    a = A.me_nn_accum()
+    a.n_query = a.n_corr = len(nd)
+    for k, t in enumerate(tau):
+        m = nd <= t
+        a.n_inlier[k], a.sum_d[k], a.sum_d2[k] = int(m.sum()), nd[m].sum(), (nd[m] ** 2).sum()
+    a.sum_d_all, a.sum_d2_all = nd.sum(), (nd ** 2).sum()
+    for r, part in enumerate(np.array_split(nd, 3)):
+        a.rank_n[5 * r], a.rank_mean[5 * r] = len(part), part.mean()
+        a.rank_m2[5 * r] = ((part - part.mean()) ** 2).sum()
+    p = A.make_nn_params(tau, 1.0, pairing=A.ME_PAIRING_GEOMETRIC, directions=1)
+    out = A.me_nn_result()
+    assert L.me_nn_finalize(C.byref(p), C.byref(a), None, len(nd), 1, C.byref(out)) == 0
+    F = [Fraction(x) for x in nd]
+    for k in range(5):
+        mean = Fraction(out.est_to_gt.mean[k])
+        exact = float(sum((f - mean) ** 2 for f in F) / len(F)) ** 0.5
+        assert abs(out.est_to_gt.sigma[k] - exact) <= 1e-10 * exact + 1e3 * 2.0 ** -53 * 0.026, k
+    # the same accumulator without its moments falls back to the closed form, which is far off here
+    for r in range(3):
+        a.rank_n[5 * r] = a.rank_mean[5 * r] = a.rank_m2[5 * r] = 0.0
+    assert L.me_nn_finalize(C.byref(p), C.byref(a), None, len(nd), 1, C.byref(out)) == 0
+    assert abs(out.est_to_gt.sigma[0] - exact) > 1e3 * 2.0 ** -53 * 0.026

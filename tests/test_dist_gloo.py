@@ -16,7 +16,7 @@ from cloud_map_evaluation_b200 import _lib, synth
 from cloud_map_evaluation_b200 import dist as mdist
 
 
-def _partial_nn(query, ref, qb, qe, tau, R):
+def _partial_nn(query, ref, qb, qe, tau, R, slot=None):
     from oracle import oracle as O
     a = A.me_nn_accum()
     q = query[qb:qe]
@@ -33,10 +33,13 @@ def _partial_nn(query, ref, qb, qe, tau, R):
         m = nd <= t
         a.n_inlier[k], a.sum_d[k], a.sum_d2[k] = int(m.sum()), float(nd[m].sum()), float(sq[m].sum())
     a.sum_d_all, a.sum_d2_all, a.sum_nn_dist = float(nd.sum()), float(sq.sum()), float(np.sqrt(d2).sum())
+    if slot is not None and len(nd):      # this rank's (n, mean, M2), the other slots stay 0: the SUM gathers them
+        a.rank_n[slot], a.rank_mean[slot] = len(nd), float(nd.mean())
+        a.rank_m2[slot] = float(((nd - nd.mean()) ** 2).sum())
     return a
 
 
-def _worker(rank, world, port, out_dir):
+def _worker(rank, world, port, out_dir, moments=False):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
@@ -47,8 +50,9 @@ def _worker(rank, world, port, out_dir):
         p = A.make_nn_params(tau, 1.0, pairing=A.ME_PAIRING_GEOMETRIC)
         eb, ee = mdist.shard_range(len(est), rank, world)
         gb, ge = mdist.shard_range(len(gt), rank, world)
-        nn_e = _partial_nn(est, gt, eb, ee, tau, 1.0)
-        nn_g = _partial_nn(gt, est, gb, ge, tau, 1.0)
+        slot = rank if moments else None
+        nn_e = _partial_nn(est, gt, eb, ee, tau, 1.0, slot)
+        nn_g = _partial_nn(gt, est, gb, ge, tau, 1.0, slot)
         # MME partial: entropies of this rank's points from the oracle's per-point output
         _, ent = O.eval_mme(est, 0.1, 10, want_entropies=True)
         mine = ent[eb:ee]
@@ -65,6 +69,8 @@ def _worker(rank, world, port, out_dir):
             exp = O.eval_nn(est, gt, p)
             emme = O.eval_mme(est, 0.1, 10)
             assert nn_e.n_query == len(est) and nn_g.n_query == len(gt)
+            if moments:
+                assert sum(nn_e.rank_n) == nn_e.n_corr and sum(nn_g.rank_n) == nn_g.n_corr
             for d in ("est_to_gt", "gt_to_est"):
                 g, e = getattr(res, d), getattr(exp, d)
                 assert list(g.n_inlier) == list(e.n_inlier) and g.n_corr == e.n_corr
@@ -92,6 +98,21 @@ def test_sharded_accumulators_allreduce_gloo(world, tmp_path):
     mp.spawn(_worker, args=(world, port, str(tmp_path)), nprocs=world, join=True)
     assert os.path.exists(tmp_path / "ok")
 
+
+
+@pytest.mark.parametrize("world", [2, 3])
+def test_sharded_moments_allreduce_gloo(world, tmp_path):
+    """the per-rank (n, mean, M2) slots through the same single SUM all-reduce: me_nn_finalize merges them into sigma"""
+    if not os.path.exists(_lib.LIB_PATH):
+        import __graft_entry__ as g
+        g.build()
+    from oracle import oracle as O
+    O.build()
+    with socket.socket() as s:
+        s.bind(("127.0.0.1", 0))
+        port = s.getsockname()[1]
+    mp.spawn(_worker, args=(world, port, str(tmp_path), True), nprocs=world, join=True)
+    assert os.path.exists(tmp_path / "ok")
 
 def test_pack_unpack_roundtrip():
     a, b, m = A.me_nn_accum(), A.me_nn_accum(), A.me_mme_accum()

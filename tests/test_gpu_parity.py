@@ -532,14 +532,15 @@ def test_device_resident_accumulators_equal_the_host_path(api, O):
         ctx.eval_mme_accum_device(A.ME_CLOUD_GT, cfg["nn_radius"], 5)
         ctx.eval_nn_accum_device(p)
         ptr, n_sum, n_max = ctx.accum_block()
-        assert ptr and n_sum == 58 and n_max == 4
+        assert ptr and n_sum == 2 * (A.ME_NN_ACCUM_I64 + A.ME_NN_ACCUM_F64) + 14 and n_max == 4
         e2, g2, (m_e2, m_g2) = ctx.accum_fetch(want_mme=(True, True))
     for a, b in ((e, e2), (g, g2)):
         da, db = A.struct_to_dict(a), A.struct_to_dict(b)
         for k in ("n_query", "n_corr", "n_inlier", "n_ub", "n_far"):
             assert da[k] == db[k], k
-        for k in ("sum_d", "sum_d2", "sum_d_all", "sum_d2_all", "sum_nn_dist"):
+        for k in ("sum_d", "sum_d2", "sum_d_all", "sum_d2_all", "sum_nn_dist", "rank_mean", "rank_m2"):
             np.testing.assert_allclose(da[k], db[k], rtol=1e-12)
+        assert da["rank_n"] == db["rank_n"] == [da["n_corr"]] + [0.0] * (A.ME_MAX_WORLD - 1)
     for a, b in ((m_e, m_e2), (m_g, m_g2)):
         assert (a.n_query, a.n_valid) == (b.n_query, b.n_valid)
         np.testing.assert_allclose([a.sum_entropy, a.min_entropy, a.max_entropy], [b.sum_entropy, b.min_entropy, b.max_entropy], rtol=1e-12)
