@@ -64,6 +64,16 @@ def kernel_bit_names(mask):
     return {k for k, v in KERNEL_BITS.items() if mask >> v & 1}
 
 
+# enum me_trace_event: data events in the trace mask, above the sweep bits
+ME_TEV_MME_FP64_FINISH = 31
+TRACE_EVENTS = {k: v for k, v in dict(globals()).items() if k.startswith("ME_TEV_")}
+
+
+def trace_event_names(mask):
+    """the ME_TEV_* names set in a me_kernel_trace mask"""
+    return {k for k, v in TRACE_EVENTS.items() if mask >> v & 1}
+
+
 ME_N_STAGE_TIMES = 9
 STAGE_NAMES = ("grid_est", "grid_gt", "nn_est_to_gt", "nn_gt_to_est", "mme_est", "mme_gt",
                "voxel_moments", "awd", "scs")

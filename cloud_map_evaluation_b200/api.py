@@ -288,9 +288,10 @@ class MapEvalB200:
     def launch_count(self):
         return int(self._L.me_launch_count(self._ctx))
 
-    def kernel_trace(self, reset=True):
-        """(set of ME_KBIT_* names of the sweep paths run since creation or the last reset, (CAP, U) of the last
-        mme_rows_kernel or None)"""
+    def kernel_trace(self, reset=True, events=False):
+        """(set of ME_KBIT_* names of the sweep paths run since creation or the last reset — with events=True also the
+        ME_TEV_* names of the data events —, (CAP, U) of the last mme_rows_kernel or None)"""
         mask, cfg = C.c_uint64(0), C.c_int32(0)
         self._check(self._L.me_kernel_trace(self._ctx, C.byref(mask), C.byref(cfg), 1 if reset else 0))
-        return A.kernel_bit_names(mask.value), ((cfg.value >> 8, cfg.value & 255) if cfg.value else None)
+        names = A.kernel_bit_names(mask.value) | (A.trace_event_names(mask.value) if events else set())
+        return names, ((cfg.value >> 8, cfg.value & 255) if cfg.value else None)

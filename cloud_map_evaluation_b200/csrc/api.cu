@@ -68,6 +68,7 @@ static void free_cloud(Cloud &c) {
   if (c.d_nn_sq) cudaFree(c.d_nn_sq);
   if (c.d_entropy) cudaFree(c.d_entropy);
   if (c.d_entropy_caller) cudaFree(c.d_entropy_caller);
+  if (c.d_fp64_list) cudaFree(c.d_fp64_list);
   if (c.d_normal) cudaFree(c.d_normal);
   if (c.d_tiles) cudaFree(c.d_tiles);
   if (c.d_tile_pos) cudaFree(c.d_tile_pos);

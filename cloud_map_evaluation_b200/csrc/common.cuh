@@ -112,6 +112,8 @@ struct Cloud {
   double *d_entropy_caller = nullptr;   // caller order, kept when the sweep ran on a solo lattice (which the next build replaces)
   long long cap_entropy_caller = 0;
   bool entropy_caller_valid = false;
+  uint32_t *d_fp64_list = nullptr;      // MME: sorted indices of the queries left to the fp64 finish
+  long long cap_fp64_list = 0;
   double *d_normal = nullptr;           // caller order, 3 fp64 per point: normals (me_set_normals / me_estimate_normals, averaged
   long long cap_normal = 0;             // by me_voxel_downsample); the working k-NN normals of generalized ICP when !normal_valid
   bool normal_valid = false;

@@ -17,6 +17,7 @@
 //                       the fp32 error band (the neighbour COUNT is bit-exact), fp64 moment accumulation.
 //   mme_plane_kernel    (4..15 rings): the same walk with a run table of one dz plane at a time.
 //   mme_kernel          (> 15 rings): nested row walk with fp64 tests on the 32-byte records.
+//   mme_fp64_finish_kernel: the queries the fp32-offset kernels could not certify (thin surfaces), walked again as mme_kernel.
 // run_mme picks the lattice per radius: when the radius spans more than 3 cells of the shared lattice the cloud is laid
 // out on a lattice of its own with h = r/2 for this sweep.  Variants that were measured slower and dropped: shared-memory
 // tile + TMA staging, 16-byte table entries, software prefetch, plane tables at R = 2.
@@ -30,15 +31,22 @@
 namespace me {
 
 static constexpr int kThreads = 128;
+// trace events sit above the sweep bits, in the 32-bit device word
+static_assert((int)ME_KBIT_COUNT <= (int)ME_TEV_MME_FP64_FINISH && (int)ME_TEV_MME_FP64_FINISH < 32, "trace event bit");
+// an fp32-offset kernel finishes a query in fp64 when its certificate of the offsets' effect on the entropy exceeds this
+// (nats); below it the certified error is at most this (a float32 emulation of the offsets stays 13-330 times below the
+// certificate, tests/test_exact_mme.py)
+static constexpr double kFp64FinishNats = 1e-3;
 
 struct MmeAcc {
   unsigned long long n_valid, n_query;
   double sum;
   unsigned long long min_enc, max_enc;   // ordered encodings of the extrema over entropies != 0
+  unsigned long long n_fp64;             // queries an fp32-offset kernel left to mme_fp64_finish_kernel
 };
 
 __global__ void mme_init_kernel(MmeAcc *a) {
-  a->n_valid = 0; a->n_query = 0; a->sum = 0.0;
+  a->n_valid = 0; a->n_query = 0; a->sum = 0.0; a->n_fp64 = 0;
   a->min_enc = enc_ordered(INFINITY); a->max_enc = enc_ordered(-INFINITY);
 }
 
@@ -60,8 +68,29 @@ struct ThreadStats {
   __device__ __forceinline__ void init() { sum = 0.0; mn = INFINITY; mx = -INFINITY; valid = 0; queries = 0; }
 };
 
-// map_eval.cpp:1675-1697 for one query
-__device__ __forceinline__ double finish_entropy(const Moments &m, int min_neighbors, ThreadStats &t) {
+struct MmeConst {
+  float h, inv_h;            // cell edge and its inverse
+  float rc2;                 // (r/h)^2 with slack: row / cell pruning is conservative, the point test decides
+  float r2_lo, r2_hi;        // fp32 screening band around r^2
+  double r2;                 // exact r^2
+  int min_neighbors;
+  int dimx, dimy, dimz;
+  Owned own;                 // slab layout: the planes whose points this rank evaluates (the halo points are neighbours only)
+  double E2;                 // square of the bound E of the fp32 offsets' error per axis
+  double s2_max;             // fp64 finish when s^2 exceeds this (the s at which 0.5 |ln(1 - rho')| = kFp64FinishNats)
+  uint32_t *fp64_list;       // sorted indices of the queries left to the fp64 finish (count: MmeAcc::n_fp64)
+};
+
+// map_eval.cpp:1675-1697 for one query.
+// CERT (the fp32-offset kernels): the moments were accumulated from offsets that carry an error of up to C.E per axis.
+// To first order that moves ln det by at most rho = 2 sqrt(3) s + 3 s^2, s = E sqrt(k / (k - 1) * tr adj(C) / det) (rotation
+// invariant: on a surface of normal noise sigma it grows like E / sigma); rho' = rho + 3 rho^2 bounds the quadratic terms.
+// rho' grows with s, so the test is s^2 <= s2_max, cleared of the square root and the division.  A query whose
+// certificate exceeds kFp64FinishNats — thin surfaces, det <= 0 — is not finished here: its sorted index goes to
+// C.fp64_list, and mme_fp64_finish_kernel evaluates it again from fp64 offsets (tests/exact_ref.py states the bounds).
+template <bool CERT = false>
+__device__ __forceinline__ double finish_entropy(const Moments &m, int min_neighbors, ThreadStats &t,
+                                                 const MmeConst *C = nullptr, long long i = 0, MmeAcc *acc = nullptr) {
   t.queries++;
   if (m.cnt == 0) return 0.0;
   const long long k = (long long)m.cnt - 1;                 // erase(begin()): the query itself (:1672-1673)
@@ -75,7 +104,16 @@ __device__ __forceinline__ double finish_entropy(const Moments &m, int min_neigh
   c[5] = (m.syz - m.s1y * m.s1z / kd) * inv;
   c[8] = (m.szz - m.s1z * m.s1z / kd) * inv;
   c[3] = c[1]; c[6] = c[2]; c[7] = c[5];
-  const double e = 0.5 * log(2 * M_PI * M_E * det3(c));     // map_eval.cpp:1434 / :1656
+  const double det = det3(c);
+  if (CERT) {
+    const double adj = (c[0] * c[4] - c[1] * c[1]) + (c[0] * c[8] - c[2] * c[2]) + (c[4] * c[8] - c[5] * c[5]);
+    // s^2 = E^2 k / (k - 1) adj / det <= s2_max, with det > 0; NaN fails the test and is listed too
+    if (!(det > 0.0 && C->E2 * kd * adj <= C->s2_max * (kd - 1.0) * det)) {
+      C->fp64_list[atomicAdd(&acc->n_fp64, 1ull)] = (uint32_t)i;
+      return 0.0;
+    }
+  }
+  const double e = 0.5 * log(2 * M_PI * M_E * det);         // map_eval.cpp:1434 / :1656
   if (isnan(e) || isinf(e)) return 0.0;
   t.sum += e; t.valid++;
   if (e != 0.0) { t.mn = fmin(t.mn, e); t.mx = fmax(t.mx, e); }
@@ -166,6 +204,30 @@ mme_kernel(const P4 *__restrict__ S, long long q_begin, long long q_end, CellInd
   flush_stats(ts, acc);
 }
 
+// the queries an fp32-offset kernel listed (finish_entropy<true>): walked again with fp64 offsets (the differences of the
+// records, as mme_kernel), finished and folded into the accumulators.  The count is read on the device, so the launch
+// needs no host round trip; with an empty list it returns at once.  The listing kernel has counted the queries.
+__global__ void __launch_bounds__(kThreads)
+mme_fp64_finish_kernel(const P4 *__restrict__ S, const uint32_t *__restrict__ list, CellIndex I, Lattice L, double r2,
+                       float rc2, int rings, int min_neighbors, double *__restrict__ entropy_sorted, MmeAcc *__restrict__ acc,
+                       unsigned int *trace) {
+  const unsigned long long n = *(volatile unsigned long long *)&acc->n_fp64;
+  if (n == 0) return;
+  if (blockIdx.x == 0 && threadIdx.x == 0) atomicOr(trace, 1u << ME_TEV_MME_FP64_FINISH);
+  ThreadStats ts;
+  ts.init();
+  for (unsigned long long t = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; t < n;
+       t += (unsigned long long)gridDim.x * blockDim.x) {
+    const uint32_t i = list[t];
+    Moments m;
+    m.init();
+    walk_global(load_p4(S + i), S, I, L, r2, rc2, rings, m);
+    entropy_sorted[i] = finish_entropy(m, min_neighbors, ts);
+  }
+  ts.queries = 0;
+  flush_stats(ts, acc);
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // flat kernel (rings <= 3): the dominant kernel of the pass.
 //
@@ -182,15 +244,6 @@ mme_kernel(const P4 *__restrict__ S, long long q_begin, long long q_end, CellInd
 // raw records with the reference's operation order (nanoflann: d2 < r2, strict), so the neighbour COUNT — and with it
 // the k >= min_neighbors validity test — is bit-exact.  Accepted offsets are accumulated in fp64.
 // ---------------------------------------------------------------------------------------------------------------
-struct MmeConst {
-  float h, inv_h;            // cell edge and its inverse
-  float rc2;                 // (r/h)^2 with slack: row / cell pruning is conservative, the point test decides
-  float r2_lo, r2_hi;        // fp32 screening band around r^2
-  double r2;                 // exact r^2
-  int min_neighbors;
-  int dimx, dimy, dimz;
-  Owned own;                 // slab layout: the planes whose points this rank evaluates (the halo points are neighbours only)
-};
 
 // squared gap (in cells) between a point at u in [0,1) of its cell and the cell d steps away on the same axis
 __device__ __forceinline__ float gap2(int d, float u) {
@@ -276,7 +329,7 @@ mme_flat_kernel(const P4 *__restrict__ S, const float4 *__restrict__ rel, long l
       float y0, z0;
       while (w.next(T, tid, h, qr.y, qr.z, R, j0, y0, z0)) process(__ldg(rel + j0), y0, z0, j0);
     }
-    entropy_sorted[i] = finish_entropy(m, C.min_neighbors, ts);
+    entropy_sorted[i] = finish_entropy<true>(m, C.min_neighbors, ts, &C, i, acc);
   }
   flush_stats(ts, acc);
 }
@@ -415,7 +468,7 @@ mme_rows_kernel(const P4 *__restrict__ S, const float4 *__restrict__ rel, long l
       if (++dy > R) { dy = -R; ++dz; }
     }
     drain();
-    const double ent = finish_entropy(m, C.min_neighbors, ts);
+    const double ent = finish_entropy<true>(m, C.min_neighbors, ts, &C, i, acc);      // dead lanes have no moments
     if (live) entropy_sorted[i] = ent;
     else ts.queries--;       // finish_entropy counted the dead lane
   }
@@ -530,7 +583,7 @@ mme_plane_kernel(const P4 *__restrict__ S, const float4 *__restrict__ rel, long 
         if (v1) process(c1, y1, j1);
       }
     }
-    entropy_sorted[i] = finish_entropy(m, C.min_neighbors, ts);
+    entropy_sorted[i] = finish_entropy<true>(m, C.min_neighbors, ts, &C, i, acc);
   }
   flush_stats(ts, acc);
 }
@@ -643,6 +696,15 @@ int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors, me_mme_acc
       C.min_neighbors = min_neighbors;
       C.dimx = c.lat.dims[0]; C.dimy = c.lat.dims[1]; C.dimz = c.lat.dims[2];
       C.own = owned_of(c);
+      C.E2 = E * E;
+      {      // rho' = rho + 3 rho^2 at 0.5 |ln(1 - rho')| = tau, then rho = 2 sqrt(3) s + 3 s^2 solved for s
+        const double rho_p = -std::expm1(-2.0 * kFp64FinishNats);
+        const double rho = (std::sqrt(1.0 + 12.0 * rho_p) - 1.0) / 6.0;
+        const double s = (std::sqrt(12.0 + 12.0 * rho) - 2.0 * std::sqrt(3.0)) / 6.0;
+        C.s2_max = s * s;
+      }
+      ME_TRY(ensure(ctx, (void **)&c.d_fp64_list, &c.cap_fp64_list, qe - qb, sizeof(uint32_t)));
+      C.fp64_list = c.d_fp64_list;
       // default: the run-table walk; ME_MME_KERNEL=rows selects the warp-synchronous row walk with deferred accumulation
       // (6.2 ms against 5.3 ms for C3's sweep on one H100: half of its issue slots idle while the longest run of a row
       // finishes)
@@ -657,6 +719,17 @@ int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors, me_mme_acc
       else if (rings == 2) ME_TRY(launch_flat<2>(ctx, c, qb, qe, C, acc));
       else if (rings == 3) ME_TRY(launch_flat<3>(ctx, c, qb, qe, C, acc));
       else ME_TRY(launch_plane(ctx, c, qb, qe, C, rings, acc));
+      // the listed queries (thin surfaces: certificate above kFp64FinishNats) again with fp64 offsets
+      mme_fp64_finish_kernel<<<ctx->sm_count * 4, kThreads, 0, ctx->stream>>>(c.d_sorted, c.d_fp64_list, index_of(c), c.lat,
+                                                                             radius * radius, rc2, rings, min_neighbors,
+                                                                             c.d_entropy, acc, ctx->d_trace);
+      ME_LAUNCH_CHECK(ctx);
+      if (getenv("ME_DEBUG_MME")) {
+        unsigned long long nf = 0;
+        ME_CUDA(ctx, cudaMemcpyAsync(&nf, &acc->n_fp64, sizeof(nf), cudaMemcpyDeviceToHost, ctx->stream));
+        ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        fprintf(stderr, "[mapeval] mme: rank %d cloud %d: %llu of %lld queries finished in fp64\n", ctx->rank, which, nf, qe - qb);
+      }
     } else {
       const int blocks = (int)std::min<long long>((qe - qb + kThreads - 1) / kThreads, (long long)ctx->sm_count * 64);
       mme_kernel<<<blocks, kThreads, 0, ctx->stream>>>(c.d_sorted, qb, qe, index_of(c), c.lat, radius * radius, rc2, rings,

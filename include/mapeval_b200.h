@@ -358,6 +358,11 @@ enum me_kernel_bit {
   ME_KBIT_SCS_RT_UNCACHED = 21,    /* scs_kernel, run-time radius too large for the per-lane cache         */
   ME_KBIT_COUNT = 22
 };
+/* Data events of the same mask, above the sweep bits.  They record what the data made a sweep do rather than which sweep
+ * ran, so they are not part of enum me_kernel_bit; they are set on the device only when a query reaches the path. */
+enum me_trace_event {
+  ME_TEV_MME_FP64_FINISH = 31      /* an fp32-offset MME sweep left queries to mme_fp64_finish_kernel (thin surfaces)  */
+};
 /* *mask (nullable) = the trace since creation or the last reset; *mme_rows_cfg (nullable) = (CAP << 8) | U of the last
  * mme_rows_kernel<R, CAP, U> launched (ring slots, candidates per iteration), 0 if none.  reset != 0 clears both.
  * Synchronises the context's stream. */

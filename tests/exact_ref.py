@@ -28,6 +28,7 @@ sum_k A_kk / L_kk + S1_kk sqrt(S2_kk) / L1_kk over the two Cholesky factorisatio
 A = L1 S2 L1^T) is their first-order sensitivity to a relative perturbation u of their inputs: with eigenvalues clamped at
 1e-6 next to eigenvalues of ~10 it exceeds tr_sum by three orders, and no fp64 evaluation of the quirk does better.
 """
+import math
 from fractions import Fraction
 
 import mpmath as mp
@@ -295,3 +296,216 @@ def scs_exact(w_table, radius=5):
             total += mp.sqrt(var) / mean
             count += 1
         return (total / count if count else mp.nan), count
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# mean map entropy (map_eval.cpp:1433-1436, 1438-1737)
+#
+# Neighbours are the reference's fp64 decisions, reproduced in fp64: d2 = ((dx dx) + dy dy) + dz dz (d2_kd, nanoflann),
+# strict d2 < r^2, the query itself removed once (duplicates of it stay), valid iff k >= min_neighbors.  The centred
+# covariance sum (p - pbar)(p - pbar)^T / (k - 1) of the fp64 coordinates, its determinant and its adjugate are exact
+# rationals; the entropy 0.5 ln(2 pi e det) is taken with mpmath.  det <= 0 rejects the point (the isnan / isinf test of
+# map_eval.cpp:1692, :1574, :1472 / :1505).
+#
+# B64, the bound an fp64 evaluation of the neighbourhood meets (the reference's centred product, or the library's moments
+# about the query, cov = (S2 - S1 S1^T / k) / (k - 1)): every covariance entry is within
+#   dC_ij = C_MME u (k + 2) (sum_p |d_pi| |d_pj| + |S1_i S1_j| / k) / (k - 1),   d_p = p - q,
+# the gamma_{k+2} bound of a recursive sum of k products and the centring, with a margin of C_MME.  The permanent
+# majorises the determinant's change: |det(C + D) - det C| <= per(|C| + dC) - per(|C|) = ddet.  A query is determined when
+# ddet < det / 2 (its validity is then decided, and B64 = 0.5 ddet / (det - ddet) + C_BOUND u (1 + |e|)), or when
+# det = ddet = 0 (an exactly flat or straight neighbourhood along the axes: rejected by every fp64 evaluation).
+# C_MME is deliberately not C_BOUND: with 10^3 the bound would be 0.02 nats on a 1 um plane and could not tell an fp64
+# evaluation (2e-7) from one built on fp32 offsets (5e-4).
+#
+# B32(E), the first-order certificate of an evaluation whose offsets carry an error of at most E per axis (the library's
+# fp32-offset sweeps): with q = tr adj(C) / det = sum 1 / lambda_i and s = E sqrt(k / (k - 1)) sqrt(q),
+#   rho = 2 sqrt(3) s + 3 s^2,  rho' = rho + 3 rho^2,  B32 = 0.5 |ln(1 - rho')|  (undetermined when rho' >= 1/2).
+# It is rotation invariant: on a tilted plane of normal noise sigma it grows like E / sigma, where entrywise bounds grow
+# like E r / sigma^2.  mme_fp32_certificate evaluates it on any covariance, the exact one or a kernel's own.
+# ---------------------------------------------------------------------------------------------------------------
+C_MME = 4.0
+TAU_FP64 = 1e-3       # nats: a fp32-offset sweep finishes a query in fp64 when its certificate exceeds this
+
+
+def d2_kd(q, p):
+    """squared distances of (n, 3) fp64 differences q - p in nanoflann's order ((dx dx) + dy dy) + dz dz"""
+    d = np.asarray(q, np.float64) - np.asarray(p, np.float64)
+    return (d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1]) + d[..., 2] * d[..., 2]
+
+
+def mme_neighbours(pts, r, le=False):
+    """per query the indices of its neighbours: d2_kd < r^2 (or <= with le, a deliberately wrong variant), the query itself
+    removed once"""
+    from scipy.spatial import cKDTree
+    pts = np.asarray(pts, np.float64)
+    r2 = r * r
+    cand = cKDTree(pts).query_ball_point(pts, r * (1 + 1e-6) + 1e-300)
+    out = []
+    for i, c in enumerate(cand):
+        c = np.asarray(sorted(c), dtype=np.int64)
+        d2 = d2_kd(pts[i], pts[c])
+        c = c[(d2 <= r2) if le else (d2 < r2)]
+        out.append(c[c != i])
+    return out
+
+
+def _permanent_growth(a, d):
+    """per(a + d) - per(a) for non-negative 3x3 a, d, without cancellation"""
+    tot = 0.0
+    for s in ((0, 1, 2), (0, 2, 1), (1, 0, 2), (1, 2, 0), (2, 0, 1), (2, 1, 0)):
+        x = [a[i][s[i]] for i in range(3)]
+        y = [d[i][s[i]] for i in range(3)]
+        tot += (y[0] * x[1] * x[2] + x[0] * y[1] * x[2] + x[0] * x[1] * y[2] + y[0] * y[1] * x[2] + y[0] * x[1] * y[2]
+                + x[0] * y[1] * y[2] + y[0] * y[1] * y[2])
+    return tot
+
+
+def mme_fp32_certificate(cov, k, E):
+    """B32 (module notes) of a 3x3 covariance (floats or Fractions) of k neighbours under an offset error E per axis;
+    inf when undetermined (rho' >= 1/2, or det <= 0)"""
+    c = [[float(cov[a][b]) for b in range(3)] for a in range(3)]
+    det = float(np.linalg.det(np.array(c))) if not isinstance(cov[0][0], Fraction) else float(_det3(cov))
+    adj = (c[0][0] * c[1][1] - c[0][1] ** 2) + (c[0][0] * c[2][2] - c[0][2] ** 2) + (c[1][1] * c[2][2] - c[1][2] ** 2)
+    if not det > 0 or not adj > 0:
+        return float("inf")
+    s = E * math.sqrt(k / (k - 1) * adj / det)
+    rho = 2 * math.sqrt(3) * s + 3 * s * s
+    rho += 3 * rho * rho
+    return 0.5 * abs(math.log1p(-rho)) if rho < 0.5 else float("inf")
+
+
+def _det3(m):
+    return (m[0][0] * (m[1][1] * m[2][2] - m[1][2] * m[2][1]) - m[0][1] * (m[1][0] * m[2][2] - m[1][2] * m[2][0])
+            + m[0][2] * (m[1][0] * m[2][1] - m[1][1] * m[2][0]))
+
+
+def mme_point(pts, i, nb, min_neighbors, ints=None, drop_query=True, divisor=None):
+    """the exact entropy of query i with neighbours nb: dict(k, valid, determined, e (fp64 of the exact value, 0.0 when
+    rejected), cov (3x3 Fractions or None), b64).  ints: to_ints(pts) (pass it to avoid recomputing).  drop_query=False
+    and divisor='k' are deliberately wrong variants for the tests' teeth."""
+    pts = np.asarray(pts, np.float64)
+    k = len(nb)
+    out = dict(k=k, valid=False, determined=True, e=0.0, cov=None, b64=0.0)
+    if k < min_neighbors:
+        return out
+    if not drop_query:
+        nb = np.concatenate([[i], nb])
+    if ints is None:
+        ints = to_ints(pts)
+    I, ex = ints
+    X = [I[3 * j:3 * j + 3] for j in nb]
+    n = len(X)
+    den = (n - 1) if divisor is None else n
+    S = [sum(x[a] for x in X) for a in range(3)]
+    M = [[n * sum(x[a] * x[b] for x in X) - S[a] * S[b] for b in range(3)] for a in range(3)]
+    scale = _pow2(2 * ex) / (n * den)
+    cov = [[Fraction(M[a][b]) * scale for b in range(3)] for a in range(3)]
+    det = _det3(cov)
+    # the fp64 error bound of the entries, from the offsets to the query
+    d = pts[nb] - pts[i]
+    ad = np.abs(d)
+    s1 = d.sum(0)
+    dC = C_MME * U * (n + 2) * ((ad.T @ ad) + np.abs(np.outer(s1, s1)) / n) / (n - 1)
+    a = [[abs(float(cov[r][c])) for c in range(3)] for r in range(3)]
+    ddet = _permanent_growth(a, dC.tolist())
+    detf = float(det)
+    out["cov"] = cov
+    if det <= 0:
+        out["determined"] = det == 0 and ddet == 0.0
+        return out
+    if not ddet < 0.5 * detf:
+        out["determined"] = False
+        return out
+    with mp.workdps(DPS):
+        e = 0.5 * (mp.log(2 * mp.pi * mp.e) + mp.log(det.numerator) - mp.log(det.denominator))
+    ef = float(e)
+    out.update(valid=True, e=ef, b64=0.5 * ddet / (detf - ddet) + C_BOUND * U * (1 + abs(ef)))
+    return out
+
+
+def mme_exact(pts, r, min_neighbors, E=None, nbs=None):
+    """every query of the cloud: arrays k, valid, determined, e, b64 and (with E) b32 = B32(E) of the exact covariance"""
+    pts = np.asarray(pts, np.float64)
+    nbs = mme_neighbours(pts, r) if nbs is None else nbs
+    ints = to_ints(pts)
+    rows = [mme_point(pts, i, nb, min_neighbors, ints) for i, nb in enumerate(nbs)]
+    res = {f: np.array([p[f] for p in rows]) for f in ("k", "valid", "determined", "e", "b64")}
+    res["cov"] = [p["cov"] for p in rows]
+    if E is not None:
+        res["b32"] = np.array([mme_fp32_certificate(p["cov"], p["k"], E) if p["valid"] else 0.0 for p in rows])
+    res["nbs"] = nbs
+    return res
+
+
+def mme_aggregate_bounds(ex, per_point_bound):
+    """bounds of (n_valid, sum, min/max |e|) given per-point bounds over the valid determined queries: (n_undetermined,
+    bound of sum_entropy, bound of min_abs / max_abs_entropy)"""
+    und = int((~ex["determined"]).sum())
+    v = ex["valid"] & ex["determined"]
+    n = int(v.sum())
+    s_b = float(per_point_bound[v].sum()) + C_BOUND * U * n * float(np.abs(ex["e"][v]).sum())
+    ext_b = float(per_point_bound[v].max()) if n else 0.0
+    return und, s_b, ext_b
+
+
+def mme_summary(ex):
+    """(n_valid, sum, min_abs, max_abs) of the exact per-point values (fp64 of exact sums)"""
+    v = ex["valid"]
+    e = ex["e"][v]
+    s = float(sum((Fraction(x) for x in e), Fraction(0)))
+    nz = e[e != 0]
+    return int(v.sum()), s, (float(np.abs(nz.max())) if len(nz) else np.nan), (float(np.abs(nz.min())) if len(nz) else np.nan)
+
+
+def finish_entropy_fp64(d, min_neighbors):
+    """numpy statement of the library's fp64 finish (mme.cu finish_entropy): the moments of the offsets d (k, 3) about the
+    query, summed in order, cov = (S2 - S1 S1^T / k) / (k - 1), Eigen's cofactor determinant; 0.0 when rejected"""
+    d = np.asarray(d, np.float64)
+    k = len(d)
+    if k < min_neighbors or k < 2:
+        return 0.0
+    s1 = [np.cumsum(d[:, a])[-1] for a in range(3)]
+    s2 = [[np.cumsum(d[:, a] * d[:, b])[-1] for b in range(3)] for a in range(3)]
+    kd, inv = float(k), 1.0 / float(k - 1)
+    c = [[(s2[a][b] - s1[a] * s1[b] / kd) * inv for b in range(3)] for a in range(3)]
+    for a in range(3):
+        for b in range(a):
+            c[a][b] = c[b][a]
+    A = c[0][0] * (c[1][1] * c[2][2] - c[1][2] * c[2][1])
+    B = c[0][1] * (c[1][0] * c[2][2] - c[1][2] * c[2][0])
+    Cc = c[0][2] * (c[1][0] * c[2][1] - c[1][1] * c[2][0])
+    with np.errstate(all="ignore"):
+        e = 0.5 * np.log(2 * np.pi * np.e * ((A - B) + Cc))
+    return 0.0 if not np.isfinite(e) else float(e)
+
+
+def mme_offset_error(h, rings, pts):
+    """E of run_mme: the per-axis error bound of the fp32 offsets on a lattice of edge h searched at `rings` rings"""
+    maxabs = float(np.abs(np.asarray(pts, np.float64)).max())
+    return 1e-7 * (2.0 * rings + 6.0) * h + 4e-15 * maxabs
+
+
+def fp32_offsets(pts, i, nb, h, R):
+    """the flat kernel's offset rebuild of the neighbours nb of query i, emulated in float32 on a lattice of edge h (origin
+    at the cell below the cloud's minimum): rel = fp32(x - cell origin), w = fp32(ix);
+    dx = fma(c.w - q.w, h, c.x - q.x), dy = c.y + fma(dyc - R + R, h, -q.y), dz likewise"""
+    pts = np.asarray(pts, np.float64)
+    o = np.floor(pts.min(0) / h) * h
+    cell = np.floor((pts - o) / h)
+    rel = (pts - (o + cell * h)).astype(np.float32)
+    h32 = np.float32(h)
+    f32 = np.float32
+
+    def fma(a, b, c):                       # float32 fused multiply-add: a * b is exact in fp64
+        return (np.float64(a) * np.float64(b) + np.float64(c)).astype(np.float32)
+
+    q, qc = rel[i], cell[i]
+    c, cc = rel[nb], cell[nb]
+    wq, wc = f32(qc[0]), cc[:, 0].astype(np.float32)
+    dx = fma(wc - wq, h32, c[:, 0] - q[0])
+    cy = fma((cc[:, 1] - qc[1]).astype(np.float32), h32, -q[1])
+    cz = fma((cc[:, 2] - qc[2]).astype(np.float32), h32, -q[2])
+    assert np.all(np.abs(cc - qc) <= R)
+    dy = c[:, 1] + cy
+    dz = c[:, 2] + cz
+    return np.column_stack([dx, dy, dz]).astype(np.float64)

@@ -65,6 +65,21 @@ def test_kernel_bit_enum_mirror_matches_the_header():
     assert A.kernel_bit_names((1 << A.ME_KBIT_NN_TILE) | (1 << A.ME_KBIT_SCS_R5)) == {"ME_KBIT_NN_TILE", "ME_KBIT_SCS_R5"}
 
 
+def test_trace_event_enum_mirror_matches_the_header():
+    """enum me_trace_event of the header and its ctypes mirror: the same names with the same values, above the sweep bits
+    and inside the 32-bit device word; kernel_bit_names leaves them out."""
+    text = open(os.path.join(ROOT, "include", "mapeval_b200.h")).read()
+    body = re.search(r"enum\s+me_trace_event\s*\{(.*?)\};", text, flags=re.S).group(1)
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    declared = {k: int(v) for k, v in re.findall(r"\b(ME_TEV_\w+)\s*=\s*(\d+)", body)}
+    assert declared and len(declared) == body.count("=")
+    assert declared == A.TRACE_EVENTS
+    assert all(A.ME_KBIT_COUNT <= v < 32 for v in declared.values())
+    mask = (1 << A.ME_KBIT_MME_SOLO) | (1 << A.ME_TEV_MME_FP64_FINISH)
+    assert A.kernel_bit_names(mask) == {"ME_KBIT_MME_SOLO"}
+    assert A.trace_event_names(mask) == {"ME_TEV_MME_FP64_FINISH"}
+
+
 def test_no_cpu_fallback_without_a_device(L):
     import torch
     if torch.cuda.is_available():

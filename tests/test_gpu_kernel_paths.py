@@ -90,7 +90,11 @@ MME_SCENES = {
     "on_radius_origin": tuple(MME_SELECTORS),
     "on_radius_far": tuple(MME_SELECTORS),
     "near_flat": tuple(MME_SELECTORS),
+    "thin_plane": ("flat-r2-dense", "flat-r3-sparse", "rows12x2-r1", "plane-r5", "solo"),
 }
+# data events (ME_TEV_*) a scene must raise on the sweeps it runs: on a 1 um plane the fp32 offsets cannot certify the
+# entropies, so every fp32-offset sweep hands its queries to the fp64 finish
+MME_SCENE_EVENTS = {"thin_plane": {"ME_TEV_MME_FP64_FINISH"}}
 # the collinear cloud reaches the generic kernel through its lattice (>= 2^24 cells along x), without a hook
 COLLINEAR_MME_BITS = {"ME_KBIT_MME_GENERIC"}
 SCS_RADII = {5: "ME_KBIT_SCS_R5", 2: "ME_KBIT_SCS_RT_CACHED", 7: "ME_KBIT_SCS_RT_UNCACHED"}
@@ -233,6 +237,16 @@ def _mme_scene(name):
         a, b = np.array([0.8, 0.36, 0.48]), np.array([-0.6, 0.48, 0.64])
         pts = u[:, None] * a + v[:, None] * b + w[:, None] * np.cross(a, b) + np.array([731.25, -1204.5, 88.0])
         return _f32(pts), 0.1, 5, 2e-6
+    if name == "thin_plane":
+        # the near-flat plane with 1 um of normal noise
+        n = 40_000
+        idx = np.arange(n, dtype=np.uint64)
+        u = synth.uniform24(78, idx, 0).astype(np.float64) * 2.0
+        v = synth.uniform24(78, idx, 1).astype(np.float64) * 2.0
+        w = 1e-6 * synth.gaussian(78, idx, 8)
+        a, b = np.array([0.8, 0.36, 0.48]), np.array([-0.6, 0.48, 0.64])
+        pts = u[:, None] * a + v[:, None] * b + w[:, None] * np.cross(a, b) + np.array([731.25, -1204.5, 88.0])
+        return np.ascontiguousarray(pts), 0.1, 10, RTOL_ENT
     if name == "collinear":
         est = _collinear()[0]
         return est, 2.5e-6, 10, RTOL_ENT
@@ -347,9 +361,12 @@ def test_mme_kernel(api, scenes, monkeypatch, scene, sel, bits):
         ctx.set_cloud(EST, pts)
         ctx.set_cloud(GT, pts[:10])
         got, ent = ctx.computeMME(EST, r, k, want_entropies=True)
-        trace, rows_cfg = ctx.kernel_trace()
+        trace, rows_cfg = ctx.kernel_trace(events=True)
+    events = trace - set(A.KERNEL_BITS)
+    trace = trace & set(A.KERNEL_BITS)
     _REACHED[case] = trace
     assert trace & MME_SWEEPS == bits, sorted(trace)
+    assert MME_SCENE_EVENTS.get(scene, set()) <= events, sorted(events)
     assert rows_cfg == cfg
     assert (got.n_valid, got.n_total) == (exp.n_valid, exp.n_total)
     np.testing.assert_array_equal(ent != 0, oent != 0)
