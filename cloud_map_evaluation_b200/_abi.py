@@ -30,6 +30,8 @@ ME_LAYOUT_SLAB = 1
 ME_ICP_POINT_TO_POINT = 0
 ME_ICP_POINT_TO_PLANE = 1
 ME_ICP_GENERALIZED = 2
+ME_ICP_BLOCK_P2P = 17
+ME_ICP_BLOCK_NE = 29
 
 # enum me_kernel_bit: bit (1 << value) of the me_kernel_trace mask
 ME_KBIT_NN_ROWS_DENSE = 0

@@ -21,6 +21,7 @@ SYMBOLS = (
     "me_accum_reset", "me_eval_nn_accum_device", "me_eval_mme_accum_device", "me_accum_block", "me_accum_fetch",
     "me_set_layout", "me_layout_active", "me_voxel_begin", "me_voxel_w_table", "me_voxel_finish_accum_device", "me_accum_fetch_awd",
     "me_plan_slab_cut", "me_plan_lattice", "me_kernel_trace",
+    "me_icp_begin", "me_icp_normals_slice", "me_icp_block", "me_icp_step", "me_icp_end", "me_icp_update",
 )
 
 _lib = None
@@ -56,6 +57,12 @@ def load():
     L.me_awd_from_rows.argtypes = [ctx, dp, C.c_int64, C.c_double, C.c_int32, dp, C.POINTER(A.me_awd_result)]
     L.me_icp_point_to_point.argtypes = [ctx, C.c_double, C.c_int32, C.c_double, C.c_double, dp, C.POINTER(A.me_icp_result)]
     L.me_icp.argtypes = [ctx, C.c_int32, C.c_double, C.c_int32, C.c_double, C.c_double, dp, C.POINTER(A.me_icp_result)]
+    L.me_icp_begin.argtypes = [ctx, C.c_int32, C.c_double, C.c_int32, C.c_double, C.c_double, dp]
+    L.me_icp_normals_slice.argtypes = [ctx, C.c_int, C.POINTER(dp), C.POINTER(C.c_int64), C.POINTER(C.c_int32)]
+    L.me_icp_block.argtypes = [ctx, C.POINTER(dp), C.POINTER(C.c_int32)]
+    L.me_icp_step.argtypes = [ctx, C.POINTER(C.c_int32)]
+    L.me_icp_end.argtypes = [ctx, C.POINTER(A.me_icp_result)]
+    L.me_icp_update.argtypes = [C.c_int32, dp, dp, dp]
     L.me_set_normals.argtypes = [ctx, C.c_int, dp, C.c_int64]
     L.me_estimate_normals.argtypes = [ctx, C.c_int, C.c_int32]
     L.me_get_normals.argtypes = [ctx, C.c_int, dp]

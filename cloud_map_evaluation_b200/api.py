@@ -18,6 +18,23 @@ class MapEvalError(RuntimeError):
         self.code = code
 
 
+def icp_update(method, block, center=None):
+    """me_icp_update (host only): the 4x4 update of one ICP iteration from a reduced block (ME_ICP_BLOCK_P2P values about
+    `center` for point-to-point, ME_ICP_BLOCK_NE for point-to-plane / generalized ICP)"""
+    L = _lib.load()
+    b = np.ascontiguousarray(block, dtype=np.float64)
+    n_need = A.ME_ICP_BLOCK_P2P if method == A.ME_ICP_POINT_TO_POINT else A.ME_ICP_BLOCK_NE
+    if b.size != n_need:
+        raise ValueError(f"the block of method {method} has {n_need} values")
+    dp = C.POINTER(C.c_double)
+    c = None if center is None else np.ascontiguousarray(center, dtype=np.float64).reshape(3)
+    out = np.empty(16, np.float64)
+    rc = L.me_icp_update(int(method), b.ctypes.data_as(dp), c.ctypes.data_as(dp) if c is not None else None, out.ctypes.data_as(dp))
+    if rc != A.ME_OK:
+        raise MapEvalError(rc, "me_icp_update")
+    return out.reshape(4, 4)
+
+
 class MapEvalB200:
     """One context = one GPU.  rank/world select this context's contiguous query range (multi-GPU sharding)."""
 
@@ -109,6 +126,41 @@ class MapEvalB200:
         self._check(self._L.me_icp(self._ctx, int(method), float(max_correspondence_distance), int(max_iteration),
                                    float(relative_fitness), float(relative_rmse),
                                    T.ctypes.data_as(C.POINTER(C.c_double)), C.byref(out)))
+        self._keep[A.ME_CLOUD_EST] = None
+        return np.array(list(out.transformation)).reshape(4, 4), out
+
+    # -- registration split at its collective (multi-GPU; dist.icp_distributed runs the loop) -------------------------
+    def icp_begin(self, max_correspondence_distance, T_init=None, max_iteration=30, relative_fitness=1e-6,
+                  relative_rmse=1e-6, method=A.ME_ICP_GENERALIZED):
+        T = np.ascontiguousarray(np.eye(4) if T_init is None else T_init, dtype=np.float64).reshape(16)
+        self._check(self._L.me_icp_begin(self._ctx, int(method), float(max_correspondence_distance), int(max_iteration),
+                                         float(relative_fitness), float(relative_rmse), T.ctypes.data_as(C.POINTER(C.c_double))))
+
+    def icp_normals_slice(self, which):
+        """(device pointer of the world * slice * 3 fp64 normal buffer or None, slice points, pending): pending = True when
+        the caller must all-gather the buffer in place (this rank filled rows [rank * slice, (rank + 1) * slice))"""
+        ptr = C.POINTER(C.c_double)()
+        s, pend = C.c_int64(0), C.c_int32(0)
+        self._check(self._L.me_icp_normals_slice(self._ctx, int(which), C.byref(ptr), C.byref(s), C.byref(pend)))
+        return C.cast(ptr, C.c_void_p).value, s.value, bool(pend.value)
+
+    def icp_block(self):
+        """(device pointer, n_sum) of this rank's partial ICP sums (SUM-all-reduce in place); the first call sweeps"""
+        ptr = C.POINTER(C.c_double)()
+        ns = C.c_int32(0)
+        self._check(self._L.me_icp_block(self._ctx, C.byref(ptr), C.byref(ns)))
+        return C.cast(ptr, C.c_void_p).value, ns.value
+
+    def icp_step(self):
+        """reads the reduced block, updates T, moves and sweeps again; True when the loop is over"""
+        done = C.c_int32(0)
+        self._check(self._L.me_icp_step(self._ctx, C.byref(done)))
+        return bool(done.value)
+
+    def icp_end(self):
+        """est := Transform(original, T); returns (T 4x4, me_icp_result) like performICPRegistration"""
+        out = A.me_icp_result()
+        self._check(self._L.me_icp_end(self._ctx, C.byref(out)))
         self._keep[A.ME_CLOUD_EST] = None
         return np.array(list(out.transformation)).reshape(4, 4), out
 

@@ -229,6 +229,7 @@ void me_destroy(me_ctx *ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   if (ctx->stream) cudaStreamSynchronize(ctx->stream);
+  icp_close(ctx, false);
   if (ctx->copy_stream) { cudaStreamSynchronize(ctx->copy_stream); cudaStreamDestroy(ctx->copy_stream); }
   if (ctx->compute_mark) cudaEventDestroy(ctx->compute_mark);
   free_cloud(ctx->cloud[0]);
@@ -431,6 +432,46 @@ int me_icp(me_ctx *ctx, int32_t method, double max_correspondence_distance, int3
   ME_ENTER(ctx);
   if (!T_init || !out) return fail(ctx, ME_ERR_INVALID, "null argument");
   return run_icp(ctx, method, max_correspondence_distance, max_iteration, relative_fitness, relative_rmse, T_init, out);
+}
+
+int me_icp_begin(me_ctx *ctx, int32_t method, double max_correspondence_distance, int32_t max_iteration, double relative_fitness,
+                 double relative_rmse, const double T_init[16]) {
+  ME_ENTER(ctx);
+  if (!T_init) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return icp_begin(ctx, method, max_correspondence_distance, max_iteration, relative_fitness, relative_rmse, T_init);
+}
+
+int me_icp_normals_slice(me_ctx *ctx, int which, double **device_normals, int64_t *slice_points, int32_t *pending) {
+  ME_ENTER(ctx);
+  if (which != ME_CLOUD_EST && which != ME_CLOUD_GT) return fail(ctx, ME_ERR_INVALID, "bad cloud id");
+  if (!device_normals || !slice_points || !pending) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return icp_normals_slice(ctx, which, device_normals, slice_points, pending);
+}
+
+int me_icp_block(me_ctx *ctx, double **device_block, int32_t *n_sum) {
+  ME_ENTER(ctx);
+  if (!device_block || !n_sum) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return icp_block(ctx, device_block, n_sum);
+}
+
+int me_icp_step(me_ctx *ctx, int32_t *done) {
+  ME_ENTER(ctx);
+  if (!done) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return icp_step(ctx, done);
+}
+
+int me_icp_end(me_ctx *ctx, me_icp_result *out) {
+  ME_ENTER(ctx);
+  if (!out) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return icp_end(ctx, out);
+}
+
+int me_icp_update(int32_t method, const double *block, const double center[3], double update[16]) {
+  if (!block || !update) return ME_ERR_INVALID;
+  if (method != ME_ICP_POINT_TO_POINT && method != ME_ICP_POINT_TO_PLANE && method != ME_ICP_GENERALIZED) return ME_ERR_INVALID;
+  if (method == ME_ICP_POINT_TO_POINT && !center) return ME_ERR_INVALID;
+  icp_update_host(method, block, center, update);
+  return ME_OK;
 }
 
 int me_set_normals(me_ctx *ctx, int which, const double *normals_host, int64_t n) {

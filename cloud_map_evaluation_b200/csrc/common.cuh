@@ -97,6 +97,7 @@ struct Cloud {
   long long shard_b = 0, shard_e = 0;   // this rank's cell-aligned query range (query_shard)
   int shard_rank = -1, shard_world = 0;
   bool shard_valid = false;
+  long long nn_b = 0, nn_e = 0;         // sorted range of the queries the last NN sweep may have filled (others: -2)
   long long max_cell_count = 0;     // points in the fullest cell
   cudaEvent_t upload_done = nullptr;  // recorded on the copy stream after me_set_cloud's H2D
   bool upload_pending = false;
@@ -138,6 +139,26 @@ struct PlanCache {
   bool slab_planned = false, slab_on = false;
   int slab_axis = 0;
   long long slab_k0 = 0, slab_k1 = 0;
+};
+
+// an open registration (me_icp_begin .. me_icp_end, icp.cu): the loop state, identical on every rank
+struct IcpRun {
+  bool open = false;
+  int method = 0, max_iter = 0;
+  double max_dist = 0, rel_fitness = 0, rel_rmse = 0;
+  double T[16];                       // accumulated transformation (T_init included)
+  double c[3] = {0, 0, 0};            // point-to-point: the point the sums are taken about (centre of the gt bounding box)
+  double *orig = nullptr;             // the estimated cloud as handed in
+  long long cap_orig = 0;
+  const double *xyz = nullptr;        // the estimated cloud's buffer and size at me_icp_begin
+  long long n_est = 0;
+  bool had_normals[2] = {false, false};       // the clouds' own normals
+  bool normals_pending[2] = {false, false};   // generalized ICP: k-NN normals not estimated yet (me_icp_normals_slice)
+  bool swept = false;                 // the initial sweep ran (first me_icp_block)
+  bool have_prev = false, done = false;
+  double fitness = 0, rmse = 0;       // of the last block me_icp_step read
+  long long n_corr = 0;
+  int it = 0, converged = 0;
 };
 
 }  // namespace me
@@ -192,6 +213,7 @@ struct me_ctx {
   unsigned long long kernel_mask = 0;
   int mme_rows_cfg = 0;
   unsigned int *d_trace = nullptr;
+  me::IcpRun icp;
   std::string err;
 };
 
@@ -288,7 +310,8 @@ int exclusive_scan_inplace(me_ctx *ctx, uint32_t *a, long long n, unsigned long 
 int voxel_downsample(me_ctx *ctx, int which, double voxel_size, int64_t *n_out);
 int radix_sort_pairs(me_ctx *ctx, unsigned long long *keys, uint32_t *vals, unsigned long long *keys_tmp, uint32_t *vals_tmp,
                      long long n, int key_bits, unsigned long long **keys_sorted, uint32_t **vals_sorted);
-int run_nn(me_ctx *ctx, const me_nn_params *p, me_nn_accum *e2g, me_nn_accum *g2e, bool to_block = false);
+// sweep_only: the per-query results only (d_nn_idx / d_nn_d2), no accumulators handed out (registration)
+int run_nn(me_ctx *ctx, const me_nn_params *p, me_nn_accum *e2g, me_nn_accum *g2e, bool to_block = false, bool sweep_only = false);
 int unsort_nn(me_ctx *ctx, int which_query, int32_t *h_idx, double *h_d2);
 int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors, me_mme_accum *out, bool to_block = false);
 
@@ -319,7 +342,14 @@ int voxel_finish_block(me_ctx *ctx, int scs_radius);
 int transform_cloud(me_ctx *ctx, int which, const double T[16]);
 int run_icp(me_ctx *ctx, int method, double max_dist, int max_iter, double rel_fitness, double rel_rmse, const double T_init[16],
             me_icp_result *out);
-int estimate_normals(me_ctx *ctx, int which, int knn);
+int icp_begin(me_ctx *ctx, int method, double max_dist, int max_iter, double rel_fitness, double rel_rmse, const double T_init[16]);
+int icp_normals_slice(me_ctx *ctx, int which, double **d_normals, int64_t *slice_points, int32_t *pending);
+int icp_block(me_ctx *ctx, double **d_block, int32_t *n_sum);
+int icp_step(me_ctx *ctx, int32_t *done);
+int icp_end(me_ctx *ctx, me_icp_result *out);
+void icp_close(me_ctx *ctx, bool restore);
+void icp_update_host(int method, const double *blk, const double c[3], double upd[16]);
+int estimate_normals(me_ctx *ctx, int which, int knn, long long lo = 0, long long hi = -1, long long cap_points = 0);
 void invalidate_cloud(Cloud &c);      // the cloud's coordinates changed: bbox, lattice, NN and entropy results are stale
 int run_awd_rows(me_ctx *ctx, const double *rows27, int64_t n_rows, double voxel_size, int scs_radius, double *w_out,
                  me_awd_result *out);

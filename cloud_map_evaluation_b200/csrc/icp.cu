@@ -26,6 +26,14 @@
 //                    the 6x6 solve and TransformVector6dToMatrix4d run on the host.
 // Per iteration: the est lattice is laid out again (the cloud moved), the flat NN sweep finds the correspondences, one
 // reduction kernel, one transform.
+//
+// The loop is split at its only collective (me_icp_begin / _normals_slice / _block / _step / _end): a rank sweeps the query
+// range of the cell-sorted moved cloud that query_shard gives it, and its reduction kernel leaves the partial sums as a
+// block of fp64 (the count rides as fp64, exact below 2^53) in device memory.  The caller SUM-all-reduces the block in
+// place; every rank then runs the same host algebra on the same doubles, so T stays identical on all ranks.  me_icp is the
+// same sequence at world = 1 without the collective.  The k-NN normals of generalized ICP shard by caller index: rank r
+// estimates [r s, (r + 1) s), s = ceil(N / world), visiting those points in cell-sorted order through a compacted list,
+// and the caller all-gathers the slices in place.
 #include "common.cuh"
 #include <algorithm>
 #include <cmath>
@@ -35,20 +43,21 @@ namespace me {
 
 static constexpr int kThreads = 256;
 
-struct IcpAcc {
-  unsigned long long n;
-  double sp[3], sq[3], sqp[9], err2;
-};
+// the fp64 block of one sweep: [0] count, then the sums (ME_ICP_BLOCK_P2P / ME_ICP_BLOCK_NE values in all)
+static double *icp_block_dev(me_ctx *ctx) { return (double *)((char *)ctx->d_scratch + 2048); }
+static double *icp_block_host(me_ctx *ctx) { return (double *)((char *)ctx->h_pinned + 2048); }
+static int icp_block_len(int method) { return method == ME_ICP_POINT_TO_POINT ? ME_ICP_BLOCK_P2P : ME_ICP_BLOCK_NE; }
 
-// sums about `c` (a point near the clouds: keeps the magnitudes, and with them the cancellation in sigma, small)
+// sums about `c` (a point near the clouds: keeps the magnitudes, and with them the cancellation in sigma, small) over the
+// queries [qb, qe) of the cell-sorted cloud; acc = [count, sum p (3), sum q (3), sum q p^T (9, row-major), sum d2]
 __global__ void __launch_bounds__(kThreads)
-icp_accum_kernel(const P4 *__restrict__ Q, long long n, const int32_t *__restrict__ nn_idx, const double *__restrict__ nn_d2,
-                 const double *__restrict__ gt_xyz, double r2, double cx, double cy, double cz, IcpAcc *__restrict__ acc) {
+icp_accum_kernel(const P4 *__restrict__ Q, long long qb, long long qe, const int32_t *__restrict__ nn_idx, const double *__restrict__ nn_d2,
+                 const double *__restrict__ gt_xyz, double r2, double cx, double cy, double cz, double *__restrict__ acc) {
   double v[17];
 #pragma unroll
   for (int k = 0; k < 17; ++k) v[k] = 0.0;
   unsigned long long cnt = 0;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+  for (long long i = qb + blockIdx.x * (long long)blockDim.x + threadIdx.x; i < qe; i += (long long)gridDim.x * blockDim.x) {
     const int32_t j = __ldg(nn_idx + i);
     if (j < 0) continue;
     const double d2 = __ldg(nn_d2 + i);
@@ -78,12 +87,11 @@ icp_accum_kernel(const P4 *__restrict__ Q, long long n, const int32_t *__restric
   if (threadIdx.x < 16) {
     double s = 0;
     for (int w = 0; w < kThreads / 32; ++w) s += sh[w][threadIdx.x];
-    double *dst = &acc->sp[0];                             // sp, sq, sqp, err2 are contiguous
-    if (s != 0.0) atomicAdd(dst + threadIdx.x, s);
+    if (s != 0.0) atomicAdd(acc + 1 + threadIdx.x, s);
   } else if (threadIdx.x == 32) {
     unsigned long long s = 0;
     for (int w = 0; w < kThreads / 32; ++w) s += shc[w];
-    if (s) atomicAdd(&acc->n, s);
+    if (s) atomicAdd(acc, (double)s);                      // block counts < 2^53: the fp64 sum is exact
   }
 }
 
@@ -112,13 +120,15 @@ static double det3_host(const double *m) {
   return m[0] * (m[4] * m[8] - m[5] * m[7]) - m[1] * (m[3] * m[8] - m[5] * m[6]) + m[2] * (m[3] * m[7] - m[4] * m[6]);
 }
 
-// Eigen::umeyama without scaling from the reduced sums: R = U S V^T of sigma = (1/n) sum (q - qm)(p - pm)^T
-static void umeyama_from_sums(const IcpAcc &a, const double c[3], double upd[16]) {
-  const double n = (double)a.n;
+// Eigen::umeyama without scaling from the reduced sums (icp_accum_kernel's block): R = U S V^T of
+// sigma = (1/n) sum (q - qm)(p - pm)^T
+static void umeyama_from_sums(const double *blk, const double c[3], double upd[16]) {
+  const double n = blk[0];
+  const double *sp = blk + 1, *sq = blk + 4, *sqp = blk + 7;
   double pm[3], qm[3], sigma[9];
-  for (int k = 0; k < 3; ++k) { pm[k] = a.sp[k] / n; qm[k] = a.sq[k] / n; }
+  for (int k = 0; k < 3; ++k) { pm[k] = sp[k] / n; qm[k] = sq[k] / n; }
   for (int r = 0; r < 3; ++r)
-    for (int col = 0; col < 3; ++col) sigma[r * 3 + col] = a.sqp[r * 3 + col] / n - qm[r] * pm[col];
+    for (int col = 0; col < 3; ++col) sigma[r * 3 + col] = sqp[r * 3 + col] / n - qm[r] * pm[col];
   // SVD through the symmetric eigen-problem of sigma^T sigma
   double ata[9], w[3], V[9];
   for (int r = 0; r < 3; ++r)
@@ -257,17 +267,19 @@ __device__ void fast_eigen3x3_normal(const double cov[9], double nrm[3]) {
 // included), their covariance, the eigenvector of its smallest eigenvalue.  One thread per point; the k best (d2,
 // position) pairs sit sorted in shared memory ([slot][thread]); the lattice is searched shell by shell (Chebyshev rings)
 // until the k-th distance beats the distance to the border of the searched block.  Ties go to the smaller caller index.
+// The queries are the n points of the cell-sorted cloud, or (list != nullptr) the sorted positions list[0 .. n): the
+// neighbours, and with them the arithmetic of every normal, do not depend on which points are queried together.
 // ---------------------------------------------------------------------------------------------------------------
 static constexpr int kKnnThreads = 128;
 
 __global__ void __launch_bounds__(kKnnThreads)
-knn_normals_kernel(const P4 *__restrict__ S, long long n, CellIndex I, Lattice L, CoarseGrid CG, int k, double slack,
-                   double *__restrict__ normals) {
+knn_normals_kernel(const P4 *__restrict__ S, long long n, const uint32_t *__restrict__ list, CellIndex I, Lattice L,
+                   CoarseGrid CG, int k, double slack, double *__restrict__ normals) {
   extern __shared__ __align__(16) unsigned char knn_smem[];
   double *dk = reinterpret_cast<double *>(knn_smem) + threadIdx.x;                                     // dk[t * kKnnThreads]
   uint32_t *ik = reinterpret_cast<uint32_t *>(knn_smem + (size_t)k * kKnnThreads * sizeof(double)) + threadIdx.x;
   for (long long i = blockIdx.x * (long long)kKnnThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kKnnThreads) {
-    const P4 q = load_p4(S + i);
+    const P4 q = load_p4(S + (list ? (long long)__ldg(list + i) : i));
     int cix, ciy, ciz;
     long long xs = I.sparse ? cell_coord(q.x, L, 0) : 0;
     xs = xs < 0 ? 0 : (xs >= L.dims[0] ? L.dims[0] - 1 : xs);
@@ -391,35 +403,73 @@ knn_normals_kernel(const P4 *__restrict__ S, long long n, CellIndex I, Lattice L
   }
 }
 
-int estimate_normals(me_ctx *ctx, int which, int knn) {
+// the sorted positions whose caller index lies in [lo, hi), in sorted order: flag (n + 1 entries, the last 0) -> exclusive
+// scan -> compaction
+__global__ void __launch_bounds__(kThreads) slice_flag_kernel(const P4 *__restrict__ S, long long n, long long lo, long long hi,
+                                                              uint32_t *__restrict__ flag) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i <= n; i += (long long)gridDim.x * blockDim.x) {
+    bool in = false;
+    if (i < n) {
+      const long long o = orig_of(__double_as_longlong(__ldg(reinterpret_cast<const double *>(S + i) + 3)));
+      in = o >= lo && o < hi;
+    }
+    flag[i] = in ? 1u : 0u;
+  }
+}
+__global__ void __launch_bounds__(kThreads) slice_compact_kernel(const uint32_t *__restrict__ pos, long long n,
+                                                                 uint32_t *__restrict__ list) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const uint32_t p = __ldg(pos + i);
+    if (__ldg(pos + i + 1) != p) list[p] = (uint32_t)i;
+  }
+}
+
+// the normals of the points with caller index in [lo, hi) (hi < 0: all of them) into c.d_normal, which holds at least
+// `cap_points` normals (the padded buffer of a sharded estimate)
+int estimate_normals(me_ctx *ctx, int which, int knn, long long lo, long long hi, long long cap_points) {
   Cloud &c = ctx->cloud[which];
   if (c.n <= 0) return fail(ctx, ME_ERR_EMPTY, "cloud is empty");
   if (knn < 1 || knn > 64) return fail(ctx, ME_ERR_INVALID, "knn must be in 1..64");
   ME_TRY(build_grid(ctx, which, c.grid_valid && c.grid_solo ? c.solo_h : 0.0));
   if (c.slab) return fail(ctx, ME_ERR_INVALID, "me_estimate_normals needs the replicated layout (ME_LAYOUT_REPLICATED)");
-  ME_TRY(ensure(ctx, (void **)&c.d_normal, &c.cap_normal, 3 * c.n, sizeof(double)));
-  const int k = (int)std::min<long long>(knn, c.n);
-  const size_t smem = (size_t)k * kKnnThreads * (sizeof(double) + sizeof(uint32_t));
-  if (smem > 48 * 1024)
-    ME_CUDA(ctx, cudaFuncSetAttribute(knn_normals_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  double maxabs = 0;
-  for (int a = 0; a < 3; ++a) maxabs = std::max(maxabs, std::max(std::fabs(c.bbox_min[a]), std::fabs(c.bbox_max[a])));
-  const double slack = 1e-9 * c.lat.h + 4e-14 * maxabs;
-  const int blocks = (int)std::min<long long>((c.n + kKnnThreads - 1) / kKnnThreads, (long long)ctx->sm_count * 32);
-  knn_normals_kernel<<<blocks, kKnnThreads, smem, ctx->stream>>>(c.d_sorted, c.n, index_of(c), c.lat, coarse_of(c), k, slack, c.d_normal);
-  ME_LAUNCH_CHECK(ctx);
+  ME_TRY(ensure(ctx, (void **)&c.d_normal, &c.cap_normal, 3 * std::max(c.n, cap_points), sizeof(double)));
+  const bool sliced = hi >= 0;
+  lo = sliced ? std::min(std::max(lo, 0ll), c.n) : 0;
+  hi = sliced ? std::min(std::max(hi, lo), c.n) : c.n;
+  const long long nq = hi - lo;
+  uint32_t *list = nullptr;
+  if (sliced && nq < c.n) {
+    ME_TRY(ensure_work(ctx, (size_t)(c.n + 1 + nq) * sizeof(uint32_t)));
+    uint32_t *pos = (uint32_t *)ctx->d_work;
+    list = pos + c.n + 1;
+    const int fb = (int)std::min<long long>((c.n + kThreads) / kThreads, (long long)ctx->sm_count * 16);
+    slice_flag_kernel<<<fb, kThreads, 0, ctx->stream>>>(c.d_sorted, c.n, lo, hi, pos);
+    ME_LAUNCH_CHECK(ctx);
+    ME_TRY(exclusive_scan_inplace(ctx, pos, c.n + 1));
+    slice_compact_kernel<<<fb, kThreads, 0, ctx->stream>>>(pos, c.n, list);
+    ME_LAUNCH_CHECK(ctx);
+  }
+  if (nq > 0) {
+    const int k = (int)std::min<long long>(knn, c.n);
+    const size_t smem = (size_t)k * kKnnThreads * (sizeof(double) + sizeof(uint32_t));
+    if (smem > 48 * 1024)
+      ME_CUDA(ctx, cudaFuncSetAttribute(knn_normals_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    double maxabs = 0;
+    for (int a = 0; a < 3; ++a) maxabs = std::max(maxabs, std::max(std::fabs(c.bbox_min[a]), std::fabs(c.bbox_max[a])));
+    const double slack = 1e-9 * c.lat.h + 4e-14 * maxabs;
+    const int blocks = (int)std::min<long long>((nq + kKnnThreads - 1) / kKnnThreads, (long long)ctx->sm_count * 32);
+    knn_normals_kernel<<<blocks, kKnnThreads, smem, ctx->stream>>>(c.d_sorted, nq, list, index_of(c), c.lat, coarse_of(c), k,
+                                                                   slack, c.d_normal);
+    ME_LAUNCH_CHECK(ctx);
+  }
   c.normal_valid = true;
   return ME_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// normal equations of point-to-plane (method 1) and generalized ICP (method 2) over the kept correspondences:
-// v[0..20] upper triangle of JTJ (row-major), v[21..26] JTr, v[27] sum d2
+// normal equations of point-to-plane (method 1) and generalized ICP (method 2) over the kept correspondences of the
+// queries [qb, qe): acc = [count, v] with v[0..20] the upper triangle of JTJ (row-major), v[21..26] JTr, v[27] sum d2
 // ---------------------------------------------------------------------------------------------------------------
-struct NeAcc {
-  unsigned long long n;
-  double v[28];
-};
 struct Mat9 { double r[9]; };
 
 // GetRotationFromE1ToX(x) diag(eps, 1, 1) GetRotationFromE1ToX(x)^T with x as given (Open3D does not normalise it):
@@ -450,14 +500,14 @@ __device__ __forceinline__ void gicp_cov(const double x[3], double eps, const do
 }
 
 __global__ void __launch_bounds__(kThreads)
-icp_ne_accum_kernel(const P4 *__restrict__ Q, long long n, const int32_t *__restrict__ nn_idx, const double *__restrict__ nn_d2,
-                    const double *__restrict__ gt_xyz, const double *__restrict__ gt_nrm, const double *__restrict__ est_nrm,
-                    Mat9 Rs, double r2, double eps, int method, NeAcc *__restrict__ acc) {
+icp_ne_accum_kernel(const P4 *__restrict__ Q, long long qb, long long qe, const int32_t *__restrict__ nn_idx,
+                    const double *__restrict__ nn_d2, const double *__restrict__ gt_xyz, const double *__restrict__ gt_nrm,
+                    const double *__restrict__ est_nrm, Mat9 Rs, double r2, double eps, int method, double *__restrict__ acc) {
   double v[28];
 #pragma unroll
   for (int k = 0; k < 28; ++k) v[k] = 0.0;
   unsigned long long cnt = 0;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+  for (long long i = qb + blockIdx.x * (long long)blockDim.x + threadIdx.x; i < qe; i += (long long)gridDim.x * blockDim.x) {
     const int32_t j = __ldg(nn_idx + i);
     if (j < 0) continue;
     const double d2 = __ldg(nn_d2 + i);
@@ -526,11 +576,11 @@ icp_ne_accum_kernel(const P4 *__restrict__ Q, long long n, const int32_t *__rest
   if (threadIdx.x < 28) {
     double s = 0;
     for (int w2 = 0; w2 < kThreads / 32; ++w2) s += sh[w2][threadIdx.x];
-    if (s != 0.0) atomicAdd(&acc->v[threadIdx.x], s);
+    if (s != 0.0) atomicAdd(acc + 1 + threadIdx.x, s);
   } else if (threadIdx.x == 32) {
     unsigned long long s = 0;
     for (int w2 = 0; w2 < kThreads / 32; ++w2) s += shc[w2];
-    if (s) atomicAdd(&acc->n, s);
+    if (s) atomicAdd(acc, (double)s);
   }
 }
 
@@ -568,134 +618,221 @@ static void vec6_to_mat4_host(const double x[6], double T[16]) {
   T[12] = T[13] = T[14] = 0; T[15] = 1;
 }
 
-int run_icp(me_ctx *ctx, int method, double max_dist, int max_iter, double rel_fitness, double rel_rmse, const double T_init[16],
-            me_icp_result *out) {
-  std::memset(out, 0, sizeof(*out));
+// the update of one iteration from a reduced block: Umeyama (point-to-point, sums about c) or the 6x6 solve +
+// TransformVector6dToMatrix4d; the identity when there are no correspondences or the solve fails (Open3D)
+void icp_update_host(int method, const double *blk, const double c[3], double upd[16]) {
+  static const double I[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  std::memcpy(upd, I, sizeof(I));
+  if (!(blk[0] > 0)) return;
+  if (method == ME_ICP_POINT_TO_POINT) { umeyama_from_sums(blk, c, upd); return; }
+  const double *v = blk + 1;
+  double JTJ[36], nb[6], x[6];
+  int t = 0;
+  for (int a = 0; a < 6; ++a)
+    for (int b = a; b < 6; ++b) { JTJ[a * 6 + b] = v[t]; JTJ[b * 6 + a] = v[t]; ++t; }
+  for (int a = 0; a < 6; ++a) nb[a] = -v[21 + a];
+  if (solve6_host(JTJ, nb, x)) vec6_to_mat4_host(x, upd);
+}
+
+// every failure of an open registration closes it: the estimated cloud (and its normals) come back as they were handed in
+void icp_close(me_ctx *ctx, bool restore) {
+  IcpRun &S = ctx->icp;
+  if (!S.open) return;
+  Cloud &E = ctx->cloud[ME_CLOUD_EST], &G = ctx->cloud[ME_CLOUD_GT];
+  if (restore && S.orig && E.d_xyz == S.xyz && E.n == S.n_est)
+    cudaMemcpyAsync(E.d_xyz, S.orig, (size_t)E.n * 3 * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream);
+  invalidate_cloud(E);
+  E.normal_valid = S.had_normals[ME_CLOUD_EST];      // the working normals of generalized ICP do not outlive the call
+  G.normal_valid = S.had_normals[ME_CLOUD_GT];
+  cudaStreamSynchronize(ctx->stream);
+  if (S.orig) cudaFree(S.orig);
+  S = IcpRun();
+}
+static int icp_fail(me_ctx *ctx, int rc) {
+  icp_close(ctx, true);
+  return rc;
+}
+
+int icp_begin(me_ctx *ctx, int method, double max_dist, int max_iter, double rel_fitness, double rel_rmse, const double T_init[16]) {
+  if (ctx->icp.open) return icp_fail(ctx, fail(ctx, ME_ERR_INVALID, "me_icp_begin while a registration is open (me_icp_end first)"));
   Cloud &E = ctx->cloud[ME_CLOUD_EST], &G = ctx->cloud[ME_CLOUD_GT];
   if (E.n <= 0 || G.n <= 0) return fail(ctx, ME_ERR_EMPTY, "both clouds must be set (map_eval.cpp:32-35)");
   if (method != ME_ICP_POINT_TO_POINT && method != ME_ICP_POINT_TO_PLANE && method != ME_ICP_GENERALIZED)
     return fail(ctx, ME_ERR_INVALID, "Invalid registration type specified (map_eval.cpp:1387)");
-  if (ctx->world != 1) return fail(ctx, ME_ERR_INVALID, "me_icp needs world == 1 (the update needs all correspondences)");
   if (!E.owned) return fail(ctx, ME_ERR_INVALID, "me_icp needs a library-owned estimated cloud (use me_set_cloud)");
   if (!(max_dist > 0) || max_iter < 0) return fail(ctx, ME_ERR_INVALID, "bad ICP parameters");
   if (method == ME_ICP_POINT_TO_PLANE && !G.normal_valid)
     return fail(ctx, ME_ERR_INVALID, "TransformationEstimationPointToPlane requires pre-computed normal vectors for the target "
                                      "PointCloud (me_set_normals / me_estimate_normals on the ground-truth cloud)");
+  if (ctx->world > 1 && ctx->slab_request)
+    return fail(ctx, ME_ERR_INVALID, "registration needs the replicated layout: me_set_layout(ME_LAYOUT_REPLICATED) before "
+                                     "me_icp_begin, ME_LAYOUT_SLAB again afterwards");
   ME_TRY(wait_upload(ctx, ME_CLOUD_EST));
-  const double eps = 1e-3;      // TransformationEstimationForGeneralizedICP() default epsilon
-  const bool est_had_normals = E.normal_valid, gt_had_normals = G.normal_valid;
-  int rc = ME_OK;
-  if (method == ME_ICP_GENERALIZED) {
-    // InitializePointCloudForGeneralizedICP per cloud (before the initial transform, as Open3D does): the cloud's own
-    // normals, else EstimateNormals(KNN 20) into the cloud's normal buffer as a working copy that stays invalid afterwards
-    if (!est_had_normals || !gt_had_normals) rc = build_both(ctx);
-    if (rc == ME_OK && !est_had_normals) rc = estimate_normals(ctx, ME_CLOUD_EST, 20);
-    if (rc == ME_OK && !gt_had_normals) rc = estimate_normals(ctx, ME_CLOUD_GT, 20);
-    E.normal_valid = est_had_normals; G.normal_valid = gt_had_normals;
-    if (rc != ME_OK) return rc;
-  }
+  IcpRun &S = ctx->icp;
+  S = IcpRun();
   // the original cloud: RegistrationICP iterates on a copy, the caller's cloud is transformed once at the end (:1392)
-  double *orig = nullptr;
-  long long cap_orig = 0;
-  ME_TRY(ensure(ctx, (void **)&orig, &cap_orig, 3 * E.n, sizeof(double)));
-  // the estimated cloud's normals stay as they came in while the copy moves (generalized ICP rotates the covariances
-  // with the accumulated R instead); the final transformation rotates them once, as PointCloud::Transform does
-  E.normal_valid = false;
-  if (cudaMemcpyAsync(orig, E.d_xyz, (size_t)E.n * 3 * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess)
-    rc = fail(ctx, ME_ERR_CUDA, "copy of the estimated cloud failed");
+  ME_TRY(ensure(ctx, (void **)&S.orig, &S.cap_orig, 3 * E.n, sizeof(double)));
+  S.open = true;
+  S.xyz = E.d_xyz; S.n_est = E.n;
+  S.method = method; S.max_iter = max_iter; S.max_dist = max_dist; S.rel_fitness = rel_fitness; S.rel_rmse = rel_rmse;
+  std::memcpy(S.T, T_init, sizeof(S.T));
+  for (int w = 0; w < 2; ++w) {
+    S.had_normals[w] = ctx->cloud[w].normal_valid;
+    // InitializePointCloudForGeneralizedICP per cloud: the cloud's own normals, else EstimateNormals(KNN 20)
+    S.normals_pending[w] = method == ME_ICP_GENERALIZED && !S.had_normals[w];
+  }
+  if (cudaMemcpyAsync(S.orig, E.d_xyz, (size_t)E.n * 3 * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess)
+    return icp_fail(ctx, fail(ctx, ME_ERR_CUDA, "copy of the estimated cloud failed"));
+  return ME_OK;
+}
 
-  double T[16];
-  std::memcpy(T, T_init, sizeof(T));
-  if (rc == ME_OK) rc = transform_cloud(ctx, ME_CLOUD_EST, T);
+int icp_normals_slice(me_ctx *ctx, int which, double **d_normals, int64_t *slice_points, int32_t *pending) {
+  IcpRun &S = ctx->icp;
+  *d_normals = nullptr; *slice_points = 0; *pending = 0;
+  if (!S.open) return fail(ctx, ME_ERR_INVALID, "me_icp_normals_slice before me_icp_begin");
+  if (S.swept) return icp_fail(ctx, fail(ctx, ME_ERR_INVALID, "me_icp_normals_slice after the first me_icp_block"));
+  if (!S.normals_pending[which]) return ME_OK;      // the cloud's own normals, or a method without source covariances
+  Cloud &c = ctx->cloud[which];
+  // estimated before the initial transform, as Open3D does; into the cloud's normal buffer as a working copy that stays
+  // invalid afterwards.  Rank r: caller indices [r s, (r + 1) s), s = ceil(N / world), the buffer padded to world * s.
+  const long long s = (c.n + ctx->world - 1) / ctx->world, lo = (long long)ctx->rank * s;
+  int rc = build_both(ctx);
+  if (rc == ME_OK) rc = ctx->world == 1 ? estimate_normals(ctx, which, 20) : estimate_normals(ctx, which, 20, lo, lo + s, s * ctx->world);
+  c.normal_valid = false;
+  if (rc != ME_OK) return icp_fail(ctx, rc);
+  S.normals_pending[which] = false;
+  *d_normals = c.d_normal; *slice_points = s; *pending = ctx->world > 1 ? 1 : 0;
+  return ME_OK;
+}
+
+// one correspondence sweep of the moved cloud and this rank's partial sums into the block
+static int icp_sweep(me_ctx *ctx) {
+  IcpRun &S = ctx->icp;
+  Cloud &E = ctx->cloud[ME_CLOUD_EST], &G = ctx->cloud[ME_CLOUD_GT];
   me_nn_params p;
   std::memset(&p, 0, sizeof(p));
-  p.icp_max_distance = max_dist;
+  p.icp_max_distance = S.max_dist;
   p.cutoff_mode = ME_CUTOFF_DIST_LT_R;
   p.pairing = ME_PAIRING_GEOMETRIC;
   p.want_full_cd = 0;
   p.directions = 1;
-  IcpAcc *d_acc = (IcpAcc *)((char *)ctx->d_scratch + 1024), *h_acc = (IcpAcc *)((char *)ctx->h_pinned + 1536);
-  NeAcc *d_ne = (NeAcc *)((char *)ctx->d_scratch + 2048), *h_ne = (NeAcc *)((char *)ctx->h_pinned + 2048);
-  IcpAcc res;
-  NeAcc ne;
-  std::memset(&res, 0, sizeof(res));
-  std::memset(&ne, 0, sizeof(ne));
-  unsigned long long n_corr = 0;
-  double fitness = 0, rmse = 0, c[3] = {0, 0, 0};
-  auto evaluate = [&]() -> int {
-    me_nn_accum e2g;
-    ME_TRY(run_nn(ctx, &p, &e2g, nullptr));                                  // lays the moved cloud out again, then sweeps
-    const int blocks = (int)std::min<long long>((E.n + kThreads - 1) / kThreads, (long long)ctx->sm_count * 8);
-    double err2 = 0;
-    if (method == ME_ICP_POINT_TO_POINT) {
-      for (int a = 0; a < 3; ++a) c[a] = 0.5 * (G.bbox_min[a] + G.bbox_max[a]);
-      ME_CUDA(ctx, cudaMemsetAsync(d_acc, 0, sizeof(IcpAcc), ctx->stream));
-      icp_accum_kernel<<<blocks, kThreads, 0, ctx->stream>>>(E.d_sorted, E.n, E.d_nn_idx, E.d_nn_d2, G.d_xyz, max_dist * max_dist,
-                                                            c[0], c[1], c[2], d_acc);
-      ME_LAUNCH_CHECK(ctx);
-      ME_CUDA(ctx, cudaMemcpyAsync(h_acc, d_acc, sizeof(IcpAcc), cudaMemcpyDeviceToHost, ctx->stream));
-      ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-      res = *h_acc;
-      n_corr = res.n; err2 = res.err2;
-    } else {
-      Mat9 R;      // rotation block of the accumulated transformation: the source covariances are R C(n) R^T
-      for (int r = 0; r < 3; ++r)
-        for (int col = 0; col < 3; ++col) R.r[r * 3 + col] = T[r * 4 + col];
-      ME_CUDA(ctx, cudaMemsetAsync(d_ne, 0, sizeof(NeAcc), ctx->stream));
-      icp_ne_accum_kernel<<<blocks, kThreads, 0, ctx->stream>>>(E.d_sorted, E.n, E.d_nn_idx, E.d_nn_d2, G.d_xyz, G.d_normal,
-                                                               E.d_normal, R, max_dist * max_dist, eps, method, d_ne);
-      ME_LAUNCH_CHECK(ctx);
-      ME_CUDA(ctx, cudaMemcpyAsync(h_ne, d_ne, sizeof(NeAcc), cudaMemcpyDeviceToHost, ctx->stream));
-      ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-      ne = *h_ne;
-      n_corr = ne.n; err2 = ne.v[27];
-    }
-    fitness = (double)n_corr / (double)E.n;
-    rmse = n_corr > 0 ? std::sqrt(err2 / (double)n_corr) : 0.0;
-    return ME_OK;
-  };
-  int it = 0, converged = 0;
-  if (rc == ME_OK) rc = evaluate();
-  for (; rc == ME_OK && it < max_iter; ++it) {
-    // ComputeTransformation: the identity when there are no correspondences or the solve fails (Open3D)
-    double upd[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    if (n_corr > 0) {
-      if (method == ME_ICP_POINT_TO_POINT) umeyama_from_sums(res, c, upd);
-      else {
-        double JTJ[36], nb[6], x[6];
-        int t = 0;
-        for (int a = 0; a < 6; ++a)
-          for (int b = a; b < 6; ++b) { JTJ[a * 6 + b] = ne.v[t]; JTJ[b * 6 + a] = ne.v[t]; ++t; }
-        for (int a = 0; a < 6; ++a) nb[a] = -ne.v[21 + a];
-        if (solve6_host(JTJ, nb, x)) vec6_to_mat4_host(x, upd);
-      }
-    }
-    double Tn[16];
-    for (int r = 0; r < 4; ++r)
-      for (int col = 0; col < 4; ++col) { double s = 0; for (int k = 0; k < 4; ++k) s += upd[r * 4 + k] * T[k * 4 + col]; Tn[r * 4 + col] = s; }
-    std::memcpy(T, Tn, sizeof(T));
-    rc = transform_cloud(ctx, ME_CLOUD_EST, upd);
-    if (rc != ME_OK) break;
-    const double f0 = fitness, r0 = rmse;
-    rc = evaluate();
-    if (rc != ME_OK) break;
-    if (std::fabs(f0 - fitness) < rel_fitness && std::fabs(r0 - rmse) < rel_rmse) { ++it; converged = 1; break; }
+  ME_TRY(run_nn(ctx, &p, nullptr, nullptr, false, true));      // lays the moved cloud out again, then sweeps this rank's queries
+  const long long qb = E.nn_b, qe = E.nn_e;
+  const int blocks = (int)std::max(1ll, std::min<long long>((qe - qb + kThreads - 1) / kThreads, (long long)ctx->sm_count * 8));
+  double *blk = icp_block_dev(ctx);
+  ME_CUDA(ctx, cudaMemsetAsync(blk, 0, ME_ICP_BLOCK_NE * sizeof(double), ctx->stream));
+  const double r2 = S.max_dist * S.max_dist;
+  if (S.method == ME_ICP_POINT_TO_POINT) {
+    for (int a = 0; a < 3; ++a) S.c[a] = 0.5 * (G.bbox_min[a] + G.bbox_max[a]);
+    icp_accum_kernel<<<blocks, kThreads, 0, ctx->stream>>>(E.d_sorted, qb, qe, E.d_nn_idx, E.d_nn_d2, G.d_xyz, r2, S.c[0], S.c[1],
+                                                          S.c[2], blk);
+  } else {
+    Mat9 R;      // rotation block of the accumulated transformation: the source covariances are R C(n) R^T
+    for (int r = 0; r < 3; ++r)
+      for (int col = 0; col < 3; ++col) R.r[r * 3 + col] = S.T[r * 4 + col];
+    const double eps = 1e-3;      // TransformationEstimationForGeneralizedICP() default epsilon
+    icp_ne_accum_kernel<<<blocks, kThreads, 0, ctx->stream>>>(E.d_sorted, qb, qe, E.d_nn_idx, E.d_nn_d2, G.d_xyz, G.d_normal,
+                                                             E.d_normal, R, r2, eps, S.method, blk);
   }
-  // est := Transform(original, T) (map_eval.cpp:1392), normals handed in included.  On an error the original cloud (and
-  // its normals) come back untouched; either way every derived structure of the estimated cloud is stale now.
-  int rc2 = ME_OK;
-  if (cudaMemcpyAsync(E.d_xyz, orig, (size_t)E.n * 3 * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess)
-    rc2 = fail(ctx, ME_ERR_CUDA, "restoring the estimated cloud failed");
-  invalidate_cloud(E);
-  E.normal_valid = est_had_normals;               // the working normals of generalized ICP do not outlive the call
-  if (rc == ME_OK && rc2 == ME_OK) rc2 = transform_cloud(ctx, ME_CLOUD_EST, T);
-  if (cudaStreamSynchronize(ctx->stream) != cudaSuccess && rc2 == ME_OK) rc2 = fail(ctx, ME_ERR_CUDA, "synchronize after ICP failed");
-  cudaFree(orig);
-  if (rc != ME_OK) return rc;
-  if (rc2 != ME_OK) return rc2;
-  std::memcpy(out->transformation, T, sizeof(T));
-  out->fitness = fitness; out->inlier_rmse = rmse; out->n_corr = (int64_t)n_corr; out->iterations = it; out->converged = converged;
+  ME_LAUNCH_CHECK(ctx);
   return ME_OK;
+}
+
+static int icp_ready(me_ctx *ctx, const char *call) {
+  IcpRun &S = ctx->icp;
+  if (!S.open) return fail(ctx, ME_ERR_INVALID, std::string(call) + " before me_icp_begin");
+  const Cloud &E = ctx->cloud[ME_CLOUD_EST];
+  if (E.d_xyz != S.xyz || E.n != S.n_est)
+    return icp_fail(ctx, fail(ctx, ME_ERR_INVALID, std::string(call) + ": the estimated cloud was replaced during the registration"));
+  if (S.normals_pending[0] || S.normals_pending[1])
+    return icp_fail(ctx, fail(ctx, ME_ERR_INVALID, std::string(call) + ": the k-NN normals of generalized ICP are still pending "
+                                                   "(me_icp_normals_slice for both clouds, all-gathered, first)"));
+  return ME_OK;
+}
+
+int icp_block(me_ctx *ctx, double **d_block, int32_t *n_sum) {
+  ME_TRY(icp_ready(ctx, "me_icp_block"));
+  IcpRun &S = ctx->icp;
+  if (!S.swept) {      // the initial sweep: pcd = est transformed by init, result = correspondences(pcd)
+    Cloud &E = ctx->cloud[ME_CLOUD_EST];
+    E.normal_valid = false;      // the estimated cloud's normals stay as handed in while the copy moves
+    int rc = transform_cloud(ctx, ME_CLOUD_EST, S.T);
+    if (rc == ME_OK) rc = icp_sweep(ctx);
+    if (rc != ME_OK) return icp_fail(ctx, rc);
+    S.swept = true;
+  }
+  *d_block = icp_block_dev(ctx);
+  *n_sum = icp_block_len(S.method);
+  return ME_OK;
+}
+
+int icp_step(me_ctx *ctx, int32_t *done) {
+  *done = 0;
+  ME_TRY(icp_ready(ctx, "me_icp_step"));
+  IcpRun &S = ctx->icp;
+  if (!S.swept) return icp_fail(ctx, fail(ctx, ME_ERR_INVALID, "me_icp_step before the first me_icp_block"));
+  if (S.done) { *done = 1; return ME_OK; }
+  const int nb = icp_block_len(S.method);
+  double *h = icp_block_host(ctx);
+  if (cudaMemcpyAsync(h, icp_block_dev(ctx), nb * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
+      cudaStreamSynchronize(ctx->stream) != cudaSuccess)
+    return icp_fail(ctx, fail(ctx, ME_ERR_CUDA, "reading the ICP block failed"));
+  double blk[ME_ICP_BLOCK_NE];
+  std::memcpy(blk, h, nb * sizeof(double));
+  const double n_est = (double)ctx->cloud[ME_CLOUD_EST].n;
+  S.n_corr = (long long)std::llround(blk[0]);
+  const double fitness = (double)S.n_corr / n_est;
+  const double rmse = S.n_corr > 0 ? std::sqrt(blk[nb - 1] / (double)S.n_corr) : 0.0;
+  if (S.have_prev) {      // the block of an update: ICPConvergenceCriteria
+    ++S.it;
+    if (std::fabs(S.fitness - fitness) < S.rel_fitness && std::fabs(S.rmse - rmse) < S.rel_rmse) S.converged = 1;
+  }
+  S.fitness = fitness; S.rmse = rmse; S.have_prev = true;
+  if (S.converged || S.it >= S.max_iter) { S.done = true; *done = 1; return ME_OK; }
+  double upd[16], Tn[16];
+  icp_update_host(S.method, blk, S.c, upd);
+  for (int r = 0; r < 4; ++r)
+    for (int col = 0; col < 4; ++col) { double s = 0; for (int k = 0; k < 4; ++k) s += upd[r * 4 + k] * S.T[k * 4 + col]; Tn[r * 4 + col] = s; }
+  std::memcpy(S.T, Tn, sizeof(Tn));
+  int rc = transform_cloud(ctx, ME_CLOUD_EST, upd);
+  if (rc == ME_OK) rc = icp_sweep(ctx);
+  if (rc != ME_OK) return icp_fail(ctx, rc);
+  return ME_OK;
+}
+
+int icp_end(me_ctx *ctx, me_icp_result *out) {
+  std::memset(out, 0, sizeof(*out));
+  IcpRun &S = ctx->icp;
+  if (!S.open) return fail(ctx, ME_ERR_INVALID, "me_icp_end without me_icp_begin");
+  if (!S.have_prev) return icp_fail(ctx, fail(ctx, ME_ERR_INVALID, "me_icp_end before the first me_icp_step"));
+  // est := Transform(original, T) (map_eval.cpp:1392), normals handed in included
+  double T[16];
+  std::memcpy(T, S.T, sizeof(T));
+  out->fitness = S.fitness; out->inlier_rmse = S.rmse; out->n_corr = (int64_t)S.n_corr;
+  out->iterations = S.it; out->converged = S.converged;
+  std::memcpy(out->transformation, T, sizeof(T));
+  icp_close(ctx, true);
+  int rc = transform_cloud(ctx, ME_CLOUD_EST, T);
+  if (rc == ME_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) rc = fail(ctx, ME_ERR_CUDA, "synchronize after ICP failed");
+  if (rc != ME_OK) std::memset(out, 0, sizeof(*out));
+  return rc;
+}
+
+int run_icp(me_ctx *ctx, int method, double max_dist, int max_iter, double rel_fitness, double rel_rmse, const double T_init[16],
+            me_icp_result *out) {
+  std::memset(out, 0, sizeof(*out));
+  if (ctx->world != 1) return fail(ctx, ME_ERR_INVALID, "me_icp needs world == 1 (the update needs all correspondences; "
+                                                        "use me_icp_begin .. me_icp_end with an all-reduce per iteration)");
+  // the split loop without its collectives: at world = 1 the normals need no gather and the block no reduction
+  ME_TRY(icp_begin(ctx, method, max_dist, max_iter, rel_fitness, rel_rmse, T_init));
+  double *d = nullptr;
+  int64_t s = 0;
+  int32_t pending = 0, n_sum = 0, done = 0;
+  ME_TRY(icp_normals_slice(ctx, ME_CLOUD_EST, &d, &s, &pending));
+  ME_TRY(icp_normals_slice(ctx, ME_CLOUD_GT, &d, &s, &pending));
+  ME_TRY(icp_block(ctx, &d, &n_sum));
+  while (!done) ME_TRY(icp_step(ctx, &done));
+  return icp_end(ctx, out);
 }
 
 }  // namespace me

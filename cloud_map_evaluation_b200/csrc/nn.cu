@@ -1074,6 +1074,12 @@ static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, me_nn_a
       ME_LAUNCH_CHECK(ctx);
     }
   }
+  Qc.nn_b = use_tile ? 0 : qb;
+  Qc.nn_e = use_tile ? Qc.n : qe;
+  if (!out && !to_block) {      // sweep only: the caller reads the per-query results
+    Qc.nn_valid = true;
+    return ME_OK;
+  }
   if (sharded && use_tile) {
     count_marked_kernel<<<fill_blocks, kThreads, 0, ctx->stream>>>(Qc.d_nn_idx, Qc.n, n_eval);
     ME_LAUNCH_CHECK(ctx);
@@ -1112,15 +1118,16 @@ int build_both(me_ctx *ctx) {
   return fail(ctx, ME_ERR_RANGE, "could not lay both clouds out on a common lattice");
 }
 
-int run_nn(me_ctx *ctx, const me_nn_params *p, me_nn_accum *e2g, me_nn_accum *g2e, bool to_block) {
+int run_nn(me_ctx *ctx, const me_nn_params *p, me_nn_accum *e2g, me_nn_accum *g2e, bool to_block, bool sweep_only) {
   if (ctx->cloud[0].n <= 0 || ctx->cloud[1].n <= 0)
     return fail(ctx, ME_ERR_EMPTY, "both clouds must be set (map_eval.cpp:32-35)");
   ME_TRY(build_both(ctx));
   const int dirs = p->directions ? p->directions : 3;
   if (e2g) std::memset(e2g, 0, sizeof(*e2g));
   if (g2e) std::memset(g2e, 0, sizeof(*g2e));
-  if ((dirs & 1) && (e2g || to_block)) ME_TRY(run_direction(ctx, ME_CLOUD_EST, p, e2g, 2, to_block));
-  if ((dirs & 2) && (g2e || to_block)) ME_TRY(run_direction(ctx, ME_CLOUD_GT, p, g2e, 3, to_block));
+  if (sweep_only) { e2g = g2e = nullptr; to_block = false; }
+  if ((dirs & 1) && (e2g || to_block || sweep_only)) ME_TRY(run_direction(ctx, ME_CLOUD_EST, p, e2g, 2, to_block));
+  if ((dirs & 2) && (g2e || to_block || sweep_only)) ME_TRY(run_direction(ctx, ME_CLOUD_GT, p, g2e, 3, to_block));
   return ME_OK;
 }
 

@@ -99,6 +99,45 @@ def allreduce_block(ctx, device, group=None):
     dist.all_reduce(t[n_sum:], op=dist.ReduceOp.MAX, group=group)
 
 
+def icp_distributed(ctx, device, max_correspondence_distance, T_init=None, max_iteration=30, relative_fitness=1e-6,
+                    relative_rmse=1e-6, method=A.ME_ICP_GENERALIZED, group=None):
+    """performICPRegistration on every rank of the job (map_eval.cpp:1366-1394): the clouds are replicated, every rank
+    sweeps its query range and estimates its slice of the missing k-NN normals.  One in-place all-gather per estimated
+    cloud, then ONE SUM all-reduce of the 17 / 29-value block per iteration; every rank applies the same update to the same
+    reduced doubles, so T is identical everywhere.  Returns (T 4x4, me_icp_result) like performICPRegistration; the
+    estimated cloud held by ctx is the original transformed by T."""
+    import torch
+    import torch.distributed as dist
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    rank = dist.get_rank(group) if dist.is_initialized() else 0
+    assert (rank, world) == (ctx.rank, ctx.world), "the context's shard must be this process's rank in the group"
+
+    def _torch_waits_for_ctx():
+        ctx.synchronize()
+
+    def _ctx_waits_for_torch():
+        torch.cuda.current_stream(device).synchronize()
+
+    ctx.icp_begin(max_correspondence_distance, T_init, max_iteration, relative_fitness, relative_rmse, method)
+    for which in (A.ME_CLOUD_EST, A.ME_CLOUD_GT):
+        ptr, s, pending = ctx.icp_normals_slice(which)
+        if pending:
+            _torch_waits_for_ctx()
+            buf = torch.as_tensor(_DeviceBlock(ptr, world * s * 3), device=device)
+            dist.all_gather_into_tensor(buf, buf[rank * s * 3:(rank + 1) * s * 3], group=group)
+            _ctx_waits_for_torch()
+    done = False
+    ptr, n_sum = ctx.icp_block()
+    blk = torch.as_tensor(_DeviceBlock(ptr, n_sum), device=device)
+    while not done:
+        if world > 1:
+            _torch_waits_for_ctx()
+            dist.all_reduce(blk, group=group)
+            _ctx_waits_for_torch()
+        done = ctx.icp_step()
+    return ctx.icp_end()
+
+
 def allreduce_voxel_w(ctx, device, group=None):
     """Slab layout, between MapEvalB200.voxel_begin and voxel_finish_accum_device: MAX-all-reduce of the W table over the
     estimated cloud's voxels in place (-1 = no pair; every voxel has one owner), so that the SCS sweep of every rank sees

@@ -103,6 +103,26 @@ class GpuGroup {
     return true;
   }
 
+  // collectives on buffers the contexts own (the ICP block, the normal slices), in place on the devices.  The caller has
+  // waited for the contexts' streams (me_synchronize); on return the result is complete on every device.
+  bool allreduce_device(const std::vector<double *> &ptr, size_t len, ncclRedOp_t op) {
+    const int n = size();
+    if (n == 1 || len == 0) return true;
+    ncclGroupStart();
+    for (int r = 0; r < n; ++r) ncclAllReduce(ptr[r], ptr[r], len, ncclDouble, op, comm_[r], stream_[r]);
+    if (ncclGroupEnd() != ncclSuccess) { err_ = "ncclAllReduce failed"; return false; }
+    return sync_streams();
+  }
+  // rank r contributes ptr[r] + r * per_rank (per_rank doubles); every ptr[r] holds all n slices afterwards
+  bool allgather_device(const std::vector<double *> &ptr, size_t per_rank) {
+    const int n = size();
+    if (n == 1 || per_rank == 0) return true;
+    ncclGroupStart();
+    for (int r = 0; r < n; ++r) ncclAllGather(ptr[r] + (size_t)r * per_rank, ptr[r], per_rank, ncclDouble, comm_[r], stream_[r]);
+    if (ncclGroupEnd() != ncclSuccess) { err_ = "ncclAllGather failed"; return false; }
+    return sync_streams();
+  }
+
   // sum-reduce the NN accumulators of all ranks (counts ride along as fp64: exact below 2^53, order-independent)
   bool reduce_nn(std::vector<me_nn_accum> &e2g, std::vector<me_nn_accum> &g2e) {
     const int n = size();
@@ -136,6 +156,13 @@ class GpuGroup {
   }
 
  private:
+  bool sync_streams() {
+    for (int r = 0; r < size(); ++r) {
+      cudaSetDevice(dev_[r]);
+      if (cudaStreamSynchronize(stream_[r]) != cudaSuccess) { err_ = "collective failed on its stream"; return false; }
+    }
+    return true;
+  }
   static constexpr int kMaxValues = 2 * (ME_NN_ACCUM_I64 + ME_NN_ACCUM_F64);
   static void pack(const me_nn_accum &a, std::vector<double> &v) {
     v.push_back((double)a.n_query); v.push_back((double)a.n_corr);

@@ -485,15 +485,48 @@ inline int MapEvalB200::calculateMetricsWithInitialMatrix() {
 
 inline int MapEvalB200::performRegistration() {
   TicToc tic_toc;
-  if (gpus_.size() > 1) std::cout << "INFO: ICP runs on GPU " << param_.gpu_device_ << " only; the metric sweeps are sharded." << std::endl;
-  // ICP needs all correspondences on one GPU: run it on a single-shard context, then hand every GPU the aligned cloud
-  me_icp_result reg{};
-  me_set_shard(ctx_, 0, 1);
   // performICPRegistration (:1366-1394): ICPConvergenceCriteria() = {1e-6, 1e-6, 30}; the normals loaded with the
-  // clouds (down-sampled along with them) are already on the context
-  const int rc = me_icp(ctx_, param_.evaluation_method_, param_.icp_max_distance_, 30, 1e-6, 1e-6, param_.initial_matrix_, &reg);
-  me_set_shard(ctx_, 0, gpus_.size());
-  if (rc != ME_OK) return fail("me_icp");
+  // clouds (down-sampled along with them) are already on the contexts.  On one GPU: me_icp.  On several, every GPU sweeps
+  // its query range and estimates its slice of the missing k-NN normals; the slices are all-gathered and the 17 / 29
+  // partial sums all-reduced once per iteration, so that every GPU applies the same update and holds the aligned cloud.
+  me_icp_result reg{};
+  if (gpus_.size() == 1) {
+    if (me_icp(ctx_, param_.evaluation_method_, param_.icp_max_distance_, 30, 1e-6, 1e-6, param_.initial_matrix_, &reg) != ME_OK)
+      return fail("me_icp");
+  } else {
+    const int n = gpus_.size();
+    std::vector<double *> ptr(n, nullptr);
+    std::vector<int64_t> slice(n, 0);
+    std::vector<int32_t> pending(n, 0), n_sum(n, 0), done(n, 0);
+    std::vector<me_icp_result> res(n);
+    if (gpus_.for_each([&](int, me_ctx *c) {
+          return me_icp_begin(c, param_.evaluation_method_, param_.icp_max_distance_, 30, 1e-6, 1e-6, param_.initial_matrix_);
+        }) != ME_OK)
+      return fail("me_icp_begin");
+    for (int which : {ME_CLOUD_EST, ME_CLOUD_GT}) {
+      if (gpus_.for_each([&](int r, me_ctx *c) {
+            const int rc = me_icp_normals_slice(c, which, &ptr[r], &slice[r], &pending[r]);
+            return rc != ME_OK ? rc : me_synchronize(c);
+          }) != ME_OK)
+        return fail("me_icp_normals_slice");
+      if (pending[0] && !gpus_.allgather_device(ptr, (size_t)slice[0] * 3)) return fail("all-gather of the normals");
+    }
+    if (gpus_.for_each([&](int r, me_ctx *c) {
+          const int rc = me_icp_block(c, &ptr[r], &n_sum[r]);
+          return rc != ME_OK ? rc : me_synchronize(c);
+        }) != ME_OK)
+      return fail("me_icp_block");
+    while (!done[0]) {
+      if (!gpus_.allreduce_device(ptr, (size_t)n_sum[0], ncclSum)) return fail("all-reduce of the ICP block");
+      if (gpus_.for_each([&](int r, me_ctx *c) {
+            const int rc = me_icp_step(c, &done[r]);
+            return rc != ME_OK ? rc : me_synchronize(c);
+          }) != ME_OK)
+        return fail("me_icp_step");
+    }
+    if (gpus_.for_each([&](int r, me_ctx *c) { return me_icp_end(c, &res[r]); }) != ME_OK) return fail("me_icp_end");
+    reg = res[0];
+  }
   t4 = tic_toc.toc();
   std::cout << "INFO: ICP registration time: " << (t4 - t3) / 1000.0 << " [s]" << std::endl;
   std::cout << "INFO: Aligned transformation: \n" << eigenMatrix4(reg.transformation, 6) << std::endl;
@@ -502,9 +535,6 @@ inline int MapEvalB200::performRegistration() {
   std::cout << "INFO: ICP correspondences size: " << reg.n_corr << std::endl;
   file_result << std::fixed << std::setprecision(5) << "Aligned cloud: " << eigenMatrix4(reg.transformation, 5) << std::endl;
   file_result << std::fixed << std::setprecision(5) << "Aligned results: " << reg.fitness << " " << reg.n_corr << std::endl;
-  // the other GPUs apply the same transformation to their copy of the (down-sampled) cloud
-  for (int r = 1; r < gpus_.size(); ++r)
-    if (me_transform(gpus_.ctx(r), ME_CLOUD_EST, reg.transformation) != ME_OK) return fail("me_transform (aligned cloud)");
   // calculateMetrics(reg) (:1147-1202): est->gt on the ICP correspondences (NN within R, strict), gt->est through
   // EvaluateRegistration(gt, est, R) (:1168), cd_vec (:1171), full Chamfer distance (:1194)
   TicToc tic;

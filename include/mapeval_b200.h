@@ -254,6 +254,40 @@ ME_API int  me_icp_point_to_point(me_ctx *ctx, double max_correspondence_distanc
  * me_icp_point_to_point; normals the estimated cloud held are rotated by the result, the ground truth's are unchanged. */
 ME_API int  me_icp(me_ctx *ctx, int32_t method, double max_correspondence_distance, int32_t max_iteration,
                    double relative_fitness, double relative_rmse, const double T_init[16], me_icp_result *out);
+/* Registration on every rank of a multi-GPU job: me_icp split at its collective (me_icp is this sequence at world = 1).
+ * Both clouds are replicated; every rank runs the same calls with the same arguments:
+ *   me_icp_begin                        checks as me_icp, keeps a copy of the estimated cloud
+ *   me_icp_normals_slice(EST), (GT)     generalized ICP, cloud without normals: this rank's k-NN normals (KNN 20) of the
+ *                                       caller indices [rank s, (rank + 1) s), s = *slice_points = ceil(N / world), into
+ *                                       *device_normals, a buffer of world * s * 3 doubles (caller order).  *pending = 1:
+ *                                       the caller all-gathers it in place (ncclAllGather, sendbuff = *device_normals +
+ *                                       rank * s * 3, s * 3 doubles).  *pending = 0 and NULL: nothing to gather (the cloud's
+ *                                       own normals are used, another method, or world = 1).  The gathered normals are
+ *                                       bit-identical to me_estimate_normals at world = 1.
+ *   me_icp_block                        the first call moves the cloud by T_init and sweeps; every call hands out the DEVICE
+ *                                       address of the fp64 block of this rank's partial sums (*n_sum values: count first,
+ *                                       exact below 2^53).  The caller SUM-all-reduces it in place.
+ *   me_icp_step(&done)                  reads the reduced block: convergence test, update, move, sweep -> the next block
+ *                                       (same address); *done = 1: nothing left to reduce
+ *   me_icp_end                          est := Transform(original, T) with the result, as me_icp leaves it
+ * The device work of a call is queued on the context's stream: the caller orders its collective after it (me_synchronize,
+ * or a collective on that stream).  Out of order calls (step / block / end before begin, a block or step with normals still
+ * pending, a step before the first block) fail with ME_ERR_INVALID; any failure while a registration is open closes it
+ * and leaves the estimated cloud as it was handed in.  A context of world > 1 with ME_LAYOUT_SLAB requested refuses
+ * me_icp_begin: the sweeps of the registration run on the replicated layout (set it for the registration, back afterwards). */
+#define ME_ICP_BLOCK_P2P 17   /* count, sum p (3), sum q (3), sum q p^T (9, row-major), sum d2; p, q about the centre */
+#define ME_ICP_BLOCK_NE 29    /* count, J^T J upper triangle (21, row-major), J^T r (6), sum d2 */
+ME_API int  me_icp_begin(me_ctx *ctx, int32_t method, double max_correspondence_distance, int32_t max_iteration,
+                         double relative_fitness, double relative_rmse, const double T_init[16]);
+ME_API int  me_icp_normals_slice(me_ctx *ctx, int which, double **device_normals, int64_t *slice_points, int32_t *pending);
+ME_API int  me_icp_block(me_ctx *ctx, double **device_block, int32_t *n_sum);
+ME_API int  me_icp_step(me_ctx *ctx, int32_t *done);
+ME_API int  me_icp_end(me_ctx *ctx, me_icp_result *out);
+/* The update of one iteration from a reduced block as a pure host function (no context, no device): Eigen::umeyama
+ * without scaling (point-to-point; the sums are taken about `center`, the centre of the ground truth's bounding box), or
+ * the 6x6 normal equations solved with partial pivoting + TransformVector6dToMatrix4d (point-to-plane, generalized ICP;
+ * center may be NULL).  The identity when the count is 0 or the solve fails (Open3D).  update: row-major 4x4. */
+ME_API int  me_icp_update(int32_t method, const double *block, const double center[3], double update[16]);
 /* normals of a cloud held by the context, caller order, N x 3 fp64 (open3d PointCloud::normals_): upload / estimate as
  * PointCloud::EstimateNormals(KDTreeSearchParamKNN(knn)) does (k nearest neighbours incl. the point, covariance, the
  * eigenvector of the smallest eigenvalue; sign as Open3D's FastEigen3x3 leaves it) / read back.  me_transform rotates them. */
