@@ -22,6 +22,7 @@ SYMBOLS = (
     "me_set_layout", "me_layout_active", "me_voxel_begin", "me_voxel_w_table", "me_voxel_finish_accum_device", "me_accum_fetch_awd",
     "me_plan_slab_cut", "me_plan_lattice", "me_kernel_trace",
     "me_icp_begin", "me_icp_normals_slice", "me_icp_block", "me_icp_step", "me_icp_end", "me_icp_update",
+    "me_copy_cloud", "me_add_gaussian_noise", "me_add_non_uniform_density", "me_add_sparse_outliers", "me_add_local_deformation",
 )
 
 _lib = None
@@ -68,6 +69,11 @@ def load():
     L.me_get_normals.argtypes = [ctx, C.c_int, dp]
     L.me_voxel_downsample.argtypes = [ctx, C.c_int, C.c_double, C.POINTER(C.c_int64)]
     L.me_get_cloud.argtypes = [ctx, C.c_int, dp, C.c_int64, C.POINTER(C.c_int64)]
+    L.me_copy_cloud.argtypes = [ctx, C.c_int, C.c_int]
+    L.me_add_gaussian_noise.argtypes = [ctx, C.c_int, C.c_double, C.c_uint64]
+    L.me_add_non_uniform_density.argtypes = [ctx, C.c_int, C.c_double, C.c_double, C.c_double, C.c_uint64, C.POINTER(C.c_int64)]
+    L.me_add_sparse_outliers.argtypes = [ctx, C.c_int, C.c_double, C.c_double, C.c_uint64, C.POINTER(C.c_int64)]
+    L.me_add_local_deformation.argtypes = [ctx, C.c_int, C.c_double, C.c_double, dp]
     L.me_build_grid.argtypes = [ctx, C.c_int]
     L.me_eval_nn_accum.argtypes = [ctx, C.POINTER(A.me_nn_params), C.POINTER(A.me_nn_accum), C.POINTER(A.me_nn_accum)]
     L.me_nn_finalize.argtypes = [C.POINTER(A.me_nn_params), C.POINTER(A.me_nn_accum), C.POINTER(A.me_nn_accum),

@@ -187,6 +187,40 @@ class MapEvalB200:
         self._keep[which] = None
         return n.value
 
+    # -- simulated degradation (evaluate_noised_gt; map_eval.cpp:1745-1829): pure functions of (cloud, parameters, seed) -------
+    def copy_cloud(self, src, dst):
+        """dst := src (points, and normals when src holds them) in library-owned memory; also turns a borrowed ground
+        truth into an owned estimate that the operators below may change."""
+        self._check(self._L.me_copy_cloud(self._ctx, int(src), int(dst)))
+        self.n[dst] = self.n[src]
+        self._keep[dst] = None
+
+    def add_gaussian_noise(self, which, std_dev, seed):
+        """MapEval::addGaussianNoise: p += std_dev * N(0, 1) per axis, in place."""
+        self._check(self._L.me_add_gaussian_noise(self._ctx, int(which), float(std_dev), int(seed)))
+
+    def add_non_uniform_density(self, which, sparse_ratio, dense_ratio, region_size, seed):
+        """MapEval::addNonUniformDensity (stable compaction); returns the new point count."""
+        n = C.c_int64(0)
+        self._check(self._L.me_add_non_uniform_density(self._ctx, int(which), float(sparse_ratio), float(dense_ratio),
+                                                       float(region_size), int(seed), C.byref(n)))
+        self.n[which] = n.value
+        return n.value
+
+    def add_sparse_outliers(self, which, outlier_ratio, outlier_range, seed):
+        """MapEval::addSparseOutliers (outliers appended; the cloud loses its normals); returns the new point count."""
+        n = C.c_int64(0)
+        self._check(self._L.me_add_sparse_outliers(self._ctx, int(which), float(outlier_ratio), float(outlier_range), int(seed),
+                                                   C.byref(n)))
+        self.n[which] = n.value
+        return n.value
+
+    def add_local_deformation(self, which, radius, strength, center):
+        """MapEval::addLocalDeformation: radial push inside the radius, cosine fall-off, in place."""
+        c = np.ascontiguousarray(center, dtype=np.float64).reshape(3)
+        self._check(self._L.me_add_local_deformation(self._ctx, int(which), float(radius), float(strength),
+                                                     c.ctypes.data_as(C.POINTER(C.c_double))))
+
     def get_cloud(self, which):
         """The cloud currently held by the context as an (N, 3) float64 array."""
         n = C.c_int64(0)

@@ -405,6 +405,42 @@ int me_voxel_downsample(me_ctx *ctx, int which, double voxel_size, int64_t *n_ou
   return voxel_downsample(ctx, which, voxel_size, n_out);
 }
 
+static bool cloud_id(int which) { return which == ME_CLOUD_EST || which == ME_CLOUD_GT; }
+
+int me_copy_cloud(me_ctx *ctx, int src, int dst) {
+  ME_ENTER(ctx);
+  if (!cloud_id(src) || !cloud_id(dst) || src == dst) return fail(ctx, ME_ERR_INVALID, "me_copy_cloud: src and dst must be the two clouds");
+  return copy_cloud(ctx, src, dst);
+}
+
+int me_add_gaussian_noise(me_ctx *ctx, int which, double std_dev, uint64_t seed) {
+  ME_ENTER(ctx);
+  if (!cloud_id(which)) return fail(ctx, ME_ERR_INVALID, "bad cloud id");
+  if (!(std::isfinite(std_dev) && std_dev >= 0.0)) return fail(ctx, ME_ERR_INVALID, "me_add_gaussian_noise: std_dev must be finite and >= 0");
+  return add_gaussian_noise(ctx, which, std_dev, seed);
+}
+
+int me_add_non_uniform_density(me_ctx *ctx, int which, double sparse_ratio, double dense_ratio, double region_size, uint64_t seed,
+                               int64_t *n_out) {
+  ME_ENTER(ctx);
+  if (!cloud_id(which)) return fail(ctx, ME_ERR_INVALID, "bad cloud id");
+  return add_non_uniform_density(ctx, which, sparse_ratio, dense_ratio, region_size, seed, n_out);
+}
+
+int me_add_sparse_outliers(me_ctx *ctx, int which, double outlier_ratio, double outlier_range, uint64_t seed, int64_t *n_out) {
+  ME_ENTER(ctx);
+  if (!cloud_id(which)) return fail(ctx, ME_ERR_INVALID, "bad cloud id");
+  if (!(std::isfinite(outlier_range) && outlier_range >= 0.0))
+    return fail(ctx, ME_ERR_INVALID, "me_add_sparse_outliers: outlier_range must be finite and >= 0");
+  return add_sparse_outliers(ctx, which, outlier_ratio, outlier_range, seed, n_out);
+}
+
+int me_add_local_deformation(me_ctx *ctx, int which, double radius, double strength, const double center[3]) {
+  ME_ENTER(ctx);
+  if (!cloud_id(which) || !center) return fail(ctx, ME_ERR_INVALID, "bad arguments");
+  return add_local_deformation(ctx, which, radius, strength, center);
+}
+
 int me_get_cloud(me_ctx *ctx, int which, double *xyz_host, int64_t capacity_points, int64_t *n) {
   ME_ENTER(ctx);
   if (which != ME_CLOUD_EST && which != ME_CLOUD_GT) return fail(ctx, ME_ERR_INVALID, "bad cloud id");

@@ -353,6 +353,13 @@ int estimate_normals(me_ctx *ctx, int which, int knn, long long lo = 0, long lon
 void invalidate_cloud(Cloud &c);      // the cloud's coordinates changed: bbox, lattice, NN and entropy results are stale
 int run_awd_rows(me_ctx *ctx, const double *rows27, int64_t n_rows, double voxel_size, int scs_radius, double *w_out,
                  me_awd_result *out);
+// degraded copies of a cloud (perturb.cu)
+int copy_cloud(me_ctx *ctx, int src, int dst);
+int add_gaussian_noise(me_ctx *ctx, int which, double std_dev, uint64_t seed);
+int add_non_uniform_density(me_ctx *ctx, int which, double sparse_ratio, double dense_ratio, double region_size, uint64_t seed,
+                            int64_t *n_out);
+int add_sparse_outliers(me_ctx *ctx, int which, double outlier_ratio, double outlier_range, uint64_t seed, int64_t *n_out);
+int add_local_deformation(me_ctx *ctx, int which, double radius, double strength, const double center[3]);
 
 // ------------------------------------------------------------------------------------------------
 // device helpers

@@ -73,6 +73,14 @@ struct Param {   // map_eval.h:60-116
   int gpu_device_ = 0;
   int n_gpus_ = 1;                      // GPUs gpu_device_ .. gpu_device_ + n_gpus_ - 1 share the sweeps (NCCL all-reduce)
   bool geometric_gt_pairing_ = false;   // false = reproduce map_eval.cpp:1233/:1241 verbatim
+  // evaluate_noised_gt: the degradation of the ground truth that stands in for the estimate (map_eval.cpp:1745-1829); the
+  // operators run in the order deformation -> density -> noise -> outliers, every draw a function of simulation_seed_
+  uint64_t simulation_seed_ = 20250002;   // synth.EST_SEED
+  bool density_set_ = false;            // density is applied when density_region_size is given
+  double density_sparse_ratio_ = 0.5, density_dense_ratio_ = 1.0, density_region_size_ = 0.0;
+  double outlier_ratio_ = 0.0, outlier_range_ = 1.0;   // applied when outlier_ratio > 0
+  double deform_radius_ = 0.0, deform_strength_ = 0.0; // applied when deform_radius > 0
+  double deform_center_[3] = {0, 0, 0};
 };
 
 // map_eval_main.cpp:120-208
@@ -113,6 +121,19 @@ inline Param loadParametersFromYAML(const std::string &yaml_file_path) {
     if (config["gpu_device"]) param.gpu_device_ = config["gpu_device"].as<int>();
     if (config["n_gpus"]) param.n_gpus_ = config["n_gpus"].as<int>();
     if (config["geometric_gt_pairing"]) param.geometric_gt_pairing_ = config["geometric_gt_pairing"].as<bool>();
+    if (config["simulation_seed"]) param.simulation_seed_ = config["simulation_seed"].as<uint64_t>();
+    if (config["density_sparse_ratio"]) param.density_sparse_ratio_ = config["density_sparse_ratio"].as<double>();
+    if (config["density_dense_ratio"]) param.density_dense_ratio_ = config["density_dense_ratio"].as<double>();
+    if (config["density_region_size"]) {
+      param.density_region_size_ = config["density_region_size"].as<double>();
+      param.density_set_ = true;
+    }
+    if (config["outlier_ratio"]) param.outlier_ratio_ = config["outlier_ratio"].as<double>();
+    if (config["outlier_range"]) param.outlier_range_ = config["outlier_range"].as<double>();
+    if (config["deform_radius"]) param.deform_radius_ = config["deform_radius"].as<double>();
+    if (config["deform_strength"]) param.deform_strength_ = config["deform_strength"].as<double>();
+    if (config["deform_center"] && config["deform_center"].size() >= 3)
+      for (int a = 0; a < 3; ++a) param.deform_center_[a] = config["deform_center"][a].as<double>();
     return param;
   } catch (const std::exception &e) {
     std::cerr << "Error loading parameters: " << e.what() << std::endl;
@@ -132,7 +153,11 @@ inline void dumpParam(const Param &p, std::ostream &os) {
      << "\nestimate_map_path=" << p.evaluation_map_pcd_path_ << "\ngt_map_path=" << p.map_gt_path_ << "\nscene_name=" << p.name_
      << "\nresult_path=" << p.result_path_ << "\npcd_file_name=" << p.pcd_file_name_ << "\nevaluate_noised_gt=" << p.evaluate_noised_gt_
      << "\nnoise_std_dev=" << p.noise_std_dev_ << "\nvoxel_size=" << p.voxel_size_ << "\nuse_visualization=" << p.use_visualization
-     << "\nenable_debug=" << p.enable_debug << "\nuse_tbb_mme=" << p.use_tbb_mme << "\n";
+     << "\nenable_debug=" << p.enable_debug << "\nuse_tbb_mme=" << p.use_tbb_mme << "\nsimulation_seed=" << p.simulation_seed_
+     << "\ndensity_sparse_ratio=" << p.density_sparse_ratio_ << "\ndensity_dense_ratio=" << p.density_dense_ratio_
+     << "\ndensity_region_size=" << p.density_region_size_ << "\ndensity_set=" << p.density_set_ << "\noutlier_ratio=" << p.outlier_ratio_
+     << "\noutlier_range=" << p.outlier_range_ << "\ndeform_radius=" << p.deform_radius_ << "\ndeform_strength=" << p.deform_strength_
+     << "\ndeform_center=" << p.deform_center_[0] << "," << p.deform_center_[1] << "," << p.deform_center_[2] << "\n";
 }
 
 // Eigen's default IOFormat for `vec.transpose()`: coefficients right-aligned to a common width, one space apart
@@ -249,6 +274,8 @@ class MapEvalB200 {
     return -1;
   }
   render::ColoredCloud map_3d_entropy_, gt_3d_entropy_, map_3d_render_raw_, map_3d_render_inlier_;   // map_eval.h:341-347
+  int simulateEstimate(me_ctx *c, int64_t *n);     // evaluate_noised_gt: estimate := degraded copy of the ground truth
+  std::string simulationSummary() const;
   int renderEntropy(int which, int64_t n, render::ColoredCloud *out);
   int renderDistances(bool cutoff_strict);
   GpuGroup gpus_;            // one context per GPU; rank r evaluates the r-th shard of every sweep's query range
@@ -281,15 +308,19 @@ inline int MapEvalB200::process() {
     return -1;
   }
   if (!gt_ok && param_.enable_debug) std::cerr << "WARNING: " << err << std::endl;   // the reference ignores this return value
-  bool success = cloud_io::read_pcd(param_.evaluation_map_pcd_path_ + param_.pcd_file_name_, map_3d_, &err,
-                                    load_normals ? &map_normals_ : nullptr);
-  if (param_.enable_debug)
-    std::cout << "INFO: Loading map point cloud from: " << param_.evaluation_map_pcd_path_ + param_.pcd_file_name_ << std::endl;
-  if (!success) {
-    std::cerr << "ERROR: Failed to load point cloud from the specified path." << std::endl;
-    return -1;
+  // evaluate_noised_gt (config.yaml:55-59): the estimate file is not read; every GPU degrades a copy of the ground truth
+  const bool simulate = param_.evaluate_noised_gt_;
+  if (!simulate) {
+    bool success = cloud_io::read_pcd(param_.evaluation_map_pcd_path_ + param_.pcd_file_name_, map_3d_, &err,
+                                      load_normals ? &map_normals_ : nullptr);
+    if (param_.enable_debug)
+      std::cout << "INFO: Loading map point cloud from: " << param_.evaluation_map_pcd_path_ + param_.pcd_file_name_ << std::endl;
+    if (!success) {
+      std::cerr << "ERROR: Failed to load point cloud from the specified path." << std::endl;
+      return -1;
+    }
   }
-  if (map_3d_.empty() || gt_3d_.empty()) {
+  if ((!simulate && map_3d_.empty()) || gt_3d_.empty()) {
     std::cerr << "ERROR: One or both point clouds are empty!" << std::endl;
     return -1;
   }
@@ -307,11 +338,13 @@ inline int MapEvalB200::process() {
   std::vector<int64_t> ne(gpus_.size(), (int64_t)(map_3d_.size() / 3)), ng(gpus_.size(), (int64_t)(gt_3d_.size() / 3));
   const bool map_has_normals = !map_normals_.empty() && map_normals_.size() == map_3d_.size();
   const bool gt_has_normals = !gt_normals_.empty() && gt_normals_.size() == gt_3d_.size();
+  if (simulate) std::cout << "INFO: " << simulationSummary() << std::endl;
   if (gpus_.for_each([&](int r, me_ctx *c) {
-        int rc = me_set_cloud(c, ME_CLOUD_EST, map_3d_.data(), (int64_t)(map_3d_.size() / 3));
+        int rc = simulate ? ME_OK : me_set_cloud(c, ME_CLOUD_EST, map_3d_.data(), (int64_t)(map_3d_.size() / 3));
         if (rc == ME_OK) rc = me_set_cloud(c, ME_CLOUD_GT, gt_3d_.data(), (int64_t)(gt_3d_.size() / 3));
         if (rc == ME_OK && map_has_normals) rc = me_set_normals(c, ME_CLOUD_EST, map_normals_.data(), (int64_t)(map_normals_.size() / 3));
         if (rc == ME_OK && gt_has_normals) rc = me_set_normals(c, ME_CLOUD_GT, gt_normals_.data(), (int64_t)(gt_normals_.size() / 3));
+        if (rc == ME_OK && simulate) rc = simulateEstimate(c, &ne[r]);
         if (rc == ME_OK && param_.downsample_size > 0) {
           rc = me_voxel_downsample(c, ME_CLOUD_EST, param_.downsample_size, &ne[r]);
           if (rc == ME_OK) rc = me_voxel_downsample(c, ME_CLOUD_GT, param_.downsample_size, &ng[r]);
@@ -353,6 +386,59 @@ inline int MapEvalB200::process() {
   }
   if (param_.enable_debug) std::cout << "INFO: Results saved successfully." << std::endl;
   return 0;
+}
+
+// evaluate_noised_gt: the reference's simulation operators (map_eval.cpp:1745-1829) on a copy of the ground truth, in the
+// order deformation -> density -> noise -> outliers (outliers are drawn from the already noisy map, as addSparseOutliers
+// copies points of the cloud it gets).  Every draw is a function of simulation_seed, so every GPU builds the same map.
+inline int MapEvalB200::simulateEstimate(me_ctx *c, int64_t *n) {
+  const Param &p = param_;
+  const uint64_t seed = p.simulation_seed_;
+  *n = (int64_t)(gt_3d_.size() / 3);
+  int rc = me_copy_cloud(c, ME_CLOUD_GT, ME_CLOUD_EST);      // with the ground truth's normals when they were loaded
+  if (rc == ME_OK && p.deform_radius_ > 0)
+    rc = me_add_local_deformation(c, ME_CLOUD_EST, p.deform_radius_, p.deform_strength_, p.deform_center_);
+  if (rc == ME_OK && p.density_set_)
+    rc = me_add_non_uniform_density(c, ME_CLOUD_EST, p.density_sparse_ratio_, p.density_dense_ratio_, p.density_region_size_, seed, n);
+  if (rc == ME_OK && p.noise_std_dev_ != 0) rc = me_add_gaussian_noise(c, ME_CLOUD_EST, p.noise_std_dev_, seed);
+  if (rc == ME_OK && p.outlier_ratio_ > 0) rc = me_add_sparse_outliers(c, ME_CLOUD_EST, p.outlier_ratio_, p.outlier_range_, seed, n);
+  return rc;
+}
+
+inline std::string MapEvalB200::simulationSummary() const {
+  const Param &p = param_;
+  std::ostringstream os;
+  os << std::setprecision(6) << "evaluate_noised_gt: the estimated map is not read; it is the ground truth";
+  std::vector<std::string> ops;
+  if (p.deform_radius_ > 0) {
+    std::ostringstream o;
+    o << std::setprecision(6) << "local deformation (radius " << p.deform_radius_ << ", strength " << p.deform_strength_ << ", centre " << p.deform_center_[0]
+      << " " << p.deform_center_[1] << " " << p.deform_center_[2] << ")";
+    ops.push_back(o.str());
+  }
+  if (p.density_set_) {
+    std::ostringstream o;
+    o << std::setprecision(6) << "non-uniform density (sparse " << p.density_sparse_ratio_ << ", dense " << p.density_dense_ratio_ << ", region "
+      << p.density_region_size_ << ")";
+    ops.push_back(o.str());
+  }
+  if (p.noise_std_dev_ != 0) {
+    std::ostringstream o;
+    o << std::setprecision(6) << "Gaussian noise (std_dev " << p.noise_std_dev_ << ")";
+    ops.push_back(o.str());
+  }
+  if (p.outlier_ratio_ > 0) {
+    std::ostringstream o;
+    o << std::setprecision(6) << "sparse outliers (ratio " << p.outlier_ratio_ << ", range " << p.outlier_range_ << ")";
+    ops.push_back(o.str());
+  }
+  if (ops.empty()) os << " unchanged";
+  for (size_t i = 0; i < ops.size(); ++i) os << (i ? ", then " : " with ") << ops[i];
+  os << " (simulation_seed " << p.simulation_seed_ << ")";
+  static const double eye[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  if (!std::equal(p.initial_matrix_, p.initial_matrix_ + 16, eye))
+    os << "; initial_matrix is not the identity, but the simulated map lies in the ground truth's frame";
+  return os.str();
 }
 
 // ColorPointCloudByMME (map_eval.cpp:686-736) on the entropies of the sweep that just ran (each GPU holds its shard)
@@ -647,4 +733,16 @@ inline void MapEvalB200::saveRegistrationResults() {   // map_eval.cpp:424-482
   else if (param_.enable_debug) std::cout << "INFO: Saved raw distance error map to " << results_subfolder + "raw_rendered_dis_map.pcd" << std::endl;
   if (!render::write_pcd(results_subfolder + "inlier_rendered_dis_map.pcd", map_3d_render_inlier_)) std::cerr << "ERROR: cannot write inlier_rendered_dis_map.pcd" << std::endl;
   else if (param_.enable_debug) std::cout << "INFO: Saved inlier distance error map to " << results_subfolder + "inlier_rendered_dis_map.pcd" << std::endl;
+  // map_eval.cpp:502-507: the estimated cloud as held here (down-sampled and registered, like map_3d_ there), no normals
+  if (param_.evaluate_noised_gt_) {
+    int64_t n = 0;
+    std::vector<double> xyz;
+    bool ok = me_get_cloud(ctx_, ME_CLOUD_EST, nullptr, 0, &n) == ME_OK;
+    if (ok) {
+      xyz.resize((size_t)n * 3);
+      ok = me_get_cloud(ctx_, ME_CLOUD_EST, xyz.data(), n, &n) == ME_OK;
+    }
+    if (!ok || !render::write_pcd_xyz(results_subfolder + "noise_gt_map.pcd", xyz)) std::cerr << "ERROR: cannot write noise_gt_map.pcd" << std::endl;
+    else if (param_.enable_debug) std::cout << "INFO: Saved noisy ground truth map to " << results_subfolder + "noise_gt_map.pcd" << std::endl;
+  }
 }

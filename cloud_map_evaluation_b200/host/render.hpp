@@ -104,4 +104,17 @@ inline bool write_pcd(const std::string &path, const ColoredCloud &c) {
   return (bool)f;
 }
 
+// the same binary layout without colours: FIELDS x y z, float32 (noise_gt_map.pcd, map_eval.cpp:502-507)
+inline bool write_pcd_xyz(const std::string &path, const std::vector<double> &xyz) {
+  std::ofstream f(path, std::ios::binary);
+  if (!f.is_open()) return false;
+  const size_t n = xyz.size() / 3;
+  f << "# .PCD v0.7 - Point Cloud Data file format\nVERSION 0.7\nFIELDS x y z\nSIZE 4 4 4\nTYPE F F F\nCOUNT 1 1 1\n"
+    << "WIDTH " << n << "\nHEIGHT 1\nVIEWPOINT 0 0 0 1 0 0 0\nPOINTS " << n << "\nDATA binary\n";
+  std::vector<float> buf(n * 3);
+  for (size_t i = 0; i < n * 3; ++i) buf[i] = (float)xyz[i];
+  f.write((const char *)buf.data(), (std::streamsize)(buf.size() * sizeof(float)));
+  return (bool)f;
+}
+
 }  // namespace render

@@ -7,6 +7,7 @@
 // the loader's observable behaviour: as<T>() of a missing key or of a malformed scalar throws.
 #pragma once
 #include <cctype>
+#include <cstdint>
 #include <fstream>
 #include <map>
 #include <sstream>
@@ -104,6 +105,14 @@ template <> inline int Node::as<int>() const {
   try { v = std::stol(scalar, &pos); } catch (...) { throw std::runtime_error("yaml: bad conversion of key '" + key + "' ('" + scalar + "') to int"); }
   if (pos != scalar.size()) throw std::runtime_error("yaml: bad conversion of key '" + key + "' ('" + scalar + "') to int");
   return (int)v;
+}
+template <> inline uint64_t Node::as<uint64_t>() const {
+  if (kind != Scalar || scalar.empty() || scalar[0] == '-') throw std::runtime_error("yaml: bad conversion of key '" + key + "' to uint64");
+  size_t pos = 0;
+  unsigned long long v = 0;
+  try { v = std::stoull(scalar, &pos); } catch (...) { throw std::runtime_error("yaml: bad conversion of key '" + key + "' ('" + scalar + "') to uint64"); }
+  if (pos != scalar.size()) throw std::runtime_error("yaml: bad conversion of key '" + key + "' ('" + scalar + "') to uint64");
+  return (uint64_t)v;
 }
 template <> inline bool Node::as<bool>() const {
   if (kind != Scalar) throw std::runtime_error("yaml: bad conversion of key '" + key + "' to bool");

@@ -236,6 +236,40 @@ ME_API int  me_voxel_downsample(me_ctx *ctx, int which, double voxel_size, int64
 /* the cloud currently held by the context (after me_transform / me_voxel_downsample), caller order, N x 3 fp64.
  * xyz_host == NULL: size query only (*n).  capacity_points < N is an error. */
 ME_API int  me_get_cloud(me_ctx *ctx, int which, double *xyz_host, int64_t capacity_points, int64_t *n);
+
+/* ---- simulated degradation of a map (evaluate_noised_gt: map_eval.h:79,87, config.yaml:55-59) ---------------------------
+ * The operators of MapEval::addGaussianNoise / addNonUniformDensity / addSparseOutliers / addLocalDeformation
+ * (map_eval.cpp:1745-1829, map_eval.h:296-310) on a cloud held by the context, applied in the order the caller calls them,
+ * on library-owned buffers.  Borrowed clouds (me_set_cloud_device) are refused with ME_ERR_INVALID: the operators never
+ * write caller memory.  Afterwards the cloud's lattice and per-point results are stale, as after me_transform.
+ * The reference draws from std::random_device; here every draw is the counter-based hash of synth.py — splitmix64 of
+ * (seed, index, lane) — so a degraded cloud is a pure function of (cloud, parameters, seed), identical on every GPU of a
+ * job, and its kept points, counts and outlier bases equal a numpy statement bit for bit.  The lanes of the four operators
+ * are disjoint (noise 0-5, density 6, outliers 7-13), so one seed serves them all. */
+/* dst := src, points and normals (when src holds them), into library-owned memory; src != dst.  This is how a borrowed
+ * ground truth becomes an owned estimate. */
+ME_API int  me_copy_cloud(me_ctx *ctx, int src, int dst);
+/* addGaussianNoise (:1745-1755): p_a += std_dev * gaussian(seed, i, 2a), a = x, y, z (Box-Muller, u1 = max(u24, 2^-25)),
+ * in place.  std_dev finite and >= 0; 0 leaves the cloud unchanged.  Normals are untouched (the reference moves points_). */
+ME_API int  me_add_gaussian_noise(me_ctx *ctx, int which, double std_dev, uint64_t seed);
+/* addNonUniformDensity (:1757-1784): xn = sin(x / region_size * pi), yn = sin(y / region_size * pi); threshold =
+ * sparse_ratio if xn * yn > 0, else dense_ratio; the point is kept iff uniform24(seed, i, 6) < threshold.  Stable: the kept
+ * points keep their order, and normals go with their points.  region_size = 0 gives NaN signs: every point takes
+ * dense_ratio, as in the reference.  *n_out (nullable) = the new point count. */
+ME_API int  me_add_non_uniform_density(me_ctx *ctx, int which, double sparse_ratio, double dense_ratio, double region_size,
+                                       uint64_t seed, int64_t *n_out);
+/* addSparseOutliers (:1786-1806): m = (int)(N * outlier_ratio) outliers (none for a negative ratio) appended after the N
+ * points in j order: base = min(floor(uniform53(seed, j, 7) * N), N - 1), uniform53 = (h >> 11) * 2^-53, and
+ * o_a = p_base,a + outlier_range * gaussian(seed, j, 8 + 2a).  outlier_range finite and >= 0.  ME_ERR_RANGE when
+ * N * outlier_ratio >= 2^31 or N + m >= 2^31 - 1.  The cloud loses its normals (Open3D: HasNormals() is false once
+ * normals_ and points_ differ in size), so generalized ICP estimates them.  *n_out (nullable) = N + m. */
+ME_API int  me_add_sparse_outliers(me_ctx *ctx, int which, double outlier_ratio, double outlier_range, uint64_t seed,
+                                   int64_t *n_out);
+/* addLocalDeformation (:1808-1829): d = sqrt of Eigen's squaredNorm of p - c; where d < radius (strict),
+ * w = 0.5 (1 + cos(pi d / radius)) and p += ((p - c) / d * strength) * w, every operation rounded on its own (no FMA); the
+ * point at the centre stays (Eigen's normalize() leaves a zero vector).  No draws.  radius <= 0 moves nothing.  Normals are
+ * untouched. */
+ME_API int  me_add_local_deformation(me_ctx *ctx, int which, double radius, double strength, const double center[3]);
 /* replaces: MapEval::performICPRegistration case 0 (map_eval.cpp:1366-1394): open3d RegistrationICP(est, gt,
  * icp_max_distance, initial_matrix, TransformationEstimationPointToPoint(), ICPConvergenceCriteria{relative_fitness,
  * relative_rmse, max_iteration} = {1e-6, 1e-6, 30}).  On return the estimated cloud held by the context is the original
