@@ -96,25 +96,43 @@ icp_accum_kernel(const P4 *__restrict__ Q, long long qb, long long qe, const int
 }
 
 // ---- host 3x3 algebra -------------------------------------------------------------------------------------------
-static void eig3_sym_host(const double a_in[9], double w[3], double v[9]) {      // cyclic Jacobi, ascending not guaranteed
+// SVD of a 3x3 by one-sided Jacobi (Hestenes): plane rotations V orthogonalise the columns of a = sigma V, so
+// sigma = U diag(w) V^T with U's columns a_j / w_j.  It works on sigma itself: the eigen-problem of sigma^T sigma would
+// square the condition number, and with it the error of the small singular values (a tilted near-planar cloud made R
+// a shear of a few per cent).  Singular values descending; only U's first two columns are formed.
+static void svd3_host(const double s_in[9], double U[9], double w[3], double V[9]) {
   double a[9];
-  for (int i = 0; i < 9; ++i) { a[i] = a_in[i]; v[i] = (i % 4 == 0) ? 1.0 : 0.0; }
-  for (int sweep = 0; sweep < 64; ++sweep) {
-    const double off = a[1] * a[1] + a[2] * a[2] + a[5] * a[5], diag = a[0] * a[0] + a[4] * a[4] + a[8] * a[8];
-    if (off <= 1e-40 * diag || off == 0.0) break;
+  for (int i = 0; i < 9; ++i) { a[i] = s_in[i]; V[i] = (i % 4 == 0) ? 1.0 : 0.0; }
+  for (int sweep = 0; sweep < 60; ++sweep) {
+    double off = 0.0;
     for (int p = 0; p < 2; ++p)
       for (int q = p + 1; q < 3; ++q) {
-        const double apq = a[p * 3 + q];
-        if (apq == 0.0) continue;
-        const double theta = (a[q * 3 + q] - a[p * 3 + p]) / (2.0 * apq);
-        const double t = (theta >= 0 ? 1.0 : -1.0) / (std::fabs(theta) + std::sqrt(theta * theta + 1.0));
-        const double c = 1.0 / std::sqrt(t * t + 1.0), s = t * c;
-        for (int k = 0; k < 3; ++k) { const double x = a[k * 3 + p], y = a[k * 3 + q]; a[k * 3 + p] = c * x - s * y; a[k * 3 + q] = s * x + c * y; }
-        for (int k = 0; k < 3; ++k) { const double x = a[p * 3 + k], y = a[q * 3 + k]; a[p * 3 + k] = c * x - s * y; a[q * 3 + k] = s * x + c * y; }
-        for (int k = 0; k < 3; ++k) { const double x = v[k * 3 + p], y = v[k * 3 + q]; v[k * 3 + p] = c * x - s * y; v[k * 3 + q] = s * x + c * y; }
+        double alpha = 0, beta = 0, gamma = 0;
+        for (int k = 0; k < 3; ++k) { alpha += a[k * 3 + p] * a[k * 3 + p]; beta += a[k * 3 + q] * a[k * 3 + q]; gamma += a[k * 3 + p] * a[k * 3 + q]; }
+        if (gamma == 0.0) continue;
+        off = std::max(off, std::fabs(gamma) / std::sqrt(alpha * beta));
+        const double zeta = (beta - alpha) / (2.0 * gamma);
+        const double t = (zeta >= 0 ? 1.0 : -1.0) / (std::fabs(zeta) + std::sqrt(1.0 + zeta * zeta));
+        const double c = 1.0 / std::sqrt(1.0 + t * t), s = c * t;
+        for (int k = 0; k < 3; ++k) {
+          const double ap = a[k * 3 + p], aq = a[k * 3 + q];
+          a[k * 3 + p] = c * ap - s * aq; a[k * 3 + q] = s * ap + c * aq;
+          const double vp = V[k * 3 + p], vq = V[k * 3 + q];
+          V[k * 3 + p] = c * vp - s * vq; V[k * 3 + q] = s * vp + c * vq;
+        }
       }
+    if (off < 1e-15) break;
   }
-  w[0] = a[0]; w[1] = a[4]; w[2] = a[8];
+  double nw[3];
+  for (int j = 0; j < 3; ++j) nw[j] = std::sqrt(a[j] * a[j] + a[3 + j] * a[3 + j] + a[6 + j] * a[6 + j]);
+  int ord[3] = {0, 1, 2};
+  std::sort(ord, ord + 3, [&](int x, int y) { return nw[x] > nw[y]; });
+  double Vs[9];
+  for (int j = 0; j < 3; ++j) {
+    w[j] = nw[ord[j]];
+    for (int k = 0; k < 3; ++k) { Vs[k * 3 + j] = V[k * 3 + ord[j]]; U[k * 3 + j] = j < 2 && w[j] > 0 ? a[k * 3 + ord[j]] / w[j] : 0.0; }
+  }
+  std::memcpy(V, Vs, sizeof(Vs));
 }
 static double det3_host(const double *m) {
   return m[0] * (m[4] * m[8] - m[5] * m[7]) - m[1] * (m[3] * m[8] - m[5] * m[6]) + m[2] * (m[3] * m[7] - m[4] * m[6]);
@@ -129,26 +147,12 @@ static void umeyama_from_sums(const double *blk, const double c[3], double upd[1
   for (int k = 0; k < 3; ++k) { pm[k] = sp[k] / n; qm[k] = sq[k] / n; }
   for (int r = 0; r < 3; ++r)
     for (int col = 0; col < 3; ++col) sigma[r * 3 + col] = sqp[r * 3 + col] / n - qm[r] * pm[col];
-  // SVD through the symmetric eigen-problem of sigma^T sigma
-  double ata[9], w[3], V[9];
-  for (int r = 0; r < 3; ++r)
-    for (int col = 0; col < 3; ++col) { double s = 0; for (int k = 0; k < 3; ++k) s += sigma[k * 3 + r] * sigma[k * 3 + col]; ata[r * 3 + col] = s; }
-  eig3_sym_host(ata, w, V);
-  int ord[3] = {0, 1, 2};
-  std::sort(ord, ord + 3, [&](int x, int y) { return w[x] > w[y]; });
-  double Vs[9], U[9], sv[3];
-  for (int j = 0; j < 3; ++j) { sv[j] = std::sqrt(std::max(w[ord[j]], 0.0)); for (int k = 0; k < 3; ++k) Vs[k * 3 + j] = V[k * 3 + ord[j]]; }
-  for (int j = 0; j < 3; ++j)
-    for (int r = 0; r < 3; ++r) {
-      double s = 0;
-      for (int k = 0; k < 3; ++k) s += sigma[r * 3 + k] * Vs[k * 3 + j];
-      U[r * 3 + j] = sv[j] > 0 ? s / sv[j] : 0.0;
-    }
-  // re-orthonormalise: the third column from the first two whenever the smallest singular value is not well separated
-  if (!(sv[2] > 1e-8 * sv[0])) {
-    U[2] = U[3] * U[7] - U[6] * U[4]; U[5] = U[6] * U[1] - U[0] * U[7]; U[8] = U[0] * U[4] - U[3] * U[1];
-    if (det3_host(Vs) < 0) { U[2] = -U[2]; U[5] = -U[5]; U[8] = -U[8]; }      // keep det(U) det(V) > 0: no reflection is forced
-  }
+  double U[9], sv[3], Vs[9];
+  svd3_host(sigma, U, sv, Vs);
+  // U's third column is always the cross product of the first two: a_3 / w_3 carries an error of u w_1 / w_3 (and is
+  // undefined at rank 2), while R = U S V^T only needs the orientation of U, which the cross product fixes (det U = +1).
+  // Eigen's rule S_3 = -1 when det(U) det(V) < 0 then makes R a rotation; in exact arithmetic this is umeyama's R.
+  U[2] = U[3] * U[7] - U[6] * U[4]; U[5] = U[6] * U[1] - U[0] * U[7]; U[8] = U[0] * U[4] - U[3] * U[1];
   double S[3] = {1, 1, 1};
   if (det3_host(U) * det3_host(Vs) < 0) S[2] = -1;
   std::memset(upd, 0, 16 * sizeof(double));
