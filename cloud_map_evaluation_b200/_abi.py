@@ -138,6 +138,39 @@ class me_icp_result(C.Structure):
                 ("n_corr", C.c_int64), ("iterations", C.c_int32), ("converged", C.c_int32)]
 
 
+class me_global_reg_params(C.Structure):
+    _fields_ = [("voxel_size", C.c_double), ("normal_knn", C.c_int32), ("feature_radius", C.c_double),
+                ("feature_max_nn", C.c_int32), ("mutual_filter", C.c_int32), ("max_correspondence_distance", C.c_double),
+                ("edge_ratio", C.c_double), ("n_hypotheses", C.c_int64), ("seed", C.c_uint64)]
+
+
+class me_global_reg_result(C.Structure):
+    _fields_ = [("T", C.c_double * 16), ("n_est_features", C.c_int64), ("n_gt_features", C.c_int64),
+                ("n_correspondences", C.c_int64), ("n_valid_hypotheses", C.c_int64), ("best_hypothesis", C.c_int64),
+                ("n_inliers", C.c_int64), ("inlier_rmse", C.c_double), ("stage_ms", C.c_double * 6)]
+
+
+GLOBAL_REG_STAGES = ("copy_downsample", "normals", "fpfh", "matching", "ransac", "refine")
+
+
+FPFH_DIM = 33
+
+
+def make_global_reg_params(voxel_size, seed=0, **overrides):
+    """me_global_reg_params with the defaults of the header (feature radius 10 voxels, inlier distance 1.5 voxels, ...)"""
+    v = float(voxel_size)
+    vals = dict(voxel_size=v, normal_knn=30, feature_radius=10.0 * v, feature_max_nn=128, mutual_filter=1,
+                max_correspondence_distance=1.5 * v, edge_ratio=0.9, n_hypotheses=100000, seed=int(seed))
+    unknown = set(overrides) - set(vals)
+    if unknown:
+        raise ValueError(f"unknown global registration parameters: {sorted(unknown)}")
+    vals.update(overrides)
+    p = me_global_reg_params()
+    for k, x in vals.items():
+        setattr(p, k, x)
+    return p
+
+
 def make_nn_params(tau, icp_max_distance=1.0, cutoff_mode=ME_CUTOFF_SQDIST_LE_R, pairing=ME_PAIRING_AS_WRITTEN,
                    want_full_cd=True, directions=0):
     p = me_nn_params()

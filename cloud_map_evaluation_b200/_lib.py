@@ -23,6 +23,7 @@ SYMBOLS = (
     "me_plan_slab_cut", "me_plan_lattice", "me_kernel_trace",
     "me_icp_begin", "me_icp_normals_slice", "me_icp_block", "me_icp_step", "me_icp_end", "me_icp_update",
     "me_copy_cloud", "me_add_gaussian_noise", "me_add_non_uniform_density", "me_add_sparse_outliers", "me_add_local_deformation",
+    "me_global_registration", "me_get_features", "me_get_correspondences",
 )
 
 _lib = None
@@ -74,6 +75,9 @@ def load():
     L.me_add_non_uniform_density.argtypes = [ctx, C.c_int, C.c_double, C.c_double, C.c_double, C.c_uint64, C.POINTER(C.c_int64)]
     L.me_add_sparse_outliers.argtypes = [ctx, C.c_int, C.c_double, C.c_double, C.c_uint64, C.POINTER(C.c_int64)]
     L.me_add_local_deformation.argtypes = [ctx, C.c_int, C.c_double, C.c_double, dp]
+    L.me_global_registration.argtypes = [ctx, C.POINTER(A.me_global_reg_params), C.POINTER(A.me_global_reg_result)]
+    L.me_get_features.argtypes = [ctx, C.c_int, dp, dp, C.POINTER(C.c_float), C.c_int64, C.POINTER(C.c_int64)]
+    L.me_get_correspondences.argtypes = [ctx, C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
     L.me_build_grid.argtypes = [ctx, C.c_int]
     L.me_eval_nn_accum.argtypes = [ctx, C.POINTER(A.me_nn_params), C.POINTER(A.me_nn_accum), C.POINTER(A.me_nn_accum)]
     L.me_nn_finalize.argtypes = [C.POINTER(A.me_nn_params), C.POINTER(A.me_nn_accum), C.POINTER(A.me_nn_accum),

@@ -229,6 +229,40 @@ class MapEvalB200:
         self._check(self._L.me_get_cloud(self._ctx, which, out.ctypes.data_as(C.POINTER(C.c_double)), n.value, C.byref(n)))
         return out
 
+    # -- coarse global registration: the initial pose from the maps alone -----------------------------------------------
+    def global_registration(self, voxel_size, seed=0, **overrides):
+        """me_global_registration: FPFH features, mutual matching and RANSAC on private feature clouds down-sampled at
+        voxel_size; the context's clouds are left alone.  overrides: any other field of me_global_reg_params.  Returns a
+        dict of me_global_reg_result with T as a 4x4 array (est -> gt)."""
+        p = A.make_global_reg_params(voxel_size, seed, **overrides)
+        out = A.me_global_reg_result()
+        self._check(self._L.me_global_registration(self._ctx, C.byref(p), C.byref(out)))
+        r = A.struct_to_dict(out)
+        r["T"] = np.array(r["T"]).reshape(4, 4)
+        r["stage_ms"] = dict(zip(A.GLOBAL_REG_STAGES, r["stage_ms"]))
+        return r
+
+    def get_correspondences(self):
+        """(est feature indices, gt feature indices) of the last global_registration's correspondences, in est order"""
+        n = C.c_int64(0)
+        self._check(self._L.me_get_correspondences(self._ctx, None, None, 0, C.byref(n)))
+        ie, ig = np.empty(n.value, np.int32), np.empty(n.value, np.int32)
+        self._check(self._L.me_get_correspondences(self._ctx, ie.ctypes.data_as(C.c_void_p), ig.ctypes.data_as(C.c_void_p),
+                                                   n.value, C.byref(n)))
+        return ie, ig
+
+    def get_features(self, which):
+        """(xyz (N, 3), oriented normals (N, 3), FPFH (N, 33) float32) of the feature cloud the last global_registration
+        built from cloud `which`, in the order of the down-sampled cloud"""
+        n = C.c_int64(0)
+        self._check(self._L.me_get_features(self._ctx, int(which), None, None, None, 0, C.byref(n)))
+        xyz, nrm = np.empty((n.value, 3), np.float64), np.empty((n.value, 3), np.float64)
+        f = np.empty((n.value, A.FPFH_DIM), np.float32)
+        dp = C.POINTER(C.c_double)
+        self._check(self._L.me_get_features(self._ctx, int(which), xyz.ctypes.data_as(dp), nrm.ctypes.data_as(dp),
+                                            f.ctypes.data_as(C.POINTER(C.c_float)), n.value, C.byref(n)))
+        return xyz, nrm, f
+
     def build_grid(self, which):
         self._check(self._L.me_build_grid(self._ctx, which))
 

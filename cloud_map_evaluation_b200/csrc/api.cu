@@ -232,8 +232,9 @@ void me_destroy(me_ctx *ctx) {
   icp_close(ctx, false);
   if (ctx->copy_stream) { cudaStreamSynchronize(ctx->copy_stream); cudaStreamDestroy(ctx->copy_stream); }
   if (ctx->compute_mark) cudaEventDestroy(ctx->compute_mark);
-  free_cloud(ctx->cloud[0]);
-  free_cloud(ctx->cloud[1]);
+  for (Cloud &c : ctx->cloud) free_cloud(c);
+  for (float *f : ctx->d_fpfh) if (f) cudaFree(f);
+  if (ctx->d_corr) cudaFree(ctx->d_corr);
   stage_pool_free(ctx);
   if (ctx->d_scratch) cudaFree(ctx->d_scratch);
   if (ctx->d_block) cudaFree(ctx->d_block);
@@ -508,6 +509,23 @@ int me_icp_update(int32_t method, const double *block, const double center[3], d
   if (method == ME_ICP_POINT_TO_POINT && !center) return ME_ERR_INVALID;
   icp_update_host(method, block, center, update);
   return ME_OK;
+}
+
+int me_global_registration(me_ctx *ctx, const me_global_reg_params *p, me_global_reg_result *out) {
+  ME_ENTER(ctx);
+  if (!p || !out) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return global_registration(ctx, p, out);
+}
+
+int me_get_features(me_ctx *ctx, int which, double *xyz, double *normals, float *fpfh33, int64_t capacity, int64_t *n) {
+  ME_ENTER(ctx);
+  if (!cloud_id(which)) return fail(ctx, ME_ERR_INVALID, "bad cloud id");
+  return get_features(ctx, which, xyz, normals, fpfh33, capacity, n);
+}
+
+int me_get_correspondences(me_ctx *ctx, int32_t *est_idx, int32_t *gt_idx, int64_t capacity, int64_t *n) {
+  ME_ENTER(ctx);
+  return get_correspondences(ctx, est_idx, gt_idx, capacity, n);
 }
 
 int me_set_normals(me_ctx *ctx, int which, const double *normals_host, int64_t n) {

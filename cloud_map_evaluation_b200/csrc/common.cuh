@@ -19,6 +19,7 @@ __host__ __device__ __forceinline__ int orig_of(long long tag) { return (int)(ta
 __host__ __device__ __forceinline__ unsigned int cell_of(long long tag) { return (unsigned int)((unsigned long long)tag >> 32); }
 
 static constexpr int kTileEdge = 4;   // query tiles are kTileEdge^3 cells
+static constexpr int kFeatureSlot = 2;   // me_ctx::cloud[kFeatureSlot + which]: feature cloud of global registration
 
 // Dense lattice of a cloud.  Cells are cubes of edge h = v / m whose boundaries coincide with the voxel
 // boundaries floor(x / v) of the reference (voxel_calculator.cpp:241-245): every cell belongs to exactly one
@@ -188,7 +189,14 @@ struct me_ctx {
   int spec_m = 0;
   cudaStream_t copy_stream = nullptr;   // H2D uploads run here and overlap kernels that do not need them yet
   cudaEvent_t compute_mark = nullptr;
-  me::Cloud cloud[2];
+  // [ME_CLOUD_EST], [ME_CLOUD_GT]: the clouds of the public calls; [kFeatureSlot + which]: the private feature clouds of global
+  // registration (globalreg.cu), which no public `which` reaches
+  me::Cloud cloud[4];
+  float *d_fpfh[2] = {nullptr, nullptr};     // FPFH of the feature clouds, 33 per point
+  long long cap_fpfh[2] = {0, 0};
+  int32_t *d_corr = nullptr;                 // the last call's correspondences: est indices, then gt indices
+  long long cap_corr = 0, n_corr = 0;
+  bool features_valid = false;
   // small device scratch for reductions / accumulators
   void *d_scratch = nullptr;
   size_t scratch_bytes = 0;
@@ -256,8 +264,9 @@ inline void shard_range(const me_ctx *ctx, long long n, long long *b, long long 
 
 struct StageTimer {
   me_ctx *ctx; int stage;
-  StageTimer(me_ctx *c, int s) : ctx(c), stage(s) { cudaEventRecord(c->ev[2 * s], c->stream); }
-  ~StageTimer() { cudaEventRecord(ctx->ev[2 * stage + 1], ctx->stream); ctx->ev_used[stage] = true; }
+  // s < 0: not timed (the lattices of the feature clouds of global registration)
+  StageTimer(me_ctx *c, int s) : ctx(c), stage(s) { if (s >= 0) cudaEventRecord(c->ev[2 * s], c->stream); }
+  ~StageTimer() { if (stage >= 0) { cudaEventRecord(ctx->ev[2 * stage + 1], ctx->stream); ctx->ev_used[stage] = true; } }
 };
 
 // the queries a sweep evaluates: all of [q_begin, q_end), or in slab layout those whose cell lies in the owned planes
@@ -354,12 +363,16 @@ void invalidate_cloud(Cloud &c);      // the cloud's coordinates changed: bbox, 
 int run_awd_rows(me_ctx *ctx, const double *rows27, int64_t n_rows, double voxel_size, int scs_radius, double *w_out,
                  me_awd_result *out);
 // degraded copies of a cloud (perturb.cu)
-int copy_cloud(me_ctx *ctx, int src, int dst);
+int copy_cloud(me_ctx *ctx, int src, int dst, bool with_normals = true);
 int add_gaussian_noise(me_ctx *ctx, int which, double std_dev, uint64_t seed);
 int add_non_uniform_density(me_ctx *ctx, int which, double sparse_ratio, double dense_ratio, double region_size, uint64_t seed,
                             int64_t *n_out);
 int add_sparse_outliers(me_ctx *ctx, int which, double outlier_ratio, double outlier_range, uint64_t seed, int64_t *n_out);
 int add_local_deformation(me_ctx *ctx, int which, double radius, double strength, const double center[3]);
+// coarse global registration (globalreg.cu)
+int global_registration(me_ctx *ctx, const me_global_reg_params *p, me_global_reg_result *out);
+int get_features(me_ctx *ctx, int which, double *xyz, double *normals, float *fpfh33, int64_t capacity, int64_t *n);
+int get_correspondences(me_ctx *ctx, int32_t *est_idx, int32_t *gt_idx, int64_t capacity, int64_t *n);
 
 // ------------------------------------------------------------------------------------------------
 // device helpers

@@ -863,13 +863,13 @@ static void slab_planes(const me_ctx *ctx, const Lattice &L, Cloud &c) {
 // the other cloud; the next ordinary build_grid() replaces it.
 int build_grid(me_ctx *ctx, int which, double solo_h) {
   Cloud &c = ctx->cloud[which];
-  Cloud &o = ctx->cloud[1 - which];
+  Cloud &o = ctx->cloud[which ^ 1];      // the partner cloud: est <-> gt (feature clouds are only ever laid out solo)
   if (c.n <= 0) return fail(ctx, ME_ERR_EMPTY, "cloud is empty");
   if (c.n >= 0x7fffffffll) return fail(ctx, ME_ERR_RANGE, "more than 2^31-1 points per cloud (the reference indexes with int)");
   const bool solo = solo_h > 0;
   if (c.grid_valid && c.grid_solo == solo && (!solo || c.solo_h == solo_h)) return ME_OK;
   ME_TRY(wait_upload(ctx, which));
-  StageTimer timer(ctx, which == ME_CLOUD_EST ? 0 : 1);
+  StageTimer timer(ctx, which >= kFeatureSlot ? -1 : (which == ME_CLOUD_EST ? 0 : 1));
   ME_TRY(compute_bbox(ctx, which));
   const long long budget = grid_budget(ctx);
   const double v_req = ctx->voxel_hint;

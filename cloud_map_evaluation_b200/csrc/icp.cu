@@ -35,6 +35,8 @@
 // estimates [r s, (r + 1) s), s = ceil(N / world), visiting those points in cell-sorted order through a compacted list,
 // and the caller all-gathers the slices in place.
 #include "common.cuh"
+#include "knn_walk.cuh"
+#include "svd3.cuh"
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -92,78 +94,6 @@ icp_accum_kernel(const P4 *__restrict__ Q, long long qb, long long qe, const int
     unsigned long long s = 0;
     for (int w = 0; w < kThreads / 32; ++w) s += shc[w];
     if (s) atomicAdd(acc, (double)s);                      // block counts < 2^53: the fp64 sum is exact
-  }
-}
-
-// ---- host 3x3 algebra -------------------------------------------------------------------------------------------
-// SVD of a 3x3 by one-sided Jacobi (Hestenes): plane rotations V orthogonalise the columns of a = sigma V, so
-// sigma = U diag(w) V^T with U's columns a_j / w_j.  It works on sigma itself: the eigen-problem of sigma^T sigma would
-// square the condition number, and with it the error of the small singular values (a tilted near-planar cloud made R
-// a shear of a few per cent).  Singular values descending; only U's first two columns are formed.
-static void svd3_host(const double s_in[9], double U[9], double w[3], double V[9]) {
-  double a[9];
-  for (int i = 0; i < 9; ++i) { a[i] = s_in[i]; V[i] = (i % 4 == 0) ? 1.0 : 0.0; }
-  for (int sweep = 0; sweep < 60; ++sweep) {
-    double off = 0.0;
-    for (int p = 0; p < 2; ++p)
-      for (int q = p + 1; q < 3; ++q) {
-        double alpha = 0, beta = 0, gamma = 0;
-        for (int k = 0; k < 3; ++k) { alpha += a[k * 3 + p] * a[k * 3 + p]; beta += a[k * 3 + q] * a[k * 3 + q]; gamma += a[k * 3 + p] * a[k * 3 + q]; }
-        if (gamma == 0.0) continue;
-        off = std::max(off, std::fabs(gamma) / std::sqrt(alpha * beta));
-        const double zeta = (beta - alpha) / (2.0 * gamma);
-        const double t = (zeta >= 0 ? 1.0 : -1.0) / (std::fabs(zeta) + std::sqrt(1.0 + zeta * zeta));
-        const double c = 1.0 / std::sqrt(1.0 + t * t), s = c * t;
-        for (int k = 0; k < 3; ++k) {
-          const double ap = a[k * 3 + p], aq = a[k * 3 + q];
-          a[k * 3 + p] = c * ap - s * aq; a[k * 3 + q] = s * ap + c * aq;
-          const double vp = V[k * 3 + p], vq = V[k * 3 + q];
-          V[k * 3 + p] = c * vp - s * vq; V[k * 3 + q] = s * vp + c * vq;
-        }
-      }
-    if (off < 1e-15) break;
-  }
-  double nw[3];
-  for (int j = 0; j < 3; ++j) nw[j] = std::sqrt(a[j] * a[j] + a[3 + j] * a[3 + j] + a[6 + j] * a[6 + j]);
-  int ord[3] = {0, 1, 2};
-  std::sort(ord, ord + 3, [&](int x, int y) { return nw[x] > nw[y]; });
-  double Vs[9];
-  for (int j = 0; j < 3; ++j) {
-    w[j] = nw[ord[j]];
-    for (int k = 0; k < 3; ++k) { Vs[k * 3 + j] = V[k * 3 + ord[j]]; U[k * 3 + j] = j < 2 && w[j] > 0 ? a[k * 3 + ord[j]] / w[j] : 0.0; }
-  }
-  std::memcpy(V, Vs, sizeof(Vs));
-}
-static double det3_host(const double *m) {
-  return m[0] * (m[4] * m[8] - m[5] * m[7]) - m[1] * (m[3] * m[8] - m[5] * m[6]) + m[2] * (m[3] * m[7] - m[4] * m[6]);
-}
-
-// Eigen::umeyama without scaling from the reduced sums (icp_accum_kernel's block): R = U S V^T of
-// sigma = (1/n) sum (q - qm)(p - pm)^T
-static void umeyama_from_sums(const double *blk, const double c[3], double upd[16]) {
-  const double n = blk[0];
-  const double *sp = blk + 1, *sq = blk + 4, *sqp = blk + 7;
-  double pm[3], qm[3], sigma[9];
-  for (int k = 0; k < 3; ++k) { pm[k] = sp[k] / n; qm[k] = sq[k] / n; }
-  for (int r = 0; r < 3; ++r)
-    for (int col = 0; col < 3; ++col) sigma[r * 3 + col] = sqp[r * 3 + col] / n - qm[r] * pm[col];
-  double U[9], sv[3], Vs[9];
-  svd3_host(sigma, U, sv, Vs);
-  // U's third column is always the cross product of the first two: a_3 / w_3 carries an error of u w_1 / w_3 (and is
-  // undefined at rank 2), while R = U S V^T only needs the orientation of U, which the cross product fixes (det U = +1).
-  // Eigen's rule S_3 = -1 when det(U) det(V) < 0 then makes R a rotation; in exact arithmetic this is umeyama's R.
-  U[2] = U[3] * U[7] - U[6] * U[4]; U[5] = U[6] * U[1] - U[0] * U[7]; U[8] = U[0] * U[4] - U[3] * U[1];
-  double S[3] = {1, 1, 1};
-  if (det3_host(U) * det3_host(Vs) < 0) S[2] = -1;
-  std::memset(upd, 0, 16 * sizeof(double));
-  upd[15] = 1.0;
-  for (int r = 0; r < 3; ++r)
-    for (int col = 0; col < 3; ++col) { double s = 0; for (int k = 0; k < 3; ++k) s += U[r * 3 + k] * S[k] * Vs[col * 3 + k]; upd[r * 4 + col] = s; }
-  // t = dst_mean - R src_mean, means back in absolute coordinates
-  for (int r = 0; r < 3; ++r) {
-    double rp = 0;
-    for (int k = 0; k < 3; ++k) rp += upd[r * 4 + k] * (pm[k] + c[k]);
-    upd[r * 4 + 3] = (qm[r] + c[r]) - rp;
   }
 }
 
@@ -269,8 +199,8 @@ __device__ void fast_eigen3x3_normal(const double cov[9], double nrm[3]) {
 // ---------------------------------------------------------------------------------------------------------------
 // PointCloud::EstimateNormals(KDTreeSearchParamKNN(k)) [ext]: per point the k nearest neighbours (the point itself
 // included), their covariance, the eigenvector of its smallest eigenvalue.  One thread per point; the k best (d2,
-// position) pairs sit sorted in shared memory ([slot][thread]); the lattice is searched shell by shell (Chebyshev rings)
-// until the k-th distance beats the distance to the border of the searched block.  Ties go to the smaller caller index.
+// position) pairs sit sorted in shared memory ([slot][thread]), found by knn_walk (knn_walk.cuh).  Ties go to the
+// smaller caller index.
 // The queries are the n points of the cell-sorted cloud, or (list != nullptr) the sorted positions list[0 .. n): the
 // neighbours, and with them the arithmetic of every normal, do not depend on which points are queried together.
 // ---------------------------------------------------------------------------------------------------------------
@@ -284,102 +214,7 @@ knn_normals_kernel(const P4 *__restrict__ S, long long n, const uint32_t *__rest
   uint32_t *ik = reinterpret_cast<uint32_t *>(knn_smem + (size_t)k * kKnnThreads * sizeof(double)) + threadIdx.x;
   for (long long i = blockIdx.x * (long long)kKnnThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kKnnThreads) {
     const P4 q = load_p4(S + (list ? (long long)__ldg(list + i) : i));
-    int cix, ciy, ciz;
-    long long xs = I.sparse ? cell_coord(q.x, L, 0) : 0;
-    xs = xs < 0 ? 0 : (xs >= L.dims[0] ? L.dims[0] - 1 : xs);
-    cell_from_tag(I, q.idx, (int)xs, cix, ciy, ciz);
-    const long long ix = cix, iy = ciy, iz = ciz;
-    int cnt = 0;
-    double kth = INFINITY;
-    // one candidate: keep the k best (d2, position) pairs sorted; ties go to the smaller caller index
-    auto offer = [&](uint32_t j) {
-      const P4 p = load_p4(S + j);
-      const double d2 = d2_kd(q.x, q.y, q.z, p.x, p.y, p.z);
-      if (cnt == k) {
-        if (d2 > kth) return;
-        if (d2 == kth && orig_of(p.idx) > orig_of(__double_as_longlong(__ldg(reinterpret_cast<const double *>(S + ik[(k - 1) * kKnnThreads]) + 3)))) return;
-      }
-      int pos = cnt < k ? cnt++ : k - 1;
-      while (pos > 0) {
-        const double dp = dk[(pos - 1) * kKnnThreads];
-        if (dp < d2) break;
-        if (dp == d2 && orig_of(__double_as_longlong(__ldg(reinterpret_cast<const double *>(S + ik[(pos - 1) * kKnnThreads]) + 3))) < orig_of(p.idx)) break;
-        dk[pos * kKnnThreads] = dp; ik[pos * kKnnThreads] = ik[(pos - 1) * kKnnThreads];
-        --pos;
-      }
-      dk[pos * kKnnThreads] = d2; ik[pos * kKnnThreads] = j;
-      if (cnt == k) kth = dk[(k - 1) * kKnnThreads];
-    };
-    bool resolved = false;
-    const int fine_rings = CG.cnt ? 8 : 0x7fffffff;      // isolated points: blocks of f^3 cells take over (empty space is skipped)
-    for (int r = 0; r <= fine_rings; ++r) {
-      for (int dz = -r; dz <= r; ++dz) {
-        const long long z = iz + dz;
-        if (z < 0 || z >= L.dims[2]) continue;
-        for (int dy = -r; dy <= r; ++dy) {
-          const long long y = iy + dy;
-          if (y < 0 || y >= L.dims[1]) continue;
-          const bool border = (dz == -r || dz == r || dy == -r || dy == r);
-          for (int part = 0; part < 2; ++part) {
-            long long xa, xb;
-            if (border) { if (part) break; xa = ix - r; xb = ix + r; }
-            else { xa = xb = part ? ix + r : ix - r; }
-            xa = max(xa, 0ll); xb = min(xb, (long long)L.dims[0] - 1);
-            if (xa > xb) continue;
-            uint32_t s, e;
-            cell_range(I, (int)z, (int)y, (int)xa, (int)xb, s, e);
-            for (uint32_t j = s; j < e; ++j) offer(j);
-          }
-        }
-      }
-      // everything closer than the border of the searched block [i - r, i + r]^3 has been seen
-      const double g = (double)r * L.h - slack;
-      if (cnt == k && g > 0 && kth < g * g) { resolved = true; break; }
-      if (ix - r <= 0 && ix + r >= L.dims[0] - 1 && iy - r <= 0 && iy + r >= L.dims[1] - 1 && iz - r <= 0 && iz + r >= L.dims[2] - 1) { resolved = true; break; }
-    }
-    if (!resolved) {
-      // coarse phase, from scratch (the blocks cover the cells of the fine phase again): Chebyshev rings of blocks, empty
-      // blocks cost one count load, blocks that cannot hold a point closer than the k-th best are skipped
-      const int f = CG.f;
-      const long long cqx = ix / f, cqy = iy / f, cqz = iz / f;
-      const double ux = cell_coord_cont(q.x, L, 0), uy = cell_coord_cont(q.y, L, 1), uz = cell_coord_cont(q.z, L, 2);
-      cnt = 0; kth = INFINITY;
-      for (int rc = 0;; ++rc) {
-        for (int dz = -rc; dz <= rc; ++dz) {
-          const long long bz = cqz + dz;
-          if (bz < 0 || bz >= CG.cd[2]) continue;
-          for (int dy = -rc; dy <= rc; ++dy) {
-            const long long by = cqy + dy;
-            if (by < 0 || by >= CG.cd[1]) continue;
-            const bool border = (dz == -rc || dz == rc || dy == -rc || dy == rc);
-            for (int dx = -rc; dx <= rc; dx += (border || rc == 0) ? 1 : 2 * rc) {
-              const long long bx = cqx + dx;
-              if (bx < 0 || bx >= CG.cd[0]) continue;
-              if (__ldg(CG.cnt + (bz * CG.cd[1] + by) * (long long)CG.cd[0] + bx) == 0) continue;
-              if (cnt == k) {
-                const double ex = fmax(0.0, fmax((double)(bx * f) - ux, ux - (double)((bx + 1) * f)));
-                const double ey = fmax(0.0, fmax((double)(by * f) - uy, uy - (double)((by + 1) * f)));
-                const double ez = fmax(0.0, fmax((double)(bz * f) - uz, uz - (double)((bz + 1) * f)));
-                const double lb = sqrt(ex * ex + ey * ey + ez * ez) * L.h - slack;
-                if (lb > 0 && lb * lb > kth) continue;
-              }
-              const int xa = (int)(bx * f), xb = (int)min(bx * f + f - 1, (long long)L.dims[0] - 1);
-              for (int row = 0; row < f * f; ++row) {
-                const long long z = bz * f + row / f, y = by * f + row % f;
-                if (z >= L.dims[2] || y >= L.dims[1]) continue;
-                uint32_t s, e;
-                cell_range(I, (int)z, (int)y, xa, xb, s, e);
-                for (uint32_t j = s; j < e; ++j) offer(j);
-              }
-            }
-          }
-        }
-        // the point lies inside its own block: everything closer than rc blocks has been seen
-        const double g = (double)rc * (double)f * L.h - slack;
-        if (cnt == k && g > 0 && kth < g * g) break;
-        if (cqx - rc <= 0 && cqx + rc >= CG.cd[0] - 1 && cqy - rc <= 0 && cqy + rc >= CG.cd[1] - 1 && cqz - rc <= 0 && cqz + rc >= CG.cd[2] - 1) break;
-      }
-    }
+    const int cnt = knn_walk<kKnnThreads>(S, I, L, CG, q, k, slack, INFINITY, false, dk, ik);
     // utility::ComputeCovariance over the neighbours (cumulants about the query point instead of the origin: same
     // covariance, without the cancellation of raw coordinates); fewer than 3 neighbours -> identity
     double cov[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};

@@ -4,11 +4,13 @@
 // The reference draws from std::random_device, so no run of it can be repeated.  Here every draw is the counter-based hash
 // of synth.py — splitmix64 of (seed, index, lane) — so a degraded map is a pure function of (cloud, parameters, seed): the
 // same on every GPU of a job without communication, and its integer structure (kept points, outlier bases) equal bit for bit
-// to the numpy statement in tests/perturb_ref.py.  Lanes (disjoint, so one seed serves all four operators):
+// to the numpy statement in tests/perturb_ref.py.  Lanes (disjoint, so one seed serves all four operators and the RANSAC
+// draws of global registration; the helpers live in rng.cuh):
 //   noise          gaussian(seed, i, 2a), a = x, y, z        lanes 0-5
 //   density        uniform24(seed, i, 6)                     lane 6
 //   outliers       uniform53(seed, j, 7) for the base,       lane 7
 //                  gaussian(seed, j, 8 + 2a) for the offset  lanes 8-13
+//   (globalreg.cu) uniform53(seed, h, 16 + t), t = 0, 1, 2   lanes 16-18: the three correspondences of hypothesis h
 // uniform24 = (h >> 40) * 2^-24 in fp32 (synth.uniform24), uniform53 = (h >> 11) * 2^-53, gaussian = Box-Muller in fp64 with
 // u1 = max(u24, 2^-25) (synth.gaussian).  The final multiply-adds are rounded separately (__dmul_rn / __dadd_rn), as numpy
 // and the reference round them; only the device's log / cos / sin differ from the host's libm, by an ulp or two.
@@ -16,6 +18,7 @@
 // After every operator the cloud's lattice, plan and per-point results are stale (invalidate_cloud), as after me_transform.
 // Borrowed clouds (me_set_cloud_device) are refused: the operators never write caller memory.
 #include "common.cuh"
+#include "rng.cuh"
 #include <algorithm>
 #include <cmath>
 
@@ -25,15 +28,6 @@ static constexpr int kThreads = 256;
 static constexpr double kPi = 3.141592653589793;          // M_PI
 static constexpr double kTwoPi = 6.283185307179586;       // 2.0 * np.pi, rounded once as numpy forms it
 
-__host__ __device__ __forceinline__ unsigned long long mix64(unsigned long long z) {     // synth._mix
-  z += 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-// the per-lane key synth.uniform24 derives from the seed (computed once on the host)
-static unsigned long long lane_key(uint64_t seed, int lane) { return mix64(seed + (unsigned long long)lane * 0xD1B54A32D192ED03ull); }
-
 struct LaneKeys { unsigned long long k[14]; };
 static LaneKeys lane_keys(uint64_t seed) {
   LaneKeys L;
@@ -41,15 +35,6 @@ static LaneKeys lane_keys(uint64_t seed) {
   return L;
 }
 
-__device__ __forceinline__ unsigned long long draw(unsigned long long key, long long idx, int lane) {
-  return mix64(key ^ ((unsigned long long)idx * 0x2545F4914F6CDD1Dull + (unsigned long long)lane));
-}
-__device__ __forceinline__ double uniform24(unsigned long long key, long long idx, int lane) {
-  return (double)((float)(draw(key, idx, lane) >> 40) * (1.0f / 16777216.0f));
-}
-__device__ __forceinline__ double uniform53(unsigned long long key, long long idx, int lane) {
-  return (double)(draw(key, idx, lane) >> 11) * 0x1p-53;
-}
 // synth.gaussian: sqrt(-2 log u1) * cos(2 pi u2) from lanes (lane, lane + 1)
 __device__ __forceinline__ double gaussian(const LaneKeys &L, long long idx, int lane) {
   const double u1 = fmax(uniform24(L.k[lane], idx, lane), 0x1p-25);
@@ -142,7 +127,7 @@ static int owned_cloud(me_ctx *ctx, int which, const char *what) {
   return wait_upload(ctx, which);
 }
 
-int copy_cloud(me_ctx *ctx, int src, int dst) {
+int copy_cloud(me_ctx *ctx, int src, int dst, bool with_normals) {
   Cloud &s = ctx->cloud[src], &d = ctx->cloud[dst];
   ME_TRY(wait_upload(ctx, src));
   ME_TRY(wait_upload(ctx, dst));
@@ -153,7 +138,7 @@ int copy_cloud(me_ctx *ctx, int src, int dst) {
   d.n = s.n;
   invalidate_cloud(d);
   d.normal_valid = false;
-  if (s.normal_valid && s.n > 0) {
+  if (with_normals && s.normal_valid && s.n > 0) {
     ME_TRY(ensure(ctx, (void **)&d.d_normal, &d.cap_normal, 3 * s.n, sizeof(double)));
     ME_CUDA(ctx, cudaMemcpyAsync(d.d_normal, s.d_normal, (size_t)s.n * 3 * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
     d.normal_valid = true;

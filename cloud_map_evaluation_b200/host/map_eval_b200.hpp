@@ -81,6 +81,12 @@ struct Param {   // map_eval.h:60-116
   double outlier_ratio_ = 0.0, outlier_range_ = 1.0;   // applied when outlier_ratio > 0
   double deform_radius_ = 0.0, deform_strength_ = 0.0; // applied when deform_radius > 0
   double deform_center_[3] = {0, 0, 0};
+  // global_registration: the initial pose from the maps themselves (me_global_registration, FPFH + RANSAC on the GPU); its T
+  // replaces initial_matrix on both paths
+  bool global_registration_ = false;
+  double global_registration_voxel_size_ = 0.5;
+  uint64_t global_registration_seed_ = 0;
+  int64_t global_registration_hypotheses_ = 100000;
 };
 
 // map_eval_main.cpp:120-208
@@ -132,6 +138,12 @@ inline Param loadParametersFromYAML(const std::string &yaml_file_path) {
     if (config["outlier_range"]) param.outlier_range_ = config["outlier_range"].as<double>();
     if (config["deform_radius"]) param.deform_radius_ = config["deform_radius"].as<double>();
     if (config["deform_strength"]) param.deform_strength_ = config["deform_strength"].as<double>();
+    if (config["global_registration"]) param.global_registration_ = config["global_registration"].as<bool>();
+    if (config["global_registration_voxel_size"])
+      param.global_registration_voxel_size_ = config["global_registration_voxel_size"].as<double>();
+    if (config["global_registration_seed"]) param.global_registration_seed_ = config["global_registration_seed"].as<uint64_t>();
+    if (config["global_registration_hypotheses"])
+      param.global_registration_hypotheses_ = (int64_t)config["global_registration_hypotheses"].as<uint64_t>();
     if (config["deform_center"] && config["deform_center"].size() >= 3)
       for (int a = 0; a < 3; ++a) param.deform_center_[a] = config["deform_center"][a].as<double>();
     return param;
@@ -157,7 +169,10 @@ inline void dumpParam(const Param &p, std::ostream &os) {
      << "\ndensity_sparse_ratio=" << p.density_sparse_ratio_ << "\ndensity_dense_ratio=" << p.density_dense_ratio_
      << "\ndensity_region_size=" << p.density_region_size_ << "\ndensity_set=" << p.density_set_ << "\noutlier_ratio=" << p.outlier_ratio_
      << "\noutlier_range=" << p.outlier_range_ << "\ndeform_radius=" << p.deform_radius_ << "\ndeform_strength=" << p.deform_strength_
-     << "\ndeform_center=" << p.deform_center_[0] << "," << p.deform_center_[1] << "," << p.deform_center_[2] << "\n";
+     << "\ndeform_center=" << p.deform_center_[0] << "," << p.deform_center_[1] << "," << p.deform_center_[2]
+     << "\nglobal_registration=" << p.global_registration_ << "\nglobal_registration_voxel_size=" << p.global_registration_voxel_size_
+     << "\nglobal_registration_seed=" << p.global_registration_seed_
+     << "\nglobal_registration_hypotheses=" << p.global_registration_hypotheses_ << "\n";
 }
 
 // Eigen's default IOFormat for `vec.transpose()`: coefficients right-aligned to a common width, one space apart
@@ -274,7 +289,8 @@ class MapEvalB200 {
     return -1;
   }
   render::ColoredCloud map_3d_entropy_, gt_3d_entropy_, map_3d_render_raw_, map_3d_render_inlier_;   // map_eval.h:341-347
-  int simulateEstimate(me_ctx *c, int64_t *n);     // evaluate_noised_gt: estimate := degraded copy of the ground truth
+  int simulateEstimate(me_ctx *c, int64_t *n);
+  int globalRegistration();                        // global_registration: T from the maps replaces initial_matrix     // evaluate_noised_gt: estimate := degraded copy of the ground truth
   std::string simulationSummary() const;
   int renderEntropy(int which, int64_t n, render::ColoredCloud *out);
   int renderDistances(bool cutoff_strict);
@@ -361,6 +377,8 @@ inline int MapEvalB200::process() {
   if (param_.enable_debug)
     std::cout << "INFO: Loaded point clouds: " << n_est << " points (Map), " << n_gt << " points (Ground Truth)."
               << std::endl;
+
+  if (param_.global_registration_ && globalRegistration() != 0) return -1;
 
   if (param_.evaluate_mme_) {
     if (param_.enable_debug) std::cout << "INFO: Starting MME calculation..." << std::endl;
@@ -566,6 +584,39 @@ inline int MapEvalB200::calculateMetricsWithInitialMatrix() {
   std::cout << "INFO: est-gt MME: " << mme_est << " " << mme_gt << std::endl;
   std::cout << "INFO: IoU: " << eigenRow(nn_.iou, 5, 6) << std::endl;
   std::cout << "INFO: Full Chamfer distance (not computed by the reference on this path): " << nn_.full_cd << std::endl;
+  return 0;
+}
+
+// global_registration: FPFH + RANSAC on context 0 (me_global_registration) on the loaded, down-sampled clouds.  The result
+// is a pure function of the clouds, the parameters and the seed, so every context of a multi-GPU run uses context 0's T
+// without a collective.  It replaces initial_matrix: path A's transform, path B's T_init.
+inline int MapEvalB200::globalRegistration() {
+  static const double eye[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  if (!std::equal(param_.initial_matrix_, param_.initial_matrix_ + 16, eye))
+    std::cout << "INFO: global_registration is on: its result replaces the initial_matrix of the configuration, which is not "
+                 "the identity" << std::endl;
+  const double v = param_.global_registration_voxel_size_;
+  me_global_reg_params gp{};
+  gp.voxel_size = v;
+  gp.normal_knn = 30;
+  gp.feature_radius = 10.0 * v;
+  gp.feature_max_nn = 128;
+  gp.mutual_filter = 1;
+  gp.max_correspondence_distance = 1.5 * v;
+  gp.edge_ratio = 0.9;
+  gp.n_hypotheses = param_.global_registration_hypotheses_;
+  gp.seed = param_.global_registration_seed_;
+  me_global_reg_result gr{};
+  TicToc tic;
+  if (me_global_registration(ctx_, &gp, &gr) != ME_OK) return fail("me_global_registration");
+  std::copy(gr.T, gr.T + 16, param_.initial_matrix_);
+  const double fitness = gr.n_correspondences > 0 ? (double)gr.n_inliers / (double)gr.n_correspondences : 0.0;
+  std::cout << "INFO: global registration (" << tic.toc() / 1000.0 << " s): " << gr.n_est_features << " / " << gr.n_gt_features
+            << " feature points, " << gr.n_correspondences << " correspondences, " << gr.n_inliers << " inliers, rmse "
+            << gr.inlier_rmse << "\n" << eigenMatrix4(gr.T, 6) << std::endl;
+  file_result << std::fixed << std::setprecision(5) << "Global registration cloud: " << eigenMatrix4(gr.T, 5) << std::endl;
+  file_result << std::fixed << std::setprecision(5) << "Global registration: " << fitness << " " << gr.n_inliers << " "
+              << gr.n_correspondences << std::endl;
   return 0;
 }
 

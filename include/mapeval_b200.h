@@ -331,6 +331,53 @@ ME_API int  me_get_normals(me_ctx *ctx, int which, double *normals_host);
 /* builds (or rebuilds) the cell-sorted grid of one cloud; the eval calls build lazily if needed */
 ME_API int  me_build_grid(me_ctx *ctx, int which);
 
+/* ---- coarse global registration: the initial pose est -> gt without a hand-made initial_matrix ---------------------------
+ * FPFH descriptors, mutual nearest-neighbour matching in descriptor space and RANSAC over the correspondences, all on the
+ * device (Open3D's registration_ransac_based_on_feature_matching in spirit; the reference never calls it, its users align the
+ * maps by hand).  The call works on two private feature clouds: the context's est and gt clouds, their normals, lattices and
+ * per-point results are left as they were.  Pipeline:
+ *   1. feature clouds: each cloud copied and down-sampled at voxel_size (me_voxel_downsample), exact k-NN normals
+ *      (normal_knn, me_estimate_normals) oriented towards centroid + (0, 0, 10 * bbox diagonal) of that feature cloud;
+ *   2. FPFH (33 fp32 per point): neighbourhood = the <= feature_max_nn nearest other points with d^2 < feature_radius^2
+ *      (ties to the smaller index); pair features, 11 bins per group, SPFH + the neighbours' SPFH weighted by 1 / d^2;
+ *   3. exact fp32 nearest neighbour in descriptor space (fixed dimension order, no contraction, ties to the smaller index)
+ *      est -> gt and gt -> est; mutual_filter != 0 keeps the pairs that are each other's nearest;
+ *   4. n_hypotheses RANSAC hypotheses h: three correspondences min(floor(uniform53(seed, h, 16 + t) * n), n - 1),
+ *      rejected when two coincide, an edge fails min^2 >= edge_ratio^2 max^2 or the three are (nearly) collinear (the
+ *      second singular value of their cross-covariance <= 1e-6 times the first), otherwise the rigid fit of the three and
+ *      the count of correspondences with |R p + t - q|^2 < max_correspondence_distance^2.  The most inliers win, ties to
+ *      the smallest h; every hypothesis is evaluated, so T is a pure function of (clouds, params, seed);
+ *   5. refinement: the rigid fit over the winner's inliers; n_inliers and inlier_rmse under it.
+ * Errors: ME_ERR_EMPTY for an empty cloud, ME_ERR_INVALID for bad parameters, fewer than 3 correspondences or no valid
+ * hypothesis (the message says which). */
+typedef struct {
+  double  voxel_size;                  /* feature cloud: me_voxel_downsample at this size                              */
+  int32_t normal_knn;                  /* 30                                                                            */
+  double  feature_radius;              /* 10 * voxel_size (5 * voxel_size does not separate smooth terrain)            */
+  int32_t feature_max_nn;              /* 128 (the largest): at most this many neighbours within the radius            */
+  int32_t mutual_filter;               /* 1                                                                             */
+  double  max_correspondence_distance; /* 1.5 * voxel_size: inlier test                                                 */
+  double  edge_ratio;                  /* 0.9                                                                           */
+  int64_t n_hypotheses;                /* 100000 (< 2^32)                                                               */
+  uint64_t seed;
+} me_global_reg_params;
+typedef struct {
+  double  T[16];                       /* row-major, est -> gt, like me_icp's transformation                           */
+  int64_t n_est_features, n_gt_features, n_correspondences, n_valid_hypotheses;
+  int64_t best_hypothesis, n_inliers;  /* the winner; inliers of the correspondences under the refined T              */
+  double  inlier_rmse;                 /* sqrt(mean |T p - q|^2) over them                                             */
+  double  stage_ms[6];                 /* CUDA-event times: copy + down-sample, normals, FPFH (both clouds), matching,
+                                          RANSAC, refinement                                                           */
+} me_global_reg_result;
+ME_API int me_global_registration(me_ctx *ctx, const me_global_reg_params *p, me_global_reg_result *out);
+/* the feature cloud of the last me_global_registration (which = ME_CLOUD_EST / ME_CLOUD_GT): points, oriented normals and
+ * FPFH descriptors (33 fp32 per point), in the order of the down-sampled cloud.  Any of the three arrays may be NULL;
+ * xyz == normals == fpfh33 == NULL: size query (*n).  capacity < n is an error. */
+ME_API int me_get_features(me_ctx *ctx, int which, double *xyz, double *normals, float *fpfh33, int64_t capacity, int64_t *n);
+/* the correspondences of the last me_global_registration that reached matching: (est feature index, gt feature index) in
+ * est order.  est_idx == gt_idx == NULL: size query (*n).  capacity < n is an error. */
+ME_API int me_get_correspondences(me_ctx *ctx, int32_t *est_idx, int32_t *gt_idx, int64_t capacity, int64_t *n);
+
 /* replaces: MapEval::calculateMetricsWithInitialMatrix (map_eval.cpp:1204-1260), getDiffRegResultWithCorrespondence
  * (:1069-1145), the metric half of calculateMetrics (:1147-1202) and computeChamferDistance (:1398-1431). */
 ME_API int  me_eval_nn_accum(me_ctx *ctx, const me_nn_params *p, me_nn_accum *est_to_gt, me_nn_accum *gt_to_est);
