@@ -117,6 +117,25 @@ class me_nn_result(C.Structure):
                 ("f1", C.c_double * 5), ("iou", C.c_double * 5), ("full_cd", C.c_double)]
 
 
+# accuracy curve (me_nn_curve*)
+ME_CURVE_MAX_LEVELS = 1024
+
+
+class me_curve_dir(C.Structure):
+    _fields_ = [("n_inlier", C.c_int64), ("mean", C.c_double), ("rmse", C.c_double), ("fitness", C.c_double),
+                ("sigma", C.c_double)]
+
+
+class me_curve_row(C.Structure):
+    _fields_ = [("tau", C.c_double), ("est_to_gt", me_curve_dir), ("gt_to_est", me_curve_dir), ("cd", C.c_double),
+                ("f1", C.c_double), ("iou", C.c_double)]
+
+
+def curve_block_len(n_tau):
+    """values of a curve block: per direction count, sum d and sum d^2 of the bins 0..K, then n_ub"""
+    return 2 * (3 * (int(n_tau) + 1) + 1)
+
+
 class me_mme_accum(C.Structure):
     _fields_ = [("n_query", C.c_int64), ("n_valid", C.c_int64), ("sum_entropy", C.c_double),
                 ("min_entropy", C.c_double), ("max_entropy", C.c_double)]

@@ -24,6 +24,7 @@ SYMBOLS = (
     "me_icp_begin", "me_icp_normals_slice", "me_icp_block", "me_icp_step", "me_icp_end", "me_icp_update",
     "me_copy_cloud", "me_add_gaussian_noise", "me_add_non_uniform_density", "me_add_sparse_outliers", "me_add_local_deformation",
     "me_global_registration", "me_get_features", "me_get_correspondences",
+    "me_nn_curve_accum_device", "me_nn_curve_finalize", "me_nn_curve",
 )
 
 _lib = None
@@ -111,6 +112,10 @@ def load():
     L.me_get_stage_times.argtypes = [ctx, dp]
     L.me_launch_count.argtypes = [ctx]
     L.me_launch_count.restype = C.c_int64
+    L.me_nn_curve_accum_device.argtypes = [ctx, dp, C.c_int32, C.POINTER(dp), C.POINTER(C.c_int32)]
+    L.me_nn_curve_finalize.argtypes = [C.POINTER(A.me_nn_params), C.POINTER(A.me_nn_accum), C.POINTER(A.me_nn_accum), dp, dp,
+                                       C.c_int32, C.c_int64, C.c_int64, C.POINTER(A.me_curve_row)]
+    L.me_nn_curve.argtypes = [ctx, dp, C.c_int32, C.POINTER(A.me_curve_row)]
     L.me_kernel_trace.argtypes = [ctx, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.c_int32]
     if L.me_abi_version() != A.ME_ABI_VERSION:
         raise RuntimeError("libmapeval_b200.so ABI version mismatch")

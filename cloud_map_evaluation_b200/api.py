@@ -35,6 +35,43 @@ def icp_update(method, block, center=None):
     return out.reshape(4, 4)
 
 
+_CURVE_DIR = np.dtype([("n_inlier", "<i8"), ("mean", "<f8"), ("rmse", "<f8"), ("fitness", "<f8"), ("sigma", "<f8")])
+# me_curve_row, field for field
+_CURVE_ROW = np.dtype([("tau", "<f8"), ("est_to_gt", _CURVE_DIR), ("gt_to_est", _CURVE_DIR), ("cd", "<f8"), ("f1", "<f8"),
+                       ("iou", "<f8")])
+assert _CURVE_ROW.itemsize == C.sizeof(A.me_curve_row)
+
+
+def _curve_levels(tau):
+    t = np.ascontiguousarray(tau, dtype=np.float64).reshape(-1)
+    return t, t.ctypes.data_as(C.POINTER(C.c_double))
+
+
+def _curve_arrays(rows):
+    """{'tau', 'cd', 'f1', 'iou': (K,) arrays, 'est_to_gt' / 'gt_to_est': {'n_inlier', 'mean', 'rmse', 'fitness', 'sigma'}}"""
+    out = {k: rows[k].copy() for k in ("tau", "cd", "f1", "iou")}
+    for d in ("est_to_gt", "gt_to_est"):
+        out[d] = {k: rows[d][k].copy() for k in _CURVE_DIR.names}
+    return out
+
+
+def curve_finalize(params, e, g, block, tau, n_est, n_gt):
+    """me_nn_curve_finalize (host only): the curve from a (reduced) curve block and the (reduced) accumulators of the
+    me_eval_nn* call whose records it was built from; numpy arrays per field as MapEvalB200.accuracy_curve"""
+    L = _lib.load()
+    t, tp = _curve_levels(tau)
+    b = np.ascontiguousarray(block, dtype=np.float64)
+    if b.size != A.curve_block_len(t.size):
+        raise ValueError(f"a curve block of {t.size} levels has {A.curve_block_len(t.size)} values")
+    rows = np.zeros(t.size, _CURVE_ROW)
+    rc = L.me_nn_curve_finalize(C.byref(params), C.byref(e) if e is not None else None, C.byref(g) if g is not None else None,
+                                b.ctypes.data_as(C.POINTER(C.c_double)), tp, t.size, int(n_est), int(n_gt),
+                                rows.ctypes.data_as(C.POINTER(A.me_curve_row)))
+    if rc != A.ME_OK:
+        raise MapEvalError(rc, "me_nn_curve_finalize: invalid levels, or a block and accumulators of different evaluations")
+    return _curve_arrays(rows)
+
+
 class MapEvalB200:
     """One context = one GPU.  rank/world select this context's contiguous query range (multi-GPU sharding)."""
 
@@ -284,6 +321,24 @@ class MapEvalB200:
         out = A.me_nn_result()
         self._check(self._L.me_eval_nn(self._ctx, C.byref(params), C.byref(out)))
         return out
+
+    def accuracy_curve(self, tau):
+        """AC / COM / CD / F1 / IoU at every level of tau (1..ME_CURVE_MAX_LEVELS thresholds, finite, >= 0, non-decreasing)
+        from the records of the last NN evaluation, without a new sweep (me_nn_curve, world 1).  Returns numpy arrays per
+        field: 'tau', 'cd', 'f1', 'iou' and per direction 'est_to_gt' / 'gt_to_est' a dict of 'n_inlier', 'mean', 'rmse',
+        'fitness', 'sigma'.  Multi-GPU: curve_accum_device + dist.allreduce_curve + curve_finalize."""
+        t, tp = _curve_levels(tau)
+        rows = np.zeros(t.size, _CURVE_ROW)
+        self._check(self._L.me_nn_curve(self._ctx, tp, t.size, rows.ctypes.data_as(C.POINTER(A.me_curve_row))))
+        return _curve_arrays(rows)
+
+    def curve_accum_device(self, tau):
+        """(device pointer, n) of this rank's SUM-reducible curve block at the levels tau (me_nn_curve_accum_device)"""
+        t, tp = _curve_levels(tau)
+        ptr = C.POINTER(C.c_double)()
+        n = C.c_int32(0)
+        self._check(self._L.me_nn_curve_accum_device(self._ctx, tp, t.size, C.byref(ptr), C.byref(n)))
+        return C.cast(ptr, C.c_void_p).value, n.value
 
     def get_nn(self, which_query):
         n = self.n[which_query]

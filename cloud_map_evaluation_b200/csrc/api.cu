@@ -348,6 +348,7 @@ int me_synchronize(me_ctx *ctx) {
 
 int me_set_cloud(me_ctx *ctx, int which, const double *xyz_host, int64_t n) {
   ME_ENTER(ctx);
+  ctx->cloud_gen++;      // stales the NN records (me_nn_curve*)
   if (which != ME_CLOUD_EST && which != ME_CLOUD_GT) return fail(ctx, ME_ERR_INVALID, "which must be ME_CLOUD_EST or ME_CLOUD_GT");
   if (n < 0 || (n > 0 && !xyz_host)) return fail(ctx, ME_ERR_INVALID, "bad cloud pointer/size");
   if (n >= 0x7fffffffll) return fail(ctx, ME_ERR_RANGE, "more than 2^31-1 points per cloud (the reference indexes with int)");
@@ -380,6 +381,7 @@ int me_set_cloud(me_ctx *ctx, int which, const double *xyz_host, int64_t n) {
 
 int me_set_cloud_device(me_ctx *ctx, int which, const double *xyz_device, int64_t n) {
   ME_ENTER(ctx);
+  ctx->cloud_gen++;      // stales the NN records (me_nn_curve*)
   if (which != ME_CLOUD_EST && which != ME_CLOUD_GT) return fail(ctx, ME_ERR_INVALID, "which must be ME_CLOUD_EST or ME_CLOUD_GT");
   if (n < 0 || (n > 0 && !xyz_device)) return fail(ctx, ME_ERR_INVALID, "bad cloud pointer/size");
   if (n >= 0x7fffffffll) return fail(ctx, ME_ERR_RANGE, "more than 2^31-1 points per cloud");
@@ -396,12 +398,14 @@ int me_set_cloud_device(me_ctx *ctx, int which, const double *xyz_device, int64_
 
 int me_transform(me_ctx *ctx, int which, const double T[16]) {
   ME_ENTER(ctx);
+  ctx->cloud_gen++;      // stales the NN records (me_nn_curve*)
   if ((which != ME_CLOUD_EST && which != ME_CLOUD_GT) || !T) return fail(ctx, ME_ERR_INVALID, "bad arguments");
   return transform_cloud(ctx, which, T);
 }
 
 int me_voxel_downsample(me_ctx *ctx, int which, double voxel_size, int64_t *n_out) {
   ME_ENTER(ctx);
+  ctx->cloud_gen++;      // stales the NN records (me_nn_curve*)
   if (which != ME_CLOUD_EST && which != ME_CLOUD_GT) return fail(ctx, ME_ERR_INVALID, "bad cloud id");
   return voxel_downsample(ctx, which, voxel_size, n_out);
 }
@@ -410,12 +414,14 @@ static bool cloud_id(int which) { return which == ME_CLOUD_EST || which == ME_CL
 
 int me_copy_cloud(me_ctx *ctx, int src, int dst) {
   ME_ENTER(ctx);
+  ctx->cloud_gen++;      // stales the NN records (me_nn_curve*)
   if (!cloud_id(src) || !cloud_id(dst) || src == dst) return fail(ctx, ME_ERR_INVALID, "me_copy_cloud: src and dst must be the two clouds");
   return copy_cloud(ctx, src, dst);
 }
 
 int me_add_gaussian_noise(me_ctx *ctx, int which, double std_dev, uint64_t seed) {
   ME_ENTER(ctx);
+  ctx->cloud_gen++;      // stales the NN records (me_nn_curve*)
   if (!cloud_id(which)) return fail(ctx, ME_ERR_INVALID, "bad cloud id");
   if (!(std::isfinite(std_dev) && std_dev >= 0.0)) return fail(ctx, ME_ERR_INVALID, "me_add_gaussian_noise: std_dev must be finite and >= 0");
   return add_gaussian_noise(ctx, which, std_dev, seed);
@@ -424,12 +430,14 @@ int me_add_gaussian_noise(me_ctx *ctx, int which, double std_dev, uint64_t seed)
 int me_add_non_uniform_density(me_ctx *ctx, int which, double sparse_ratio, double dense_ratio, double region_size, uint64_t seed,
                                int64_t *n_out) {
   ME_ENTER(ctx);
+  ctx->cloud_gen++;      // stales the NN records (me_nn_curve*)
   if (!cloud_id(which)) return fail(ctx, ME_ERR_INVALID, "bad cloud id");
   return add_non_uniform_density(ctx, which, sparse_ratio, dense_ratio, region_size, seed, n_out);
 }
 
 int me_add_sparse_outliers(me_ctx *ctx, int which, double outlier_ratio, double outlier_range, uint64_t seed, int64_t *n_out) {
   ME_ENTER(ctx);
+  ctx->cloud_gen++;      // stales the NN records (me_nn_curve*)
   if (!cloud_id(which)) return fail(ctx, ME_ERR_INVALID, "bad cloud id");
   if (!(std::isfinite(outlier_range) && outlier_range >= 0.0))
     return fail(ctx, ME_ERR_INVALID, "me_add_sparse_outliers: outlier_range must be finite and >= 0");
@@ -438,6 +446,7 @@ int me_add_sparse_outliers(me_ctx *ctx, int which, double outlier_ratio, double 
 
 int me_add_local_deformation(me_ctx *ctx, int which, double radius, double strength, const double center[3]) {
   ME_ENTER(ctx);
+  ctx->cloud_gen++;      // stales the NN records (me_nn_curve*)
   if (!cloud_id(which) || !center) return fail(ctx, ME_ERR_INVALID, "bad arguments");
   return add_local_deformation(ctx, which, radius, strength, center);
 }
@@ -460,6 +469,7 @@ int me_get_cloud(me_ctx *ctx, int which, double *xyz_host, int64_t capacity_poin
 int me_icp_point_to_point(me_ctx *ctx, double max_correspondence_distance, int32_t max_iteration, double relative_fitness,
                           double relative_rmse, const double T_init[16], me_icp_result *out) {
   ME_ENTER(ctx);
+  ctx->cloud_gen++;      // stales the NN records (me_nn_curve*)
   if (!T_init || !out) return fail(ctx, ME_ERR_INVALID, "null argument");
   return run_icp(ctx, ME_ICP_POINT_TO_POINT, max_correspondence_distance, max_iteration, relative_fitness, relative_rmse, T_init, out);
 }
@@ -467,6 +477,7 @@ int me_icp_point_to_point(me_ctx *ctx, double max_correspondence_distance, int32
 int me_icp(me_ctx *ctx, int32_t method, double max_correspondence_distance, int32_t max_iteration, double relative_fitness,
            double relative_rmse, const double T_init[16], me_icp_result *out) {
   ME_ENTER(ctx);
+  ctx->cloud_gen++;      // stales the NN records (me_nn_curve*)
   if (!T_init || !out) return fail(ctx, ME_ERR_INVALID, "null argument");
   return run_icp(ctx, method, max_correspondence_distance, max_iteration, relative_fitness, relative_rmse, T_init, out);
 }
@@ -474,6 +485,7 @@ int me_icp(me_ctx *ctx, int32_t method, double max_correspondence_distance, int3
 int me_icp_begin(me_ctx *ctx, int32_t method, double max_correspondence_distance, int32_t max_iteration, double relative_fitness,
                  double relative_rmse, const double T_init[16]) {
   ME_ENTER(ctx);
+  ctx->cloud_gen++;      // stales the NN records (me_nn_curve*)
   if (!T_init) return fail(ctx, ME_ERR_INVALID, "null argument");
   return icp_begin(ctx, method, max_correspondence_distance, max_iteration, relative_fitness, relative_rmse, T_init);
 }
@@ -563,6 +575,22 @@ int me_build_grid(me_ctx *ctx, int which) {
   return build_grid(ctx, which);
 }
 
+}  // extern "C"
+
+// a successful me_eval_nn*: its records serve me_nn_curve* until the clouds change (e, g == NULL: the accumulators are in
+// the device block)
+static void remember_nn(me_ctx *ctx, const me_nn_params *p, const me_nn_accum *e, const me_nn_accum *g) {
+  ctx->curve_valid = true;
+  ctx->curve_gen = ctx->cloud_gen;
+  ctx->curve_p = *p;
+  ctx->curve_acc_host = e || g;
+  std::memset(ctx->curve_acc, 0, sizeof(ctx->curve_acc));
+  if (e) ctx->curve_acc[0] = *e;
+  if (g) ctx->curve_acc[1] = *g;
+}
+
+extern "C" {
+
 int me_eval_nn_accum(me_ctx *ctx, const me_nn_params *p, me_nn_accum *est_to_gt, me_nn_accum *gt_to_est) {
   ME_ENTER(ctx);
   if (!p) return fail(ctx, ME_ERR_INVALID, "null params");
@@ -570,7 +598,10 @@ int me_eval_nn_accum(me_ctx *ctx, const me_nn_params *p, me_nn_accum *est_to_gt,
   if (p->pairing != ME_PAIRING_AS_WRITTEN && p->pairing != ME_PAIRING_GEOMETRIC) return fail(ctx, ME_ERR_INVALID, "bad pairing");
   const int dirs = p->directions ? p->directions : 3;
   if (((dirs & 1) && !est_to_gt) || ((dirs & 2) && !gt_to_est)) return fail(ctx, ME_ERR_INVALID, "null accumulator for a requested direction");
-  return run_nn(ctx, p, est_to_gt, gt_to_est);
+  ctx->curve_valid = false;
+  ME_TRY(run_nn(ctx, p, est_to_gt, gt_to_est));
+  remember_nn(ctx, p, est_to_gt, gt_to_est);
+  return ME_OK;
 }
 
 // ---- device-resident accumulators: sweep -> (all-reduce on the device by the caller) -> one fetch per pass ----------------
@@ -592,7 +623,10 @@ int me_eval_nn_accum_device(me_ctx *ctx, const me_nn_params *p) {
   if (!p) return fail(ctx, ME_ERR_INVALID, "null params");
   if (p->cutoff_mode != ME_CUTOFF_SQDIST_LE_R && p->cutoff_mode != ME_CUTOFF_DIST_LT_R) return fail(ctx, ME_ERR_INVALID, "bad cutoff_mode");
   if (p->pairing != ME_PAIRING_AS_WRITTEN && p->pairing != ME_PAIRING_GEOMETRIC) return fail(ctx, ME_ERR_INVALID, "bad pairing");
-  return run_nn(ctx, p, nullptr, nullptr, true);
+  ctx->curve_valid = false;
+  ME_TRY(run_nn(ctx, p, nullptr, nullptr, true));
+  remember_nn(ctx, p, nullptr, nullptr);
+  return ME_OK;
 }
 
 int me_eval_mme_accum_device(me_ctx *ctx, int which, double radius, int32_t min_neighbors) {
@@ -677,36 +711,67 @@ int me_accum_fetch(me_ctx *ctx, me_nn_accum *est_to_gt, me_nn_accum *gt_to_est, 
 
 }  // extern "C"
 
+// the per-level arithmetic of me_nn_finalize, shared with me_nn_curve_finalize so that a level both compute is one expression
+struct DirMoments {           // one direction's accumulator, reduced over the ranks
+  const me_nn_accum *a;
+  double nc;                  // |C|
+  bool moments;
+  double mean_all, m2_all;    // moments of d over all kept pairs, ranks merged in order
+};
+static DirMoments dir_moments(const me_nn_accum *a) {
+  DirMoments M;
+  M.a = a;
+  M.nc = (double)a->n_corr;
+  double n_all = 0;
+  M.mean_all = 0; M.m2_all = 0;
+  for (int s = 0; s < ME_MAX_WORLD; ++s) chan_merge(n_all, M.mean_all, M.m2_all, a->rank_n[s], a->rank_mean[s], a->rank_m2[s]);
+  // every sweep of the library fills the moments; an accumulator built from the sums only (its slots do not account for
+  // its pairs) has nothing better than the closed form, which cancels when the spread of d is small against its mean
+  M.moments = n_all == M.nc;
+  return M;
+}
+// one level (n_inlier pairs with d <= tau, their sum d and sum d^2) -> mean, rmse, fitness, sigma
+static void dir_level(const DirMoments &M, int64_t n_inlier, double sum_d, double sum_d2, int64_t n_source, double *mean_out,
+                      double *rmse_out, double *fitness_out, double *sigma_out) {
+  const double nc = M.nc;
+  const int target_num = (int)n_source;                       // map_eval.cpp:1128
+  const double mean = sum_d / nc;                              // :1125
+  *mean_out = mean;
+  *rmse_out = std::sqrt(sum_d2 / nc);                          // :1126,1131
+  *fitness_out = (double)n_inlier * 1.0 / target_num;          // :1130
+  // :1132-1138, the sum over ALL kept pairs of (d - mean_k)^2 = M2 + n (mean_all - mean_k)^2: both terms are >= 0, so
+  // nothing cancels however small the spread of d is against its mean
+  double ss;
+  if (M.moments) {
+    const double dm = M.mean_all - mean;
+    ss = M.m2_all + nc * dm * dm;
+  } else {
+    ss = M.a->sum_d2_all - 2.0 * mean * M.a->sum_d_all + nc * mean * mean;
+    if (ss < 0 && ss > -1e-9 * M.a->sum_d2_all) ss = 0;
+  }
+  *sigma_out = std::sqrt(ss / nc);
+}
+// map_eval.cpp:1245-1253 at one level
+static void pair_level(double e2g_fitness, double e2g_rmse, int64_t e2g_n_inlier, double g2e_rmse, int64_t n_est, int64_t n_gt,
+                       double *cd, double *f1, double *iou) {
+  *cd = e2g_rmse + g2e_rmse;
+  const double overlap = e2g_fitness, rmse = e2g_rmse;
+  *f1 = 2 * overlap * rmse / (overlap + rmse);
+  const int num_intersection = (int)e2g_n_inlier;
+  const int num_union = (int)(n_est + n_gt - num_intersection);
+  *iou = (double)num_intersection / num_union;
+}
+
 static void finalize_dir(const me_nn_accum *a, int64_t n_source, me_dir_result *r) {
   std::memset(r, 0, sizeof(*r));
   r->n_source = n_source;
   r->n_corr = a->n_corr;
   r->n_ub = a->n_ub;
   r->sum_nn_dist = a->sum_nn_dist;
-  const double nc = (double)a->n_corr;
-  const int target_num = (int)n_source;                       // map_eval.cpp:1128
-  double n_all = 0, mean_all = 0, m2_all = 0;                  // moments of d over all kept pairs, ranks merged in order
-  for (int s = 0; s < ME_MAX_WORLD; ++s) chan_merge(n_all, mean_all, m2_all, a->rank_n[s], a->rank_mean[s], a->rank_m2[s]);
-  // every sweep of the library fills the moments; an accumulator built from the sums only (its slots do not account for
-  // its pairs) has nothing better than the closed form, which cancels when the spread of d is small against its mean
-  const bool moments = n_all == nc;
+  const DirMoments M = dir_moments(a);
   for (int k = 0; k < 5; ++k) {
     r->n_inlier[k] = a->n_inlier[k];
-    const double mean = a->sum_d[k] / nc;                      // :1125
-    r->mean[k] = mean;
-    r->rmse[k] = std::sqrt(a->sum_d2[k] / nc);                 // :1126,1131
-    r->fitness[k] = (double)a->n_inlier[k] * 1.0 / target_num; // :1130
-    // :1132-1138, the sum over ALL kept pairs of (d - mean_k)^2 = M2 + n (mean_all - mean_k)^2: both terms are >= 0, so
-    // nothing cancels however small the spread of d is against its mean
-    double ss;
-    if (moments) {
-      const double dm = mean_all - mean;
-      ss = m2_all + nc * dm * dm;
-    } else {
-      ss = a->sum_d2_all - 2.0 * mean * a->sum_d_all + nc * mean * mean;
-      if (ss < 0 && ss > -1e-9 * a->sum_d2_all) ss = 0;
-    }
-    r->sigma[k] = std::sqrt(ss / nc);
+    dir_level(M, a->n_inlier[k], a->sum_d[k], a->sum_d2[k], n_source, &r->mean[k], &r->rmse[k], &r->fitness[k], &r->sigma[k]);
   }
 }
 
@@ -719,15 +784,78 @@ int me_nn_finalize(const me_nn_params *p, const me_nn_accum *est_to_gt, const me
   const int dirs = p->directions ? p->directions : 3;
   if (dirs & 1) finalize_dir(est_to_gt ? est_to_gt : &zero, n_est, &out->est_to_gt);
   if (dirs & 2) finalize_dir(gt_to_est ? gt_to_est : &zero, n_gt, &out->gt_to_est);
-  for (int k = 0; k < 5; ++k) {                                 // map_eval.cpp:1245-1253
-    out->cd[k] = out->est_to_gt.rmse[k] + out->gt_to_est.rmse[k];
-    const double overlap = out->est_to_gt.fitness[k], rmse = out->est_to_gt.rmse[k];
-    out->f1[k] = 2 * overlap * rmse / (overlap + rmse);
-    const int num_intersection = (int)out->est_to_gt.n_inlier[k];
-    const int num_union = (int)(n_est + n_gt - num_intersection);
-    out->iou[k] = (double)num_intersection / num_union;
-  }
+  for (int k = 0; k < 5; ++k)
+    pair_level(out->est_to_gt.fitness[k], out->est_to_gt.rmse[k], out->est_to_gt.n_inlier[k], out->gt_to_est.rmse[k], n_est, n_gt,
+               &out->cd[k], &out->f1[k], &out->iou[k]);
   out->full_cd = p->want_full_cd ? (out->est_to_gt.sum_nn_dist / (double)n_est + out->gt_to_est.sum_nn_dist / (double)n_gt) : 0.0;
+  return ME_OK;
+}
+
+// 1 <= K <= ME_CURVE_MAX_LEVELS, every level finite and >= 0, non-decreasing
+static bool curve_levels_ok(const double *tau, int32_t K) {
+  if (!tau || K < 1 || K > ME_CURVE_MAX_LEVELS) return false;
+  for (int k = 0; k < K; ++k)
+    if (!(std::isfinite(tau[k]) && tau[k] >= 0.0) || (k && tau[k] < tau[k - 1])) return false;
+  return true;
+}
+
+int me_nn_curve_finalize(const me_nn_params *p, const me_nn_accum *est_to_gt, const me_nn_accum *gt_to_est,
+                         const double *host_block, const double *tau, int32_t n_tau, int64_t n_est, int64_t n_gt,
+                         me_curve_row *rows) {
+  if (!p || !host_block || !rows || !curve_levels_ok(tau, n_tau)) return ME_ERR_INVALID;
+  const int K = n_tau, stride = 3 * (K + 1) + 1;
+  std::memset(rows, 0, (size_t)K * sizeof(me_curve_row));
+  me_nn_accum zero;
+  std::memset(&zero, 0, sizeof(zero));
+  const int dirs = p->directions ? p->directions : 3;
+  const me_nn_accum *acc[2] = {est_to_gt ? est_to_gt : &zero, gt_to_est ? gt_to_est : &zero};
+  const int64_t n_src[2] = {n_est, n_gt};
+  for (int q = 0; q < 2; ++q) {
+    if (!(dirs & (1 << q))) continue;
+    const double *cnt = host_block + q * stride, *sd = cnt + (K + 1), *sq = sd + (K + 1);
+    double all = 0;
+    for (int b = 0; b <= K; ++b) all += cnt[b];
+    if (all != (double)acc[q]->n_corr) return ME_ERR_INVALID;      // the block and the accumulators of different evaluations
+    const DirMoments M = dir_moments(acc[q]);
+    double c = 0, s1 = 0, s2 = 0;       // prefix sums over the bins: the pairs with d <= tau_k
+    for (int k = 0; k < K; ++k) {
+      c += cnt[k]; s1 += sd[k]; s2 += sq[k];
+      me_curve_dir *r = q == 0 ? &rows[k].est_to_gt : &rows[k].gt_to_est;
+      r->n_inlier = (int64_t)std::llround(c);
+      dir_level(M, r->n_inlier, s1, s2, n_src[q], &r->mean, &r->rmse, &r->fitness, &r->sigma);
+    }
+  }
+  for (int k = 0; k < K; ++k) {
+    me_curve_row &r = rows[k];
+    r.tau = tau[k];
+    pair_level(r.est_to_gt.fitness, r.est_to_gt.rmse, r.est_to_gt.n_inlier, r.gt_to_est.rmse, n_est, n_gt, &r.cd, &r.f1, &r.iou);
+  }
+  return ME_OK;
+}
+
+int me_nn_curve_accum_device(me_ctx *ctx, const double *tau, int32_t n_tau, double **device_block, int32_t *n) {
+  ME_ENTER(ctx);
+  if (!device_block || !n) return fail(ctx, ME_ERR_INVALID, "null argument");
+  if (!curve_levels_ok(tau, n_tau))
+    return fail(ctx, ME_ERR_INVALID, "me_nn_curve*: 1 <= n_tau <= ME_CURVE_MAX_LEVELS levels, finite, >= 0 and non-decreasing");
+  return nn_curve(ctx, tau, n_tau, device_block, n);
+}
+
+int me_nn_curve(me_ctx *ctx, const double *tau, int32_t n_tau, me_curve_row *rows) {
+  ME_ENTER(ctx);
+  if (!rows) return fail(ctx, ME_ERR_INVALID, "null argument");
+  if (ctx->world != 1) return fail(ctx, ME_ERR_INVALID, "me_nn_curve needs world == 1; use me_nn_curve_accum_device + all-reduce + me_nn_curve_finalize");
+  double *d_blk = nullptr;
+  int32_t n = 0;
+  ME_TRY(me_nn_curve_accum_device(ctx, tau, n_tau, &d_blk, &n));
+  me_nn_accum acc[2];
+  if (ctx->curve_acc_host) { acc[0] = ctx->curve_acc[0]; acc[1] = ctx->curve_acc[1]; }
+  else ME_TRY(me_accum_fetch(ctx, &acc[0], &acc[1], nullptr, nullptr));
+  std::vector<double> h((size_t)n);
+  ME_CUDA(ctx, cudaMemcpyAsync(h.data(), d_blk, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (me_nn_curve_finalize(&ctx->curve_p, &acc[0], &acc[1], h.data(), tau, n_tau, ctx->cloud[0].n, ctx->cloud[1].n, rows) != ME_OK)
+    return fail(ctx, ME_ERR_INVALID, "me_nn_curve_finalize: the curve block does not match the accumulators");
   return ME_OK;
 }
 

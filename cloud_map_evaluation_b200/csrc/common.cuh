@@ -222,6 +222,16 @@ struct me_ctx {
   int mme_rows_cfg = 0;
   unsigned int *d_trace = nullptr;
   me::IcpRun icp;
+  // accuracy curve (me_nn_curve*): the records of the last me_eval_nn* serve it while no call has since moved, replaced or
+  // re-swept a cloud — every such call bumps cloud_gen
+  unsigned long long cloud_gen = 0;
+  bool curve_valid = false;            // the last me_eval_nn* succeeded
+  unsigned long long curve_gen = 0;    // cloud_gen at that call
+  me_nn_params curve_p{};              // its parameters
+  bool curve_acc_host = false;         // its accumulators are curve_acc (me_eval_nn_accum), else in d_block (the _device call)
+  me_nn_accum curve_acc[2];
+  double *d_curve = nullptr;           // the curve block (both directions), then the levels
+  long long cap_curve = 0;
   std::string err;
 };
 
@@ -322,6 +332,8 @@ int radix_sort_pairs(me_ctx *ctx, unsigned long long *keys, uint32_t *vals, unsi
 // sweep_only: the per-query results only (d_nn_idx / d_nn_d2), no accumulators handed out (registration)
 int run_nn(me_ctx *ctx, const me_nn_params *p, me_nn_accum *e2g, me_nn_accum *g2e, bool to_block = false, bool sweep_only = false);
 int unsort_nn(me_ctx *ctx, int which_query, int32_t *h_idx, double *h_d2);
+// the curve block of the last me_eval_nn* at the K levels tau (host memory, checked by the caller) — me_nn_curve_accum_device
+int nn_curve(me_ctx *ctx, const double *tau, int K, double **device_block, int32_t *n);
 int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors, me_mme_accum *out, bool to_block = false);
 
 // layout of me_ctx::d_block (fp64): the SUM-reducible part first, then the MAX-reducible part.  Counts ride as fp64 (exact

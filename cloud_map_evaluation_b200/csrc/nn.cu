@@ -84,19 +84,18 @@ __device__ __forceinline__ bool keep_pair(double d2, const NNConst &c) {
   return c.cutoff_mode == ME_CUTOFF_SQDIST_LE_R ? (d2 <= c.cutoff) : (d2 < c.cutoff);
 }
 
+// the distance d of a kept pair, map_eval.cpp:1095: sqrt of Eigen's squaredNorm
+__device__ __forceinline__ double pair_dist(double sq) { return __dsqrt_rn(sq); }
+
 // map_eval.cpp:1095-1123 for one kept pair (source - target)
 // sq = Eigen's squaredNorm of (source - target), x*x + (y*y + z*z)
 template <class Acc>
 __device__ __forceinline__ void accum_sq(double sq, const NNConst &c, Acc &a) {
-  double nd = __dsqrt_rn(sq);
+  double nd = pair_dist(sq);
   a.pair(nd, sq);
 #pragma unroll
   for (int k = 0; k < 5; ++k)
     if (nd <= c.tau[k]) a.inlier(k, nd, sq);
-}
-template <class Acc>
-__device__ __forceinline__ void accum_pair(double dx, double dy, double dz, const NNConst &c, Acc &a) {
-  accum_sq(sqnorm_eigen(dx, dy, dz), c, a);
 }
 
 // (n, mean, M2) of the whole block from every thread's (n, mean, M2), valid in thread 0; every thread of the block calls it
@@ -860,6 +859,25 @@ nn_stats_kernel(long long i_begin, long long i_end, const int32_t *__restrict__ 
 // :1093-1094 reads gt[nn_est] and est[i_gt].  Reproduced verbatim; out-of-range (UB in the reference) is counted.
 // Walks every gt point; points this rank did not evaluate carry the marker -2.
 // ---------------------------------------------------------------------------------------------------------------
+enum { kAwNone = 0, kAwOutOfRange = 1, kAwPair = 2 };
+// gt query i (sorted order): kAwNone (no kept pair), kAwOutOfRange (counted in n_ub) or kAwPair with sq = Eigen's
+// squaredNorm of gt[nn_est] - est[i_gt]
+__device__ __forceinline__ int as_written_pair(const P4 *__restrict__ Qgt, long long i, const int32_t *__restrict__ nn_idx,
+                                               const double *__restrict__ nn_d2, const double *__restrict__ gt_xyz, long long n_gt,
+                                               const double *__restrict__ est_xyz, long long n_est, const NNConst &C, double &sq) {
+  const int32_t nn_est = nn_idx[i];
+  if (nn_est < 0) return kAwNone;
+  if (!keep_pair(nn_d2[i], C)) return kAwNone;
+  const long long i_gt = orig_of(__double_as_longlong(__ldg(reinterpret_cast<const double *>(Qgt + i) + 3)));
+  const long long s = nn_est, t = i_gt;          // source index into gt, target index into est
+  if (s >= n_gt || t >= n_est) return kAwOutOfRange;
+  const double dx = __dsub_rn(__ldg(gt_xyz + 3 * s), __ldg(est_xyz + 3 * t));
+  const double dy = __dsub_rn(__ldg(gt_xyz + 3 * s + 1), __ldg(est_xyz + 3 * t + 1));
+  const double dz = __dsub_rn(__ldg(gt_xyz + 3 * s + 2), __ldg(est_xyz + 3 * t + 2));
+  sq = sqnorm_eigen(dx, dy, dz);
+  return kAwPair;
+}
+
 __global__ void __launch_bounds__(kThreads, 4)      // as nn_stats_kernel
 pair_as_written_kernel(const P4 *__restrict__ Qgt, long long n, const int32_t *__restrict__ nn_idx,
                        const double *__restrict__ nn_d2, const double *__restrict__ gt_xyz, long long n_gt,
@@ -868,18 +886,129 @@ pair_as_written_kernel(const P4 *__restrict__ Qgt, long long n, const int32_t *_
   LocalAcc a;
   a.clear();
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const int32_t nn_est = nn_idx[i];
-    if (nn_est < 0) continue;
-    if (!keep_pair(nn_d2[i], C)) continue;
-    const long long i_gt = orig_of(__double_as_longlong(__ldg(reinterpret_cast<const double *>(Qgt + i) + 3)));
-    const long long s = nn_est, t = i_gt;          // source index into gt, target index into est
-    if (s >= n_gt || t >= n_est) { a.ub(); continue; }
-    const double dx = __dsub_rn(__ldg(gt_xyz + 3 * s), __ldg(est_xyz + 3 * t));
-    const double dy = __dsub_rn(__ldg(gt_xyz + 3 * s + 1), __ldg(est_xyz + 3 * t + 1));
-    const double dz = __dsub_rn(__ldg(gt_xyz + 3 * s + 2), __ldg(est_xyz + 3 * t + 2));
-    accum_pair(dx, dy, dz, C, a);
+    double sq;
+    const int r = as_written_pair(Qgt, i, nn_idx, nn_d2, gt_xyz, n_gt, est_xyz, n_est, C, sq);
+    if (r == kAwOutOfRange) a.ub();
+    else if (r == kAwPair) accum_sq(sq, C, a);
   }
   flush_acc(a, acc, mom);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Accuracy curve (me_nn_curve_accum_device): the records of the last sweep folded into K + 1 distance bins.  A kept
+// pair goes to bin b = the first level k with d <= tau_k (K when it exceeds every level); it counts for every level
+// k >= b, so the host forms each level's sums as prefix sums over the bins.  Per bin: count, sum d, sum sq.
+// Deterministic: block j owns the fixed contiguous slice j of the records; per tile every warp sorts its 32 pairs by
+// bin (bitonic, keys unique by lane) and sums each bin's segment with a fixed shuffle tree; warp 0 adds the segment
+// totals of the 8 warps in warp order into the block's bins in shared memory.  nn_curve_merge_kernel sums the blocks'
+// bins in block order.  No floating-point atomics anywhere.
+// ---------------------------------------------------------------------------------------------------------------
+static constexpr int kCurveThreads = 256;
+static constexpr int kCurveWarps = kCurveThreads / 32;
+
+struct CurveSrc {           // the per-query records of one direction
+  long long b, e;           // sorted range the sweep filled (entries < 0 in it: no neighbour / another rank's query)
+  const int32_t *nn_idx;
+  const double *nn_d2, *nn_sq;
+  int as_written;           // ME_PAIRING_AS_WRITTEN gt->est: the distance comes from the swapped indices
+  const P4 *Qgt;
+  const double *gt_xyz, *est_xyz;
+  long long n_gt, n_est;
+};
+
+// first k in [0, K) with d <= tau[k], K if none (tau non-decreasing)
+__device__ __forceinline__ int curve_bin(const double *tau, int K, double d) {
+  int lo = 0, hi = K;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (d <= tau[mid]) hi = mid; else lo = mid + 1;
+  }
+  return lo;
+}
+
+// per block: part[blockIdx.x * stride ..] = cnt[K + 1], sum_d[K + 1], sum_sq[K + 1], n_ub  (stride = 3 (K + 1) + 1)
+__global__ void __launch_bounds__(kCurveThreads, 4)
+nn_curve_kernel(CurveSrc S, NNConst C, const double *__restrict__ tau, int K, long long per_block, double *__restrict__ part) {
+  extern __shared__ double curve_sm[];
+  double *s_tau = curve_sm, *s_cnt = curve_sm + K, *s_sd = s_cnt + (K + 1), *s_sq = s_sd + (K + 1);
+  __shared__ int seg_bin[2][kCurveThreads], seg_n[2][kCurveThreads];
+  __shared__ double seg_d[2][kCurveThreads], seg_q[2][kCurveThreads];
+  __shared__ unsigned long long s_ub;
+  const int lane = threadIdx.x & 31;
+  for (int t = threadIdx.x; t < K; t += kCurveThreads) s_tau[t] = tau[t];
+  for (int t = threadIdx.x; t < 3 * (K + 1); t += kCurveThreads) s_cnt[t] = 0.0;
+  if (threadIdx.x == 0) s_ub = 0;
+  __syncthreads();
+  const long long b0 = S.b + blockIdx.x * per_block, b1 = min(S.e, b0 + per_block);
+  unsigned int ub = 0;
+  int buf = 0;
+  for (long long base = b0; base < b1; base += kCurveThreads) {
+    const long long i = base + threadIdx.x;
+    int bin = K + 1;                 // no kept pair: sorts last, never folded
+    double d = 0.0, sq = 0.0;
+    if (i < b1) {
+      bool kept = false;
+      if (S.as_written) {
+        const int r = as_written_pair(S.Qgt, i, S.nn_idx, S.nn_d2, S.gt_xyz, S.n_gt, S.est_xyz, S.n_est, C, sq);
+        ub += r == kAwOutOfRange;
+        kept = r == kAwPair;
+      } else if (__ldg(S.nn_idx + i) >= 0 && keep_pair(__ldg(S.nn_d2 + i), C)) {
+        sq = __ldg(S.nn_sq + i);
+        kept = true;
+      }
+      if (kept) { d = pair_dist(sq); bin = curve_bin(s_tau, K, d); }
+    }
+    // sort the warp's (bin, lane) keys ascending, then fetch the values in that order
+    unsigned int key = ((unsigned int)bin << 5) | (unsigned int)lane;
+#pragma unroll
+    for (int k = 2; k <= 32; k <<= 1)
+#pragma unroll
+      for (int j = k >> 1; j > 0; j >>= 1) {
+        const unsigned int o = __shfl_xor_sync(0xffffffffu, key, j);
+        const bool up = (lane & k) == 0 || k == 32, lower = (lane & j) == 0;
+        key = (lower == up) ? min(key, o) : max(key, o);
+      }
+    const int src = (int)(key & 31u), kb = (int)(key >> 5);
+    d = __shfl_sync(0xffffffffu, d, src);
+    sq = __shfl_sync(0xffffffffu, sq, src);
+    const int prev = __shfl_up_sync(0xffffffffu, kb, 1);
+    const unsigned int heads = __ballot_sync(0xffffffffu, lane == 0 || prev != kb);
+    const int head = 31 - __clz(heads & (0xffffffffu >> (31 - lane)));     // first lane of this lane's segment
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {      // inclusive scan within the segment, a fixed tree
+      const double du = __shfl_up_sync(0xffffffffu, d, o), qu = __shfl_up_sync(0xffffffffu, sq, o);
+      if (lane - o >= head) { d += du; sq += qu; }
+    }
+    const bool tail = lane == 31 || ((heads >> (lane + 1)) & 1u);
+    seg_bin[buf][threadIdx.x] = (tail && kb <= K) ? kb : -1;
+    seg_n[buf][threadIdx.x] = lane - head + 1;
+    seg_d[buf][threadIdx.x] = d;
+    seg_q[buf][threadIdx.x] = sq;
+    __syncthreads();
+    if (threadIdx.x < 32) {      // the bins of one warp's tails are distinct: one pass per warp, in warp order
+      for (int w = 0; w < kCurveWarps; ++w) {
+        const int s = w * 32 + lane, bb = seg_bin[buf][s];
+        if (bb >= 0) { s_cnt[bb] += (double)seg_n[buf][s]; s_sd[bb] += seg_d[buf][s]; s_sq[bb] += seg_q[buf][s]; }
+        __syncwarp();
+      }
+    }
+    buf ^= 1;      // the other buffer: warp 0 folds this one while the others fill the next
+  }
+  if (ub) atomicAdd(&s_ub, (unsigned long long)ub);
+  __syncthreads();
+  const int stride = 3 * (K + 1) + 1;
+  double *out = part + (long long)blockIdx.x * stride;
+  for (int t = threadIdx.x; t < 3 * (K + 1); t += kCurveThreads) out[t] = s_cnt[t];
+  if (threadIdx.x == 0) out[3 * (K + 1)] = (double)s_ub;
+}
+
+// blk[t] = sum over the blocks, in block order, of part[. * stride + t]
+__global__ void nn_curve_merge_kernel(const double *__restrict__ part, int n_blocks, int stride, double *__restrict__ blk) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= stride) return;
+  double s = 0.0;
+  for (int b = 0; b < n_blocks; ++b) s += part[(long long)b * stride + t];
+  blk[t] = s;
 }
 
 __global__ void fill_i32_kernel(int32_t *p, long long n, int32_t v) {
@@ -936,6 +1065,11 @@ __global__ void pack_nn_kernel(const AccBlock *__restrict__ a, const unsigned lo
 // ---------------------------------------------------------------------------------------------------------------
 // host driver
 // ---------------------------------------------------------------------------------------------------------------
+static void set_cutoff(NNConst &C, const me_nn_params *p) {
+  C.cutoff_mode = p->cutoff_mode;
+  C.cutoff = p->cutoff_mode == ME_CUTOFF_SQDIST_LE_R ? p->icp_max_distance : p->icp_max_distance * p->icp_max_distance;
+}
+
 static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, me_nn_accum *out, int stage, bool to_block) {
   Cloud &Qc = ctx->cloud[qwhich];
   Cloud &Rc = ctx->cloud[1 - qwhich];
@@ -943,8 +1077,7 @@ static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, me_nn_a
 
   NNConst C;
   for (int k = 0; k < 5; ++k) C.tau[k] = p->tau[k];
-  C.cutoff_mode = p->cutoff_mode;
-  C.cutoff = p->cutoff_mode == ME_CUTOFF_SQDIST_LE_R ? p->icp_max_distance : p->icp_max_distance * p->icp_max_distance;
+  set_cutoff(C, p);
   const bool as_written = (qwhich == ME_CLOUD_GT && p->pairing == ME_PAIRING_AS_WRITTEN);
   C.accumulate = as_written ? 0 : 1;
   C.want_full_cd = p->want_full_cd ? 1 : 0;
@@ -1128,6 +1261,47 @@ int run_nn(me_ctx *ctx, const me_nn_params *p, me_nn_accum *e2g, me_nn_accum *g2
   if (sweep_only) { e2g = g2e = nullptr; to_block = false; }
   if ((dirs & 1) && (e2g || to_block || sweep_only)) ME_TRY(run_direction(ctx, ME_CLOUD_EST, p, e2g, 2, to_block));
   if ((dirs & 2) && (g2e || to_block || sweep_only)) ME_TRY(run_direction(ctx, ME_CLOUD_GT, p, g2e, 3, to_block));
+  return ME_OK;
+}
+
+int nn_curve(me_ctx *ctx, const double *tau, int K, double **device_block, int32_t *n) {
+  const me_nn_params *p = &ctx->curve_p;
+  const int dirs = p->directions ? p->directions : 3;
+  bool fresh = ctx->curve_valid && ctx->curve_gen == ctx->cloud_gen;
+  for (int q = 0; q < 2; ++q) fresh = fresh && (!(dirs & (1 << q)) || ctx->cloud[q].nn_valid);
+  if (!fresh)
+    return fail(ctx, ME_ERR_INVALID, "me_nn_curve*: no current NN records; run me_eval_nn* after the last change of the clouds "
+                                     "(me_set_cloud*, me_transform, me_voxel_downsample, me_copy_cloud, me_add_*, ICP, a new layout)");
+  const int stride = 3 * (K + 1) + 1;
+  ME_TRY(ensure(ctx, (void **)&ctx->d_curve, &ctx->cap_curve, 2 * stride + K, sizeof(double)));
+  double *blk = ctx->d_curve, *d_tau = ctx->d_curve + 2 * stride;
+  const int max_blocks = ctx->sm_count * 4;
+  ME_TRY(ensure_work(ctx, (size_t)max_blocks * stride * sizeof(double)));
+  ME_CUDA(ctx, cudaMemcpyAsync(d_tau, tau, (size_t)K * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  ME_CUDA(ctx, cudaMemsetAsync(blk, 0, 2 * (size_t)stride * sizeof(double), ctx->stream));
+  const size_t smem = (size_t)(K + 3 * (K + 1)) * sizeof(double);
+  for (int q = 0; q < 2; ++q) {
+    if (!(dirs & (1 << q))) continue;
+    const Cloud &Qc = ctx->cloud[q], &Rc = ctx->cloud[1 - q];
+    NNConst C{};
+    set_cutoff(C, p);
+    CurveSrc S;
+    S.as_written = q == ME_CLOUD_GT && p->pairing == ME_PAIRING_AS_WRITTEN;
+    S.b = S.as_written ? 0 : Qc.nn_b;       // the ranges nn_stats_kernel / pair_as_written_kernel walk
+    S.e = S.as_written ? Qc.ns : Qc.nn_e;
+    S.nn_idx = Qc.d_nn_idx; S.nn_d2 = Qc.d_nn_d2; S.nn_sq = Qc.d_nn_sq;
+    S.Qgt = Qc.d_sorted; S.gt_xyz = Qc.d_xyz; S.n_gt = Qc.n; S.est_xyz = Rc.d_xyz; S.n_est = Rc.n;
+    if (S.e <= S.b) continue;
+    const int n_blocks = (int)std::min<long long>((S.e - S.b + kCurveThreads - 1) / kCurveThreads, max_blocks);
+    const long long per_block = (S.e - S.b + n_blocks - 1) / n_blocks;
+    nn_curve_kernel<<<n_blocks, kCurveThreads, smem, ctx->stream>>>(S, C, d_tau, K, per_block, (double *)ctx->d_work);
+    ME_LAUNCH_CHECK(ctx);
+    nn_curve_merge_kernel<<<(stride + 255) / 256, 256, 0, ctx->stream>>>((const double *)ctx->d_work, n_blocks, stride,
+                                                                        blk + q * stride);
+    ME_LAUNCH_CHECK(ctx);
+  }
+  *device_block = blk;
+  *n = 2 * stride;
   return ME_OK;
 }
 

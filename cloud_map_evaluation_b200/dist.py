@@ -99,6 +99,20 @@ def allreduce_block(ctx, device, group=None):
     dist.all_reduce(t[n_sum:], op=dist.ReduceOp.MAX, group=group)
 
 
+def allreduce_curve(ctx, tau, device, group=None):
+    """The accuracy curve block of every rank at the levels tau (MapEvalB200.curve_accum_device), SUM-all-reduced in place
+    on the device (counts ride as fp64, exact), returned as a host numpy array for api.curve_finalize, which every rank
+    then runs with its reduced NN accumulators."""
+    import torch
+    import torch.distributed as dist
+    ptr, n = ctx.curve_accum_device(tau)
+    ctx.synchronize()
+    t = torch.as_tensor(_DeviceBlock(ptr, n), device=device)
+    if dist.is_initialized() and dist.get_world_size(group) > 1:
+        dist.all_reduce(t, group=group)
+    return t.cpu().numpy().copy()
+
+
 def icp_distributed(ctx, device, max_correspondence_distance, T_init=None, max_iteration=30, relative_fitness=1e-6,
                     relative_rmse=1e-6, method=A.ME_ICP_GENERALIZED, group=None):
     """performICPRegistration on every rank of the job (map_eval.cpp:1366-1394): the clouds are replicated, every rank

@@ -123,6 +123,18 @@ class GpuGroup {
     return sync_streams();
   }
 
+  // the accuracy curve blocks the contexts hold (me_nn_curve_accum_device, after me_synchronize): ONE grouped SUM all-reduce
+  // in place, then rank 0's reduced block into `host` (its size = the block's length)
+  bool reduce_curve(const std::vector<double *> &ptr, std::vector<double> &host) {
+    if (!allreduce_device(ptr, host.size(), ncclSum)) return false;
+    if (cudaSetDevice(dev_[0]) != cudaSuccess ||
+        cudaMemcpy(host.data(), ptr[0], host.size() * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess) {
+      err_ = "copying the accuracy curve block back failed";
+      return false;
+    }
+    return true;
+  }
+
   // sum-reduce the NN accumulators of all ranks (counts ride along as fp64: exact below 2^53, order-independent)
   bool reduce_nn(std::vector<me_nn_accum> &e2g, std::vector<me_nn_accum> &g2e) {
     const int n = size();

@@ -87,6 +87,10 @@ struct Param {   // map_eval.h:60-116
   double global_registration_voxel_size_ = 0.5;
   uint64_t global_registration_seed_ = 0;
   int64_t global_registration_hypotheses_ = 100000;
+  // accuracy curve: AC / COM / CD / F1 / IoU at tau_k = (accuracy_curve_max * k) / accuracy_curve_steps, k = 1..steps, written to
+  // accuracy_curve.txt (me_nn_curve*: no new sweep); 0 = off.  accuracy_curve_max defaults to the largest accuracy_level
+  int accuracy_curve_steps_ = 0;
+  double accuracy_curve_max_ = 0.0;
 };
 
 // map_eval_main.cpp:120-208
@@ -146,6 +150,9 @@ inline Param loadParametersFromYAML(const std::string &yaml_file_path) {
       param.global_registration_hypotheses_ = (int64_t)config["global_registration_hypotheses"].as<uint64_t>();
     if (config["deform_center"] && config["deform_center"].size() >= 3)
       for (int a = 0; a < 3; ++a) param.deform_center_[a] = config["deform_center"][a].as<double>();
+    if (config["accuracy_curve_steps"]) param.accuracy_curve_steps_ = config["accuracy_curve_steps"].as<int>();
+    param.accuracy_curve_max_ = config["accuracy_curve_max"] ? config["accuracy_curve_max"].as<double>()
+                                                             : *std::max_element(param.trunc_dist_, param.trunc_dist_ + 5);
     return param;
   } catch (const std::exception &e) {
     std::cerr << "Error loading parameters: " << e.what() << std::endl;
@@ -172,7 +179,8 @@ inline void dumpParam(const Param &p, std::ostream &os) {
      << "\ndeform_center=" << p.deform_center_[0] << "," << p.deform_center_[1] << "," << p.deform_center_[2]
      << "\nglobal_registration=" << p.global_registration_ << "\nglobal_registration_voxel_size=" << p.global_registration_voxel_size_
      << "\nglobal_registration_seed=" << p.global_registration_seed_
-     << "\nglobal_registration_hypotheses=" << p.global_registration_hypotheses_ << "\n";
+     << "\nglobal_registration_hypotheses=" << p.global_registration_hypotheses_
+     << "\naccuracy_curve_steps=" << p.accuracy_curve_steps_ << "\naccuracy_curve_max=" << p.accuracy_curve_max_ << "\n";
 }
 
 // Eigen's default IOFormat for `vec.transpose()`: coefficients right-aligned to a common width, one space apart
@@ -227,6 +235,14 @@ class MapEvalB200 {
  public:
   // Configurations this driver cannot run, reported BEFORE map_results.txt is opened (no partial record is left behind).
   static bool validate(const Param &p, std::string *why) {
+    if (p.accuracy_curve_steps_ < 0 || p.accuracy_curve_steps_ > ME_CURVE_MAX_LEVELS) {
+      *why = "accuracy_curve_steps: " + std::to_string(p.accuracy_curve_steps_) + " is outside 0 .. " + std::to_string(ME_CURVE_MAX_LEVELS);
+      return false;
+    }
+    if (p.accuracy_curve_steps_ > 0 && !(std::isfinite(p.accuracy_curve_max_) && p.accuracy_curve_max_ >= 0.0)) {
+      *why = "accuracy_curve_max must be finite and >= 0";
+      return false;
+    }
     if (p.evaluate_using_initial_) return true;
     if (p.evaluation_method_ < 0 || p.evaluation_method_ > 2) {
       *why = "Invalid registration type specified (registration_methods: " + std::to_string(p.evaluation_method_) +
@@ -294,6 +310,7 @@ class MapEvalB200 {
   std::string simulationSummary() const;
   int renderEntropy(int which, int64_t n, render::ColoredCloud *out);
   int renderDistances(bool cutoff_strict);
+  int accuracyCurve(const me_nn_params &p, const std::vector<me_nn_accum> &e2g, const std::vector<me_nn_accum> &g2e);
   GpuGroup gpus_;            // one context per GPU; rank r evaluates the r-th shard of every sweep's query range
   me_ctx *ctx_ = nullptr;    // = gpus_.ctx(0): the voxel stage and the single-GPU calls
   std::vector<double> map_3d_, gt_3d_;   // N x 3 fp64, the layout of open3d PointCloud::points_ (as loaded)
@@ -573,6 +590,7 @@ inline int MapEvalB200::calculateMetricsWithInitialMatrix() {
   if (!gpus_.reduce_nn(e2g, g2e)) return fail("all-reduce of the NN accumulators");
   if (me_nn_finalize(&p, &e2g[0], &g2e[0], n_est_, n_gt_, &nn_) != ME_OK) return fail("me_nn_finalize");
   t_acc = tic.toc() / 1000.0;
+  if (param_.accuracy_curve_steps_ > 0 && accuracyCurve(p, e2g, g2e) != 0) return -1;
   if (nn_.gt_to_est.n_ub > 0)
     std::cerr << "WARNING: " << nn_.gt_to_est.n_ub << " gt->est pairs index past the end of a cloud (the reference reads out of "
                  "bounds there, map_eval.cpp:1233 vs :1093-1094: undefined behaviour); they are left out of the gt->est statistics, "
@@ -584,6 +602,42 @@ inline int MapEvalB200::calculateMetricsWithInitialMatrix() {
   std::cout << "INFO: est-gt MME: " << mme_est << " " << mme_gt << std::endl;
   std::cout << "INFO: IoU: " << eigenRow(nn_.iou, 5, 6) << std::endl;
   std::cout << "INFO: Full Chamfer distance (not computed by the reference on this path): " << nn_.full_cd << std::endl;
+  return 0;
+}
+
+// accuracy curve: the pass's NN records at accuracy_curve_steps levels (me_nn_curve_accum_device on every GPU, one NCCL
+// all-reduce of the blocks, me_nn_curve_finalize with the reduced accumulators) -> accuracy_curve.txt next to map_results.txt
+inline int MapEvalB200::accuracyCurve(const me_nn_params &p, const std::vector<me_nn_accum> &e2g, const std::vector<me_nn_accum> &g2e) {
+  const int K = param_.accuracy_curve_steps_;
+  std::vector<double> tau(K);
+  for (int k = 1; k <= K; ++k) tau[k - 1] = (param_.accuracy_curve_max_ * (double)k) / (double)K;
+  std::vector<double *> ptr(gpus_.size(), nullptr);
+  std::vector<int32_t> len(gpus_.size(), 0);
+  if (gpus_.for_each([&](int r, me_ctx *c) {
+        const int rc = me_nn_curve_accum_device(c, tau.data(), K, &ptr[r], &len[r]);
+        return rc != ME_OK ? rc : me_synchronize(c);
+      }) != ME_OK)
+    return fail("me_nn_curve_accum_device");
+  std::vector<double> blk((size_t)len[0]);
+  if (!gpus_.reduce_curve(ptr, blk)) return fail("all-reduce of the accuracy curve");
+  std::vector<me_curve_row> rows(K);
+  if (me_nn_curve_finalize(&p, &e2g[0], &g2e[0], blk.data(), tau.data(), K, n_est_, n_gt_, rows.data()) != ME_OK)
+    return fail("me_nn_curve_finalize");
+  const std::string path = results_subfolder + "accuracy_curve.txt";
+  std::ofstream f(path);
+  if (!f.is_open()) {
+    std::cerr << "ERROR: cannot write " << path << std::endl;
+    return -1;
+  }
+  f << "tau e2g_n_inlier e2g_mean e2g_rmse e2g_fitness e2g_sigma g2e_n_inlier g2e_mean g2e_rmse g2e_fitness g2e_sigma cd f1 iou\n";
+  f << std::fixed << std::setprecision(15);
+  for (const me_curve_row &r : rows) {
+    f << r.tau;
+    for (const me_curve_dir *d : {&r.est_to_gt, &r.gt_to_est})
+      f << " " << d->n_inlier << " " << d->mean << " " << d->rmse << " " << d->fitness << " " << d->sigma;
+    f << " " << r.cd << " " << r.f1 << " " << r.iou << "\n";
+  }
+  std::cout << "INFO: accuracy curve (" << K << " levels up to " << param_.accuracy_curve_max_ << ") saved to " << path << std::endl;
   return 0;
 }
 
@@ -687,6 +741,7 @@ inline int MapEvalB200::performRegistration() {
   if (!gpus_.reduce_nn(e2g, g2e)) return fail("all-reduce of the NN accumulators");
   if (me_nn_finalize(&p, &e2g[0], &g2e[0], n_est_, n_gt_, &nn_) != ME_OK) return fail("me_nn_finalize");
   t_acc = tic.toc() / 1000.0;
+  if (param_.accuracy_curve_steps_ > 0 && accuracyCurve(p, e2g, g2e) != 0) return -1;
   if (param_.save_immediate_result_ && renderDistances(true) != 0) return -1;
   full_chamfer_dist = nn_.full_cd;
   t_fcd = t_acc;

@@ -388,6 +388,35 @@ ME_API int  me_eval_nn(me_ctx *ctx, const me_nn_params *p, me_nn_result *out);  
  * which_query = ME_CLOUD_EST -> est->gt sweep.  Only this rank's query range is filled (others -1 / NaN). */
 ME_API int  me_get_nn(me_ctx *ctx, int which_query, int32_t *nn_index, double *nn_sqdist);
 
+/* ---- accuracy curve: AC / COM / CD / F1 / IoU at any number of thresholds ------------------------------------------------
+ * The five-level statistics of me_eval_nn* at K levels tau[0..K-1] (1 <= K <= ME_CURVE_MAX_LEVELS, finite, >= 0,
+ * non-decreasing; anything else is ME_ERR_INVALID), from the per-query records of the LAST me_eval_nn* call: the same kept
+ * pairs, the same distance d (ME_PAIRING_AS_WRITTEN: from the swapped indices, out-of-range pairs counted), d <= tau_k as
+ * the reference compares.  No new sweep.  The records go stale with any me_set_cloud*, me_transform, me_voxel_downsample,
+ * me_copy_cloud, me_add_*, ICP call or layout change after that call; the curve then fails with ME_ERR_INVALID.
+ * me_nn_curve_accum_device: this rank's SUM-reducible block, on the device, *n = 2 (3 (K + 1) + 1) fp64 values: per direction
+ * (est->gt, then gt->est) the count, sum d and sum d^2 (Eigen's squaredNorm) of the pairs of every bin b = 0..K (bin b: the
+ * first level with d <= tau_b; bin K: above every level), then n_ub.  Directions the last call did not evaluate are zero.
+ * Deterministic: two calls on the same device, world and layout give the same bits.  The caller all-reduces the block in
+ * place (ncclAllReduce / torch.distributed after me_synchronize), copies it to the host and calls me_nn_curve_finalize with
+ * the reduced accumulators of that me_eval_nn* call (host only; the formulas of me_nn_finalize per level, sigma from the
+ * rank moments).  me_nn_curve: both steps, world must be 1. */
+#define ME_CURVE_MAX_LEVELS 1024
+typedef struct {
+  int64_t n_inlier;                 /* pairs with d <= tau                                          */
+  double  mean, rmse, fitness, sigma;
+} me_curve_dir;
+typedef struct {
+  double  tau;
+  me_curve_dir est_to_gt, gt_to_est;
+  double  cd, f1, iou;              /* map_eval.cpp:1245-1253 at this level                          */
+} me_curve_row;
+ME_API int  me_nn_curve_accum_device(me_ctx *ctx, const double *tau, int32_t n_tau, double **device_block, int32_t *n);
+ME_API int  me_nn_curve_finalize(const me_nn_params *p, const me_nn_accum *est_to_gt, const me_nn_accum *gt_to_est,
+                                 const double *host_block, const double *tau, int32_t n_tau, int64_t n_est, int64_t n_gt,
+                                 me_curve_row *rows);   /* host only, no device work */
+ME_API int  me_nn_curve(me_ctx *ctx, const double *tau, int32_t n_tau, me_curve_row *rows);
+
 /* replaces: ComputeMeanMapEntropyUsingNormalTBB / ...UsingNormal (min_neighbors 10, map_eval.cpp:1608-1737, 1538-1606),
  * ComputeMeanMapEntropy (min_neighbors 5, :1438-1535), ComputeEntropy (:1433-1436) and the min/max side effect of
  * ColorPointCloudByMME (:697-701).  entropies_host (nullable) receives N fp64, zeros where invalid. */
