@@ -136,6 +136,25 @@ def curve_block_len(n_tau):
     return 2 * (3 * (int(n_tau) + 1) + 1)
 
 
+# exact distance quantiles (me_nn_quantile*)
+ME_QUANTILE_MAX_PROBS = 64
+ME_DIST_KEPT = 0
+ME_DIST_NN = 1
+# the SUM-reducible block of a selection pass: [direction][slot][digit] counts as fp64, 2 x (2 * 64 + 2) x 256
+ME_QUANTILE_BLOCK = 2 * (2 * ME_QUANTILE_MAX_PROBS + 2) * 256
+
+
+class me_quantile_dir(C.Structure):
+    _fields_ = [("n", C.c_int64), ("min", C.c_double), ("max", C.c_double), ("rank", C.c_int64 * ME_QUANTILE_MAX_PROBS),
+                ("lo", C.c_double * ME_QUANTILE_MAX_PROBS), ("hi", C.c_double * ME_QUANTILE_MAX_PROBS),
+                ("value", C.c_double * ME_QUANTILE_MAX_PROBS)]
+
+
+class me_quantile_result(C.Structure):
+    _fields_ = [("population", C.c_int32), ("n_probs", C.c_int32), ("p", C.c_double * ME_QUANTILE_MAX_PROBS),
+                ("est_to_gt", me_quantile_dir), ("gt_to_est", me_quantile_dir), ("hausdorff", C.c_double)]
+
+
 class me_mme_accum(C.Structure):
     _fields_ = [("n_query", C.c_int64), ("n_valid", C.c_int64), ("sum_entropy", C.c_double),
                 ("min_entropy", C.c_double), ("max_entropy", C.c_double)]

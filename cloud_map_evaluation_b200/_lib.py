@@ -25,6 +25,8 @@ SYMBOLS = (
     "me_copy_cloud", "me_add_gaussian_noise", "me_add_non_uniform_density", "me_add_sparse_outliers", "me_add_local_deformation",
     "me_global_registration", "me_get_features", "me_get_correspondences",
     "me_nn_curve_accum_device", "me_nn_curve_finalize", "me_nn_curve",
+    "me_nn_quantile_begin", "me_nn_quantile_block", "me_nn_quantile_step", "me_nn_quantile_end", "me_nn_quantiles",
+    "me_quantile_finalize",
 )
 
 _lib = None
@@ -116,6 +118,12 @@ def load():
     L.me_nn_curve_finalize.argtypes = [C.POINTER(A.me_nn_params), C.POINTER(A.me_nn_accum), C.POINTER(A.me_nn_accum), dp, dp,
                                        C.c_int32, C.c_int64, C.c_int64, C.POINTER(A.me_curve_row)]
     L.me_nn_curve.argtypes = [ctx, dp, C.c_int32, C.POINTER(A.me_curve_row)]
+    L.me_nn_quantile_begin.argtypes = [ctx, C.c_int32, dp, C.c_int32]
+    L.me_nn_quantile_block.argtypes = [ctx, C.POINTER(dp), C.POINTER(C.c_int32)]
+    L.me_nn_quantile_step.argtypes = [ctx, C.POINTER(C.c_int32)]
+    L.me_nn_quantile_end.argtypes = [ctx, C.POINTER(A.me_quantile_result)]
+    L.me_nn_quantiles.argtypes = [ctx, C.c_int32, dp, C.c_int32, C.POINTER(A.me_quantile_result)]
+    L.me_quantile_finalize.argtypes = [C.c_int64, dp, C.c_int32, dp, dp]
     L.me_kernel_trace.argtypes = [ctx, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.c_int32]
     if L.me_abi_version() != A.ME_ABI_VERSION:
         raise RuntimeError("libmapeval_b200.so ABI version mismatch")

@@ -72,6 +72,38 @@ def curve_finalize(params, e, g, block, tau, n_est, n_gt):
     return _curve_arrays(rows)
 
 
+def _quantile_probs(p):
+    q = np.ascontiguousarray(p, dtype=np.float64).reshape(-1)
+    return q, q.ctypes.data_as(C.POINTER(C.c_double))
+
+
+def quantile_finalize(n, p, lo_hi):
+    """me_quantile_finalize (host only): the quantile values at the probabilities p of a sorted population of n values, from
+    lo_hi = (K, 2) array of (x_k, x_min(k+1, n-1)), k = floor((n - 1) p) — numpy's method="linear" in its operation order"""
+    L = _lib.load()
+    q, qp = _quantile_probs(p)
+    lh = np.ascontiguousarray(lo_hi, dtype=np.float64).reshape(-1)
+    if lh.size != 2 * q.size:
+        raise ValueError("lo_hi holds one (lo, hi) pair per probability")
+    out = np.empty(q.size, np.float64)
+    dp = C.POINTER(C.c_double)
+    rc = L.me_quantile_finalize(int(n), qp, q.size, lh.ctypes.data_as(dp), out.ctypes.data_as(dp))
+    if rc != A.ME_OK:
+        raise MapEvalError(rc, "me_quantile_finalize: n >= 1, 1 <= K <= ME_QUANTILE_MAX_PROBS, every p finite and in [0, 1]")
+    return out
+
+
+def quantile_dict(res):
+    """me_quantile_result -> {'est_to_gt' / 'gt_to_est': {'n', 'min', 'max', 'rank', 'lo', 'hi', 'value'}, 'p', 'hausdorff'}"""
+    K = res.n_probs
+    out = {"p": np.array(res.p[:K]), "hausdorff": float(res.hausdorff)}
+    for name in ("est_to_gt", "gt_to_est"):
+        d = getattr(res, name)
+        out[name] = {"n": int(d.n), "min": float(d.min), "max": float(d.max), "rank": np.array(d.rank[:K], np.int64),
+                     "lo": np.array(d.lo[:K]), "hi": np.array(d.hi[:K]), "value": np.array(d.value[:K])}
+    return out
+
+
 class MapEvalB200:
     """One context = one GPU.  rank/world select this context's contiguous query range (multi-GPU sharding)."""
 
@@ -339,6 +371,41 @@ class MapEvalB200:
         n = C.c_int32(0)
         self._check(self._L.me_nn_curve_accum_device(self._ctx, tp, t.size, C.byref(ptr), C.byref(n)))
         return C.cast(ptr, C.c_void_p).value, n.value
+
+    def distance_quantiles(self, p, population=A.ME_DIST_KEPT):
+        """Exact quantiles at the probabilities p (1..ME_QUANTILE_MAX_PROBS values in [0, 1]) of the distances of the last NN
+        evaluation, per direction, with min, max and the Hausdorff distance (me_nn_quantiles, world 1).  population:
+        ME_DIST_KEPT (the kept pairs' d) or ME_DIST_NN (every query's NN distance; needs want_full_cd).  Returns
+        {'est_to_gt' / 'gt_to_est': {'n', 'min', 'max', 'rank', 'lo', 'hi', 'value'}, 'p', 'hausdorff'}.  Multi-GPU:
+        dist.quantiles_distributed."""
+        q, qp = _quantile_probs(p)
+        out = A.me_quantile_result()
+        self._check(self._L.me_nn_quantiles(self._ctx, int(population), qp, q.size, C.byref(out)))
+        return quantile_dict(out)
+
+    def quantile_begin(self, p, population=A.ME_DIST_KEPT):
+        """me_nn_quantile_begin: checks the arguments and the records, runs the first selection pass"""
+        q, qp = _quantile_probs(p)
+        self._check(self._L.me_nn_quantile_begin(self._ctx, int(population), qp, q.size))
+
+    def quantile_block(self):
+        """(device pointer, n) of the running pass's SUM-reducible block (all-reduce it in place after synchronize())"""
+        ptr = C.POINTER(C.c_double)()
+        n = C.c_int32(0)
+        self._check(self._L.me_nn_quantile_block(self._ctx, C.byref(ptr), C.byref(n)))
+        return C.cast(ptr, C.c_void_p).value, n.value
+
+    def quantile_step(self):
+        """reads the reduced block and runs the next pass; True after the last one"""
+        done = C.c_int32(0)
+        self._check(self._L.me_nn_quantile_step(self._ctx, C.byref(done)))
+        return bool(done.value)
+
+    def quantile_end(self):
+        """the result of the selection, as distance_quantiles"""
+        out = A.me_quantile_result()
+        self._check(self._L.me_nn_quantile_end(self._ctx, C.byref(out)))
+        return quantile_dict(out)
 
     def get_nn(self, which_query):
         n = self.n[which_query]

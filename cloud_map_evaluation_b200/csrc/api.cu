@@ -230,6 +230,7 @@ void me_destroy(me_ctx *ctx) {
   cudaSetDevice(ctx->device);
   if (ctx->stream) cudaStreamSynchronize(ctx->stream);
   icp_close(ctx, false);
+  nn_quantile_free(ctx);
   if (ctx->copy_stream) { cudaStreamSynchronize(ctx->copy_stream); cudaStreamDestroy(ctx->copy_stream); }
   if (ctx->compute_mark) cudaEventDestroy(ctx->compute_mark);
   for (Cloud &c : ctx->cloud) free_cloud(c);
@@ -857,6 +858,62 @@ int me_nn_curve(me_ctx *ctx, const double *tau, int32_t n_tau, me_curve_row *row
   if (me_nn_curve_finalize(&ctx->curve_p, &acc[0], &acc[1], h.data(), tau, n_tau, ctx->cloud[0].n, ctx->cloud[1].n, rows) != ME_OK)
     return fail(ctx, ME_ERR_INVALID, "me_nn_curve_finalize: the curve block does not match the accumulators");
   return ME_OK;
+}
+
+// 1 <= K <= ME_QUANTILE_MAX_PROBS, every probability finite and in [0, 1]
+static bool quantile_probs_ok(const double *p, int32_t K) {
+  if (!p || K < 1 || K > ME_QUANTILE_MAX_PROBS) return false;
+  for (int k = 0; k < K; ++k)
+    if (!(std::isfinite(p[k]) && p[k] >= 0.0 && p[k] <= 1.0)) return false;
+  return true;
+}
+
+int me_quantile_finalize(int64_t n, const double *p, int32_t n_probs, const double *lo_hi, double *values) {
+  if (n < 1 || !lo_hi || !values || !quantile_probs_ok(p, n_probs)) return ME_ERR_INVALID;
+  for (int k = 0; k < n_probs; ++k) {
+    long long kk;
+    double g;
+    me::quantile_rank(n, p[k], &kk, &g);
+    values[k] = me::quantile_lerp(lo_hi[2 * k], lo_hi[2 * k + 1], g);
+  }
+  return ME_OK;
+}
+
+int me_nn_quantile_begin(me_ctx *ctx, int32_t population, const double *p, int32_t n_probs) {
+  ME_ENTER(ctx);
+  if (population != ME_DIST_KEPT && population != ME_DIST_NN) return fail(ctx, ME_ERR_INVALID, "population must be ME_DIST_KEPT or ME_DIST_NN");
+  if (!quantile_probs_ok(p, n_probs))
+    return fail(ctx, ME_ERR_INVALID, "me_nn_quantile*: 1 <= n_probs <= ME_QUANTILE_MAX_PROBS probabilities, each finite and in [0, 1]");
+  return nn_quantile_begin(ctx, population, p, n_probs);
+}
+
+int me_nn_quantile_block(me_ctx *ctx, double **device_block, int32_t *n) {
+  ME_ENTER(ctx);
+  if (!device_block || !n) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return nn_quantile_block(ctx, device_block, n);
+}
+
+int me_nn_quantile_step(me_ctx *ctx, int32_t *done) {
+  ME_ENTER(ctx);
+  if (!done) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return nn_quantile_step(ctx, done);
+}
+
+int me_nn_quantile_end(me_ctx *ctx, me_quantile_result *out) {
+  ME_ENTER(ctx);
+  if (!out) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return nn_quantile_end(ctx, out);
+}
+
+int me_nn_quantiles(me_ctx *ctx, int32_t population, const double *p, int32_t n_probs, me_quantile_result *out) {
+  ME_ENTER(ctx);
+  if (!out) return fail(ctx, ME_ERR_INVALID, "null argument");
+  if (ctx->world != 1)
+    return fail(ctx, ME_ERR_INVALID, "me_nn_quantiles needs world == 1; use me_nn_quantile_begin / _block + all-reduce / _step / _end");
+  ME_TRY(me_nn_quantile_begin(ctx, population, p, n_probs));
+  int32_t done = 0;
+  while (!done) ME_TRY(me_nn_quantile_step(ctx, &done));
+  return me_nn_quantile_end(ctx, out);
 }
 
 int me_eval_nn(me_ctx *ctx, const me_nn_params *p, me_nn_result *out) {

@@ -3,7 +3,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
+#include <cmath>
 #include <string>
+#include <vector>
 #include "../../include/mapeval_b200.h"
 
 namespace me {
@@ -162,6 +164,48 @@ struct IcpRun {
   int it = 0, converged = 0;
 };
 
+// exact distance quantiles (me_nn_quantile_begin .. me_nn_quantile_end, nn.cu): radix selection over the NN records, the
+// same loop on every rank.  Slot s of a direction is one distinct prefix (the key bits the passes so far fixed) that some
+// target rank still lies under.
+static constexpr int kQuantSlots = 2 * ME_QUANTILE_MAX_PROBS + 2;   // ranks k and k + 1 per probability, then 0 and n - 1
+static constexpr int kQuantBins = 256;                               // 8-bit digits
+static constexpr int kQuantPasses = 8;                               // 64-bit keys
+static constexpr int kQuantBlock = 2 * kQuantSlots * kQuantBins;     // fp64 counts per pass: [direction][slot][digit]
+struct QuantRun {
+  bool open = false, done = false;
+  unsigned long long gen = 0;          // cloud_gen at me_nn_quantile_begin
+  int population = 0, K = 0, dirs = 0;
+  double p[ME_QUANTILE_MAX_PROBS];
+  int pass = 0;                        // passes whose histogram the block holds / held (1 after begin)
+  long long n[2] = {0, 0};             // population sizes, from the reduced block of pass 0
+  int n_targets[2] = {0, 0};
+  long long rank[2][kQuantSlots];      // target ranks in the sorted population
+  long long resid[2][kQuantSlots];     // rank of the target among the keys under its prefix
+  unsigned long long key[2][kQuantSlots];   // the prefix of the target: the digits fixed so far, lower bits zero
+  int n_slots[2] = {0, 0};
+  unsigned long long slot_pfx[2][kQuantSlots];   // distinct prefixes of the running pass, ascending
+  long long kb[2] = {0, 0}, ke[2] = {0, 0};      // the record range the keys cover
+  unsigned long long *d_keys[2] = {nullptr, nullptr};
+  long long cap_keys[2] = {0, 0};
+  unsigned long long *d_hist = nullptr;          // integer histogram of the running pass, kQuantBlock counts
+  double *d_blk = nullptr;                       // the same as fp64: the SUM-reducible block
+  unsigned long long *d_pfx = nullptr;           // slot_pfx on the device
+  std::vector<double> h_blk;
+};
+
+// numpy's method="linear" position of probability p among n sorted values: h = (n - 1) p, k = floor(h), g = h - k
+inline void quantile_rank(long long n, double p, long long *k, double *g) {
+  const double h = (double)(n - 1) * p;
+  const double f = std::floor(h);
+  *k = (long long)f;
+  *g = h - f;
+}
+// numpy's _lerp in its operation order: lo + (hi - lo) g below g = 0.5, hi - (hi - lo) (1 - g) from there
+inline double quantile_lerp(double lo, double hi, double g) {
+  const double diff = hi - lo;
+  return g >= 0.5 ? hi - diff * (1.0 - g) : lo + diff * g;
+}
+
 }  // namespace me
 
 struct me_ctx {
@@ -232,6 +276,7 @@ struct me_ctx {
   me_nn_accum curve_acc[2];
   double *d_curve = nullptr;           // the curve block (both directions), then the levels
   long long cap_curve = 0;
+  me::QuantRun quant;                  // distance quantiles (me_nn_quantile*), from the same records
   std::string err;
 };
 
@@ -334,6 +379,12 @@ int run_nn(me_ctx *ctx, const me_nn_params *p, me_nn_accum *e2g, me_nn_accum *g2
 int unsort_nn(me_ctx *ctx, int which_query, int32_t *h_idx, double *h_d2);
 // the curve block of the last me_eval_nn* at the K levels tau (host memory, checked by the caller) — me_nn_curve_accum_device
 int nn_curve(me_ctx *ctx, const double *tau, int K, double **device_block, int32_t *n);
+// exact distance quantiles of the last me_eval_nn*'s records (arguments checked by the caller) — me_nn_quantile_*
+int nn_quantile_begin(me_ctx *ctx, int population, const double *p, int K);
+int nn_quantile_block(me_ctx *ctx, double **device_block, int32_t *n);
+int nn_quantile_step(me_ctx *ctx, int32_t *done);
+int nn_quantile_end(me_ctx *ctx, me_quantile_result *out);
+void nn_quantile_free(me_ctx *ctx);
 int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors, me_mme_accum *out, bool to_block = false);
 
 // layout of me_ctx::d_block (fp64): the SUM-reducible part first, then the MAX-reducible part.  Counts ride as fp64 (exact

@@ -916,6 +916,21 @@ struct CurveSrc {           // the per-query records of one direction
   long long n_gt, n_est;
 };
 
+// the kept-pair rule of the five-level pass on record i of S (me_nn_curve* and me_nn_quantile* share it): true with sq = the
+// pair's squared norm, whose pair_dist is d; an out-of-range ME_PAIRING_AS_WRITTEN pair adds one to ub and is not kept
+__device__ __forceinline__ bool kept_record(const CurveSrc &S, const NNConst &C, long long i, double &sq, unsigned int &ub) {
+  if (S.as_written) {
+    const int r = as_written_pair(S.Qgt, i, S.nn_idx, S.nn_d2, S.gt_xyz, S.n_gt, S.est_xyz, S.n_est, C, sq);
+    ub += r == kAwOutOfRange;
+    return r == kAwPair;
+  }
+  if (__ldg(S.nn_idx + i) >= 0 && keep_pair(__ldg(S.nn_d2 + i), C)) {
+    sq = __ldg(S.nn_sq + i);
+    return true;
+  }
+  return false;
+}
+
 // first k in [0, K) with d <= tau[k], K if none (tau non-decreasing)
 __device__ __forceinline__ int curve_bin(const double *tau, int K, double d) {
   int lo = 0, hi = K;
@@ -946,18 +961,7 @@ nn_curve_kernel(CurveSrc S, NNConst C, const double *__restrict__ tau, int K, lo
     const long long i = base + threadIdx.x;
     int bin = K + 1;                 // no kept pair: sorts last, never folded
     double d = 0.0, sq = 0.0;
-    if (i < b1) {
-      bool kept = false;
-      if (S.as_written) {
-        const int r = as_written_pair(S.Qgt, i, S.nn_idx, S.nn_d2, S.gt_xyz, S.n_gt, S.est_xyz, S.n_est, C, sq);
-        ub += r == kAwOutOfRange;
-        kept = r == kAwPair;
-      } else if (__ldg(S.nn_idx + i) >= 0 && keep_pair(__ldg(S.nn_d2 + i), C)) {
-        sq = __ldg(S.nn_sq + i);
-        kept = true;
-      }
-      if (kept) { d = pair_dist(sq); bin = curve_bin(s_tau, K, d); }
-    }
+    if (i < b1 && kept_record(S, C, i, sq, ub)) { d = pair_dist(sq); bin = curve_bin(s_tau, K, d); }
     // sort the warp's (bin, lane) keys ascending, then fetch the values in that order
     unsigned int key = ((unsigned int)bin << 5) | (unsigned int)lane;
 #pragma unroll
@@ -1009,6 +1013,105 @@ __global__ void nn_curve_merge_kernel(const double *__restrict__ part, int n_blo
   double s = 0.0;
   for (int b = 0; b < n_blocks; ++b) s += part[(long long)b * stride + t];
   blk[t] = s;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Exact distance quantiles (me_nn_quantile_*): radix selection over the records.  Pass 0 turns every record of a
+// direction into a 64-bit key — the bit pattern of its d, which for a finite d >= 0 sorts as an unsigned integer, or
+// kQuantOut outside the population — and histograms the top 8-bit digit.  Pass j histograms digit j of the keys under
+// each slot's prefix (the top 8j bits some target rank still lies under).  Prefixes of one length are disjoint, so a key
+// falls under at most one slot, found by binary search over the ascending prefixes.  Counts only: per block a shared
+// integer histogram (warp-aggregated), merged into the global one with integer atomics — the result does not depend on
+// the order of the additions.
+// ---------------------------------------------------------------------------------------------------------------
+static constexpr int kQuantThreads = 512;
+static constexpr unsigned long long kQuantOut = ~0ull;     // not in the population (no finite d >= 0 has the sign bit)
+
+// d of record i of the population, false when the record is not in it
+__device__ __forceinline__ bool quant_record(const CurveSrc &S, const NNConst &C, int nn_pop, long long i, double &d) {
+  if (nn_pop) {            // the terms of nn_stats_kernel's full-CD sum
+    if (__ldg(S.nn_idx + i) < 0) return false;
+    d = __dsqrt_rn(__ldg(S.nn_d2 + i));
+    return true;
+  }
+  double sq;
+  unsigned int ub = 0;
+  if (!kept_record(S, C, i, sq, ub)) return false;
+  d = pair_dist(sq);
+  return true;
+}
+
+// one count into s_hist[bin] (bin < 0: none), the lanes of a warp with the same bin added by one atomic; the whole warp calls
+__device__ __forceinline__ void quant_count(unsigned int *s_hist, int bin) {
+  const unsigned int peers = __match_any_sync(0xffffffffu, bin);
+  if (bin >= 0 && (threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(s_hist + bin, (unsigned int)__popc(peers));
+}
+
+// the block's histogram of nbins bins, added into hist
+__device__ __forceinline__ void quant_flush(const unsigned int *s_hist, int nbins, unsigned long long *__restrict__ hist) {
+  __syncthreads();
+  for (int t = threadIdx.x; t < nbins; t += blockDim.x)
+    if (s_hist[t]) atomicAdd(hist + t, (unsigned long long)s_hist[t]);
+}
+
+// pass 0: keys[i - S.b] for every record of [S.b, S.e), and the histogram of the top digit into hist[0 .. 255]
+__global__ void __launch_bounds__(kQuantThreads)
+nn_quantile_keys_kernel(CurveSrc S, NNConst C, int nn_pop, unsigned long long *__restrict__ keys, unsigned long long *__restrict__ hist) {
+  __shared__ unsigned int s_hist[kQuantBins];
+  for (int t = threadIdx.x; t < kQuantBins; t += kQuantThreads) s_hist[t] = 0;
+  __syncthreads();
+  const long long stride = (long long)gridDim.x * kQuantThreads;
+  for (long long base = S.b + (long long)blockIdx.x * kQuantThreads; base < S.e; base += stride) {   // warp-uniform bound
+    const long long i = base + threadIdx.x;
+    int bin = -1;
+    if (i < S.e) {
+      double d;
+      unsigned long long key = kQuantOut;
+      if (quant_record(S, C, nn_pop, i, d)) {
+        key = (unsigned long long)__double_as_longlong(d == 0.0 ? 0.0 : d);     // -0 sorts with +0
+        bin = (int)(key >> 56);
+      }
+      keys[i - S.b] = key;
+    }
+    quant_count(s_hist, bin);
+  }
+  quant_flush(s_hist, kQuantBins, hist);
+}
+
+// pass j >= 1 (shift = 56 - 8j): per key under the prefix of slot s (pfx[s] = its top 8j bits, ascending), one count into
+// hist[s * 256 + digit j]
+__global__ void __launch_bounds__(kQuantThreads)
+nn_quantile_hist_kernel(const unsigned long long *__restrict__ keys, long long n, int shift, const unsigned long long *__restrict__ pfx,
+                        int n_slots, unsigned long long *__restrict__ hist) {
+  extern __shared__ unsigned int s_hist_dyn[];        // n_slots * 256
+  __shared__ unsigned long long s_pfx[kQuantSlots];
+  for (int t = threadIdx.x; t < n_slots * kQuantBins; t += kQuantThreads) s_hist_dyn[t] = 0;
+  for (int t = threadIdx.x; t < n_slots; t += kQuantThreads) s_pfx[t] = pfx[t];
+  __syncthreads();
+  const long long stride = (long long)gridDim.x * kQuantThreads;
+  for (long long base = (long long)blockIdx.x * kQuantThreads; base < n; base += stride) {
+    const long long i = base + threadIdx.x;
+    int bin = -1;
+    if (i < n) {
+      const unsigned long long key = __ldg(keys + i);
+      if (key != kQuantOut) {
+        const unsigned long long top = key >> (shift + 8);
+        int lo = 0, hi = n_slots;          // first slot with prefix >= top
+        while (lo < hi) {
+          const int mid = (lo + hi) >> 1;
+          if (s_pfx[mid] < top) lo = mid + 1; else hi = mid;
+        }
+        if (lo < n_slots && s_pfx[lo] == top) bin = lo * kQuantBins + (int)((key >> shift) & 0xffu);
+      }
+    }
+    quant_count(s_hist_dyn, bin);
+  }
+  quant_flush(s_hist_dyn, n_slots * kQuantBins, hist);
+}
+
+__global__ void quant_to_block_kernel(const unsigned long long *__restrict__ hist, int n, double *__restrict__ blk) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < n) blk[t] = (double)hist[t];
 }
 
 __global__ void fill_i32_kernel(int32_t *p, long long n, int32_t v) {
@@ -1264,14 +1367,36 @@ int run_nn(me_ctx *ctx, const me_nn_params *p, me_nn_accum *e2g, me_nn_accum *g2
   return ME_OK;
 }
 
-int nn_curve(me_ctx *ctx, const double *tau, int K, double **device_block, int32_t *n) {
+// the records of the last me_eval_nn* still describe the clouds: no call has changed them since, and every direction that
+// call evaluated holds its records.  `who` names the caller in the message.
+static int nn_records_fresh(me_ctx *ctx, const char *who) {
   const me_nn_params *p = &ctx->curve_p;
   const int dirs = p->directions ? p->directions : 3;
   bool fresh = ctx->curve_valid && ctx->curve_gen == ctx->cloud_gen;
   for (int q = 0; q < 2; ++q) fresh = fresh && (!(dirs & (1 << q)) || ctx->cloud[q].nn_valid);
   if (!fresh)
-    return fail(ctx, ME_ERR_INVALID, "me_nn_curve*: no current NN records; run me_eval_nn* after the last change of the clouds "
+    return fail(ctx, ME_ERR_INVALID, std::string(who) + ": no current NN records; run me_eval_nn* after the last change of the clouds "
                                      "(me_set_cloud*, me_transform, me_voxel_downsample, me_copy_cloud, me_add_*, ICP, a new layout)");
+  return ME_OK;
+}
+
+// the records of direction q (query cloud q) over the ranges nn_stats_kernel / pair_as_written_kernel walk
+static CurveSrc record_src(const me_ctx *ctx, int q) {
+  const me_nn_params *p = &ctx->curve_p;
+  const Cloud &Qc = ctx->cloud[q], &Rc = ctx->cloud[1 - q];
+  CurveSrc S;
+  S.as_written = q == ME_CLOUD_GT && p->pairing == ME_PAIRING_AS_WRITTEN;
+  S.b = S.as_written ? 0 : Qc.nn_b;
+  S.e = S.as_written ? Qc.ns : Qc.nn_e;
+  S.nn_idx = Qc.d_nn_idx; S.nn_d2 = Qc.d_nn_d2; S.nn_sq = Qc.d_nn_sq;
+  S.Qgt = Qc.d_sorted; S.gt_xyz = Qc.d_xyz; S.n_gt = Qc.n; S.est_xyz = Rc.d_xyz; S.n_est = Rc.n;
+  return S;
+}
+
+int nn_curve(me_ctx *ctx, const double *tau, int K, double **device_block, int32_t *n) {
+  const me_nn_params *p = &ctx->curve_p;
+  const int dirs = p->directions ? p->directions : 3;
+  ME_TRY(nn_records_fresh(ctx, "me_nn_curve*"));
   const int stride = 3 * (K + 1) + 1;
   ME_TRY(ensure(ctx, (void **)&ctx->d_curve, &ctx->cap_curve, 2 * stride + K, sizeof(double)));
   double *blk = ctx->d_curve, *d_tau = ctx->d_curve + 2 * stride;
@@ -1282,15 +1407,9 @@ int nn_curve(me_ctx *ctx, const double *tau, int K, double **device_block, int32
   const size_t smem = (size_t)(K + 3 * (K + 1)) * sizeof(double);
   for (int q = 0; q < 2; ++q) {
     if (!(dirs & (1 << q))) continue;
-    const Cloud &Qc = ctx->cloud[q], &Rc = ctx->cloud[1 - q];
     NNConst C{};
     set_cutoff(C, p);
-    CurveSrc S;
-    S.as_written = q == ME_CLOUD_GT && p->pairing == ME_PAIRING_AS_WRITTEN;
-    S.b = S.as_written ? 0 : Qc.nn_b;       // the ranges nn_stats_kernel / pair_as_written_kernel walk
-    S.e = S.as_written ? Qc.ns : Qc.nn_e;
-    S.nn_idx = Qc.d_nn_idx; S.nn_d2 = Qc.d_nn_d2; S.nn_sq = Qc.d_nn_sq;
-    S.Qgt = Qc.d_sorted; S.gt_xyz = Qc.d_xyz; S.n_gt = Qc.n; S.est_xyz = Rc.d_xyz; S.n_est = Rc.n;
+    const CurveSrc S = record_src(ctx, q);
     if (S.e <= S.b) continue;
     const int n_blocks = (int)std::min<long long>((S.e - S.b + kCurveThreads - 1) / kCurveThreads, max_blocks);
     const long long per_block = (S.e - S.b + n_blocks - 1) / n_blocks;
@@ -1302,6 +1421,217 @@ int nn_curve(me_ctx *ctx, const double *tau, int K, double **device_block, int32
   }
   *device_block = blk;
   *n = 2 * stride;
+  return ME_OK;
+}
+
+// ---- exact distance quantiles: the loop state is QuantRun (common.cuh), the same on every rank -------------------------------
+void nn_quantile_free(me_ctx *ctx) {
+  QuantRun &R = ctx->quant;
+  for (int q = 0; q < 2; ++q)
+    if (R.d_keys[q]) { cudaFree(R.d_keys[q]); R.d_keys[q] = nullptr; R.cap_keys[q] = 0; }
+  if (R.d_hist) { cudaFree(R.d_hist); R.d_hist = nullptr; R.d_blk = nullptr; R.d_pfx = nullptr; }
+  R.open = false;
+}
+
+// launch pass R.pass of every direction: pass 0 writes the keys, the later ones read them under the slots' prefixes
+static int quant_launch(me_ctx *ctx) {
+  QuantRun &R = ctx->quant;
+  ME_CUDA(ctx, cudaMemsetAsync(R.d_hist, 0, (size_t)kQuantBlock * sizeof(unsigned long long), ctx->stream));
+  if (R.pass > 0)
+    ME_CUDA(ctx, cudaMemcpyAsync(R.d_pfx, R.slot_pfx, sizeof(R.slot_pfx), cudaMemcpyHostToDevice, ctx->stream));
+  for (int q = 0; q < 2; ++q) {
+    const long long n = R.ke[q] - R.kb[q];
+    if (n <= 0 || R.n_slots[q] == 0) continue;
+    unsigned long long *hist = R.d_hist + (size_t)q * kQuantSlots * kQuantBins;
+    if (R.pass == 0) {
+      NNConst C{};
+      set_cutoff(C, &ctx->curve_p);
+      CurveSrc S = record_src(ctx, q);
+      S.b = R.kb[q]; S.e = R.ke[q];
+      const int grid = (int)std::min<long long>((n + kQuantThreads - 1) / kQuantThreads, (long long)ctx->sm_count * 4);
+      nn_quantile_keys_kernel<<<grid, kQuantThreads, 0, ctx->stream>>>(S, C, R.population == ME_DIST_NN, R.d_keys[q], hist);
+    } else {
+      const size_t smem = (size_t)R.n_slots[q] * kQuantBins * sizeof(unsigned int);
+      ME_CUDA(ctx, cudaFuncSetAttribute(nn_quantile_hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)(kQuantSlots * kQuantBins * sizeof(unsigned int))));
+      int per_sm = 0;
+      ME_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nn_quantile_hist_kernel, kQuantThreads, smem));
+      const int grid = (int)std::min<long long>((n + kQuantThreads - 1) / kQuantThreads, (long long)ctx->sm_count * std::max(per_sm, 1));
+      nn_quantile_hist_kernel<<<grid, kQuantThreads, smem, ctx->stream>>>(R.d_keys[q], n, 56 - 8 * R.pass, R.d_pfx + q * kQuantSlots,
+                                                                         R.n_slots[q], hist);
+    }
+    ME_LAUNCH_CHECK(ctx);
+  }
+  quant_to_block_kernel<<<(kQuantBlock + 255) / 256, 256, 0, ctx->stream>>>(R.d_hist, kQuantBlock, R.d_blk);
+  ME_LAUNCH_CHECK(ctx);
+  return ME_OK;
+}
+
+int nn_quantile_begin(me_ctx *ctx, int population, const double *p, int K) {
+  QuantRun &R = ctx->quant;
+  R.open = false;
+  ME_TRY(nn_records_fresh(ctx, "me_nn_quantile*"));
+  if (population == ME_DIST_NN && !ctx->curve_p.want_full_cd)
+    return fail(ctx, ME_ERR_INVALID, "me_nn_quantile*: ME_DIST_NN needs every query's nearest neighbour; the last me_eval_nn* "
+                                     "ran with want_full_cd = 0, so queries beyond the cut-off were never resolved");
+  R.population = population;
+  R.K = K;
+  for (int k = 0; k < K; ++k) R.p[k] = p[k];
+  R.dirs = ctx->curve_p.directions ? ctx->curve_p.directions : 3;
+  R.gen = ctx->cloud_gen;
+  R.done = false;
+  R.pass = 0;
+  if (!R.d_hist) {      // the integer histogram, its fp64 block and the slot prefixes in one allocation
+    const size_t bytes = (size_t)kQuantBlock * (sizeof(unsigned long long) + sizeof(double)) + sizeof(R.slot_pfx);
+    ME_CUDA(ctx, cudaMalloc((void **)&R.d_hist, bytes));
+    R.d_blk = (double *)(R.d_hist + kQuantBlock);
+    R.d_pfx = (unsigned long long *)(R.d_blk + kQuantBlock);
+  }
+  for (int q = 0; q < 2; ++q) {
+    R.n[q] = 0;
+    R.n_targets[q] = 0;
+    R.kb[q] = R.ke[q] = 0;
+    R.n_slots[q] = 0;
+    if (!(R.dirs & (1 << q))) continue;
+    const CurveSrc S = record_src(ctx, q);
+    const Cloud &Qc = ctx->cloud[q];
+    R.kb[q] = population == ME_DIST_NN ? Qc.nn_b : S.b;      // ME_DIST_NN: the range of the full-CD sum
+    R.ke[q] = std::max(R.kb[q], population == ME_DIST_NN ? Qc.nn_e : S.e);
+    ME_TRY(ensure(ctx, (void **)&R.d_keys[q], &R.cap_keys[q], R.ke[q] - R.kb[q], sizeof(unsigned long long)));
+    R.n_slots[q] = 1;      // pass 0: the empty prefix
+    R.slot_pfx[q][0] = 0;
+  }
+  ME_TRY(quant_launch(ctx));
+  R.open = true;
+  return ME_OK;
+}
+
+static int quant_ready(me_ctx *ctx, const char *who) {
+  QuantRun &R = ctx->quant;
+  if (!R.open) return fail(ctx, ME_ERR_INVALID, std::string(who) + " without an open selection (me_nn_quantile_begin first)");
+  if (R.gen != ctx->cloud_gen) {
+    R.open = false;
+    return fail(ctx, ME_ERR_INVALID, std::string(who) + ": the clouds changed after me_nn_quantile_begin; the selection is void "
+                                     "(run me_eval_nn* and me_nn_quantile_begin again)");
+  }
+  return ME_OK;
+}
+
+int nn_quantile_block(me_ctx *ctx, double **device_block, int32_t *n) {
+  ME_TRY(quant_ready(ctx, "me_nn_quantile_block"));
+  *device_block = ctx->quant.d_blk;
+  *n = kQuantBlock;
+  return ME_OK;
+}
+
+int nn_quantile_step(me_ctx *ctx, int32_t *done) {
+  ME_TRY(quant_ready(ctx, "me_nn_quantile_step"));
+  QuantRun &R = ctx->quant;
+  if (R.done) { *done = 1; return ME_OK; }
+  // the reduced block of pass R.pass: only the rows of the slots in use are read
+  R.h_blk.resize(kQuantBlock);
+  for (int q = 0; q < 2; ++q)
+    if (R.n_slots[q])
+      ME_CUDA(ctx, cudaMemcpyAsync(R.h_blk.data() + (size_t)q * kQuantSlots * kQuantBins, R.d_blk + (size_t)q * kQuantSlots * kQuantBins,
+                                   (size_t)R.n_slots[q] * kQuantBins * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  const int shift = 56 - 8 * R.pass;            // digit R.pass of a key
+  for (int q = 0; q < 2; ++q) {
+    if (!R.n_slots[q]) continue;
+    const double *rows = R.h_blk.data() + (size_t)q * kQuantSlots * kQuantBins;
+    if (R.pass == 0) {      // the population size, then the target ranks: k and k + 1 per probability, 0 and n - 1
+      double n = 0;
+      for (int b = 0; b < kQuantBins; ++b) n += rows[b];
+      R.n[q] = (long long)n;
+      if (R.n[q] > 0) {
+        int t = 0;
+        for (int k = 0; k < R.K; ++k) {
+          long long kk;
+          double g;
+          quantile_rank(R.n[q], R.p[k], &kk, &g);
+          R.rank[q][t++] = kk;
+          R.rank[q][t++] = std::min(kk + 1, R.n[q] - 1);
+        }
+        R.rank[q][t++] = 0;
+        R.rank[q][t++] = R.n[q] - 1;
+        R.n_targets[q] = t;
+        for (int i = 0; i < t; ++i) { R.resid[q][i] = R.rank[q][i]; R.key[q][i] = 0; }
+      }
+    }
+    for (int i = 0; i < R.n_targets[q]; ++i) {      // the digit of each target and its rank below that digit
+      const unsigned long long top = R.pass == 0 ? 0 : R.key[q][i] >> (shift + 8);
+      const int s = (int)(std::lower_bound(R.slot_pfx[q], R.slot_pfx[q] + R.n_slots[q], top) - R.slot_pfx[q]);
+      const double *row = rows + (size_t)s * kQuantBins;
+      long long below = 0;
+      int d = 0;
+      for (; d < kQuantBins; ++d) {
+        const long long c = (long long)row[d];
+        if (R.resid[q][i] < below + c) break;
+        below += c;
+      }
+      if (s >= R.n_slots[q] || d == kQuantBins) {
+        R.open = false;
+        return fail(ctx, ME_ERR_INVALID, "me_nn_quantile_step: the block does not hold a rank the selection needs (a block not "
+                                         "SUM-reduced over all ranks, or of another selection)");
+      }
+      R.resid[q][i] -= below;
+      R.key[q][i] |= (unsigned long long)d << shift;
+    }
+  }
+  if (R.pass == kQuantPasses - 1) {
+    R.done = true;
+    *done = 1;
+    return ME_OK;
+  }
+  ++R.pass;
+  for (int q = 0; q < 2; ++q) {      // the distinct prefixes of the next pass, ascending
+    if (!R.n_slots[q]) continue;
+    unsigned long long *s = R.slot_pfx[q];
+    for (int i = 0; i < R.n_targets[q]; ++i) s[i] = R.key[q][i] >> (64 - 8 * R.pass);
+    std::sort(s, s + R.n_targets[q]);
+    R.n_slots[q] = (int)(std::unique(s, s + R.n_targets[q]) - s);
+  }
+  ME_TRY(quant_launch(ctx));
+  *done = 0;
+  return ME_OK;
+}
+
+int nn_quantile_end(me_ctx *ctx, me_quantile_result *out) {
+  ME_TRY(quant_ready(ctx, "me_nn_quantile_end"));
+  QuantRun &R = ctx->quant;
+  if (!R.done) return fail(ctx, ME_ERR_INVALID, "me_nn_quantile_end before the last me_nn_quantile_step (*done = 1)");
+  R.open = false;
+  std::memset(out, 0, sizeof(*out));
+  out->population = R.population;
+  out->n_probs = R.K;
+  for (int k = 0; k < R.K; ++k) out->p[k] = R.p[k];
+  for (int q = 0; q < 2; ++q) {
+    me_quantile_dir &D = q == 0 ? out->est_to_gt : out->gt_to_est;
+    D.n = R.n[q];
+    auto x = [&](long long r) {      // the order statistic of rank r, one of the targets
+      for (int i = 0; i < R.n_targets[q]; ++i)
+        if (R.rank[q][i] == r) {
+          double v;
+          std::memcpy(&v, &R.key[q][i], sizeof(v));
+          return v;
+        }
+      return (double)NAN;
+    };
+    D.min = D.n > 0 ? x(0) : NAN;
+    D.max = D.n > 0 ? x(D.n - 1) : NAN;
+    for (int k = 0; k < R.K; ++k) {
+      if (D.n == 0) { D.lo[k] = D.hi[k] = D.value[k] = NAN; continue; }
+      long long kk;
+      double g;
+      quantile_rank(D.n, R.p[k], &kk, &g);
+      D.rank[k] = kk;
+      D.lo[k] = x(kk);
+      D.hi[k] = x(std::min<long long>(kk + 1, D.n - 1));
+      D.value[k] = quantile_lerp(D.lo[k], D.hi[k], g);
+    }
+  }
+  const bool both = R.population == ME_DIST_NN && R.dirs == 3 && out->est_to_gt.n > 0 && out->gt_to_est.n > 0;
+  out->hausdorff = both ? std::max(out->est_to_gt.max, out->gt_to_est.max) : NAN;
   return ME_OK;
 }
 

@@ -113,6 +113,25 @@ def allreduce_curve(ctx, tau, device, group=None):
     return t.cpu().numpy().copy()
 
 
+def quantiles_distributed(ctx, device, p, population=A.ME_DIST_KEPT, group=None):
+    """Exact distance quantiles of the last NN evaluation over every rank of the job (MapEvalB200.distance_quantiles for
+    world > 1): the selection loop with ONE in-place SUM all-reduce of the pass's integer counts (as fp64, exact) per pass.
+    Every rank reads the same reduced counts, so every rank returns the same result."""
+    import torch
+    import torch.distributed as dist
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    ctx.quantile_begin(p, population)
+    done = False
+    while not done:
+        if world > 1:
+            ptr, n = ctx.quantile_block()
+            ctx.synchronize()
+            dist.all_reduce(torch.as_tensor(_DeviceBlock(ptr, n), device=device), group=group)
+            torch.cuda.current_stream(device).synchronize()
+        done = ctx.quantile_step()
+    return ctx.quantile_end()
+
+
 def icp_distributed(ctx, device, max_correspondence_distance, T_init=None, max_iteration=30, relative_fitness=1e-6,
                     relative_rmse=1e-6, method=A.ME_ICP_GENERALIZED, group=None):
     """performICPRegistration on every rank of the job (map_eval.cpp:1366-1394): the clouds are replicated, every rank

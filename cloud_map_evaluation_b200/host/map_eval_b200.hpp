@@ -91,6 +91,9 @@ struct Param {   // map_eval.h:60-116
   // accuracy_curve.txt (me_nn_curve*: no new sweep); 0 = off.  accuracy_curve_max defaults to the largest accuracy_level
   int accuracy_curve_steps_ = 0;
   double accuracy_curve_max_ = 0.0;
+  // exact distance quantiles at these probabilities and the Hausdorff distance, written to distance_quantiles.txt
+  // (me_nn_quantile*: no new sweep); absent or empty = off
+  std::vector<double> distance_quantiles_;
 };
 
 // map_eval_main.cpp:120-208
@@ -153,6 +156,9 @@ inline Param loadParametersFromYAML(const std::string &yaml_file_path) {
     if (config["accuracy_curve_steps"]) param.accuracy_curve_steps_ = config["accuracy_curve_steps"].as<int>();
     param.accuracy_curve_max_ = config["accuracy_curve_max"] ? config["accuracy_curve_max"].as<double>()
                                                              : *std::max_element(param.trunc_dist_, param.trunc_dist_ + 5);
+    if (config["distance_quantiles"])
+      for (size_t i = 0; i < config["distance_quantiles"].size(); ++i)
+        param.distance_quantiles_.push_back(config["distance_quantiles"][i].as<double>());
     return param;
   } catch (const std::exception &e) {
     std::cerr << "Error loading parameters: " << e.what() << std::endl;
@@ -180,7 +186,10 @@ inline void dumpParam(const Param &p, std::ostream &os) {
      << "\nglobal_registration=" << p.global_registration_ << "\nglobal_registration_voxel_size=" << p.global_registration_voxel_size_
      << "\nglobal_registration_seed=" << p.global_registration_seed_
      << "\nglobal_registration_hypotheses=" << p.global_registration_hypotheses_
-     << "\naccuracy_curve_steps=" << p.accuracy_curve_steps_ << "\naccuracy_curve_max=" << p.accuracy_curve_max_ << "\n";
+     << "\naccuracy_curve_steps=" << p.accuracy_curve_steps_ << "\naccuracy_curve_max=" << p.accuracy_curve_max_
+     << "\ndistance_quantiles=";
+  for (size_t i = 0; i < p.distance_quantiles_.size(); ++i) os << (i ? "," : "") << p.distance_quantiles_[i];
+  os << "\n";
 }
 
 // Eigen's default IOFormat for `vec.transpose()`: coefficients right-aligned to a common width, one space apart
@@ -243,6 +252,16 @@ class MapEvalB200 {
       *why = "accuracy_curve_max must be finite and >= 0";
       return false;
     }
+    if (p.distance_quantiles_.size() > ME_QUANTILE_MAX_PROBS) {
+      *why = "distance_quantiles: " + std::to_string(p.distance_quantiles_.size()) + " probabilities, at most " +
+             std::to_string(ME_QUANTILE_MAX_PROBS);
+      return false;
+    }
+    for (double q : p.distance_quantiles_)
+      if (!(std::isfinite(q) && q >= 0.0 && q <= 1.0)) {
+        *why = "distance_quantiles: every probability must be finite and in [0, 1]";
+        return false;
+      }
     if (p.evaluate_using_initial_) return true;
     if (p.evaluation_method_ < 0 || p.evaluation_method_ > 2) {
       *why = "Invalid registration type specified (registration_methods: " + std::to_string(p.evaluation_method_) +
@@ -311,6 +330,7 @@ class MapEvalB200 {
   int renderEntropy(int which, int64_t n, render::ColoredCloud *out);
   int renderDistances(bool cutoff_strict);
   int accuracyCurve(const me_nn_params &p, const std::vector<me_nn_accum> &e2g, const std::vector<me_nn_accum> &g2e);
+  int distanceQuantiles();
   GpuGroup gpus_;            // one context per GPU; rank r evaluates the r-th shard of every sweep's query range
   me_ctx *ctx_ = nullptr;    // = gpus_.ctx(0): the voxel stage and the single-GPU calls
   std::vector<double> map_3d_, gt_3d_;   // N x 3 fp64, the layout of open3d PointCloud::points_ (as loaded)
@@ -591,6 +611,7 @@ inline int MapEvalB200::calculateMetricsWithInitialMatrix() {
   if (me_nn_finalize(&p, &e2g[0], &g2e[0], n_est_, n_gt_, &nn_) != ME_OK) return fail("me_nn_finalize");
   t_acc = tic.toc() / 1000.0;
   if (param_.accuracy_curve_steps_ > 0 && accuracyCurve(p, e2g, g2e) != 0) return -1;
+  if (!param_.distance_quantiles_.empty() && distanceQuantiles() != 0) return -1;
   if (nn_.gt_to_est.n_ub > 0)
     std::cerr << "WARNING: " << nn_.gt_to_est.n_ub << " gt->est pairs index past the end of a cloud (the reference reads out of "
                  "bounds there, map_eval.cpp:1233 vs :1093-1094: undefined behaviour); they are left out of the gt->est statistics, "
@@ -638,6 +659,58 @@ inline int MapEvalB200::accuracyCurve(const me_nn_params &p, const std::vector<m
     f << " " << r.cd << " " << r.f1 << " " << r.iou << "\n";
   }
   std::cout << "INFO: accuracy curve (" << K << " levels up to " << param_.accuracy_curve_max_ << ") saved to " << path << std::endl;
+  return 0;
+}
+
+// distance quantiles: both populations of the pass's NN records at the distance_quantiles probabilities (the me_nn_quantile_*
+// loop on every GPU, one NCCL all-reduce of the pass's counts per pass) -> distance_quantiles.txt next to map_results.txt
+inline int MapEvalB200::distanceQuantiles() {
+  const std::vector<double> &pr = param_.distance_quantiles_;
+  const int K = (int)pr.size();
+  me_quantile_result res[2];
+  for (int pop : {ME_DIST_KEPT, ME_DIST_NN}) {
+    if (gpus_.for_each([&](int, me_ctx *c) { return me_nn_quantile_begin(c, pop, pr.data(), K); }) != ME_OK)
+      return fail("me_nn_quantile_begin");
+    for (bool done = false; !done;) {
+      std::vector<double *> ptr(gpus_.size(), nullptr);
+      std::vector<int32_t> len(gpus_.size(), 0), flag(gpus_.size(), 0);
+      if (gpus_.for_each([&](int r, me_ctx *c) {
+            const int rc = me_nn_quantile_block(c, &ptr[r], &len[r]);
+            return rc != ME_OK ? rc : me_synchronize(c);
+          }) != ME_OK)
+        return fail("me_nn_quantile_block");
+      if (!gpus_.allreduce_device(ptr, (size_t)len[0], ncclSum)) return fail("all-reduce of the distance quantile counts");
+      if (gpus_.for_each([&](int r, me_ctx *c) { return me_nn_quantile_step(c, &flag[r]); }) != ME_OK) return fail("me_nn_quantile_step");
+      done = flag[0] != 0;
+    }
+    if (gpus_.for_each([&](int r, me_ctx *c) {
+          me_quantile_result mine;
+          const int rc = me_nn_quantile_end(c, &mine);
+          if (r == 0) res[pop] = mine;
+          return rc;
+        }) != ME_OK)
+      return fail("me_nn_quantile_end");
+  }
+  const std::string path = results_subfolder + "distance_quantiles.txt";
+  std::ofstream f(path);
+  if (!f.is_open()) {
+    std::cerr << "ERROR: cannot write " << path << std::endl;
+    return -1;
+  }
+  f << "# kept: the kept pairs' distances; nn: every query's nearest-neighbour distance.  value: numpy quantile(method=linear)\n";
+  f << "population direction n p value lo hi\n";
+  f << std::fixed << std::setprecision(15);
+  for (int pop : {ME_DIST_KEPT, ME_DIST_NN})
+    for (int q = 0; q < 2; ++q) {
+      const me_quantile_dir &d = q == 0 ? res[pop].est_to_gt : res[pop].gt_to_est;
+      for (int k = 0; k < K; ++k)
+        f << (pop == ME_DIST_KEPT ? "kept" : "nn") << " " << (q == 0 ? "est_to_gt" : "gt_to_est") << " " << d.n << " " << pr[k] << " "
+          << d.value[k] << " " << d.lo[k] << " " << d.hi[k] << "\n";
+    }
+  const me_quantile_result &nn = res[ME_DIST_NN];
+  f << "hausdorff_est_to_gt " << nn.est_to_gt.max << "\nhausdorff_gt_to_est " << nn.gt_to_est.max << "\nhausdorff " << nn.hausdorff << "\n";
+  std::cout << "INFO: Hausdorff distance: " << nn.hausdorff << " (est->gt " << nn.est_to_gt.max << ", gt->est " << nn.gt_to_est.max
+            << "); distance quantiles saved to " << path << std::endl;
   return 0;
 }
 
@@ -742,6 +815,7 @@ inline int MapEvalB200::performRegistration() {
   if (me_nn_finalize(&p, &e2g[0], &g2e[0], n_est_, n_gt_, &nn_) != ME_OK) return fail("me_nn_finalize");
   t_acc = tic.toc() / 1000.0;
   if (param_.accuracy_curve_steps_ > 0 && accuracyCurve(p, e2g, g2e) != 0) return -1;
+  if (!param_.distance_quantiles_.empty() && distanceQuantiles() != 0) return -1;
   if (param_.save_immediate_result_ && renderDistances(true) != 0) return -1;
   full_chamfer_dist = nn_.full_cd;
   t_fcd = t_acc;

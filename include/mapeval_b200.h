@@ -417,6 +417,45 @@ ME_API int  me_nn_curve_finalize(const me_nn_params *p, const me_nn_accum *est_t
                                  me_curve_row *rows);   /* host only, no device work */
 ME_API int  me_nn_curve(me_ctx *ctx, const double *tau, int32_t n_tau, me_curve_row *rows);
 
+/* ---- exact distance quantiles and the Hausdorff distance ------------------------------------------------------------------
+ * From the per-query records of the LAST me_eval_nn* call (stale as for me_nn_curve*), per direction one population of fp64
+ * distances:
+ *   ME_DIST_KEPT  the kept pairs and their d, exactly as the five-level statistics and me_nn_curve* keep them (both cut-off
+ *                 modes; ME_PAIRING_AS_WRITTEN gt->est: d from the swapped indices, out-of-range pairs left out).  n = n_corr.
+ *   ME_DIST_NN    every evaluated query's nearest-neighbour distance sqrt(d2), the terms of sum_nn_dist (full CD).  Needs
+ *                 want_full_cd = 1 in that call (else ME_ERR_INVALID).  n = n_query.
+ * For probabilities p[0..K-1] (1 <= K <= ME_QUANTILE_MAX_PROBS, each finite and in [0, 1]; anything else is ME_ERR_INVALID) and
+ * the sorted population x_0 <= .. <= x_{n-1}: h = (double)(n - 1) p, k = floor(h), g = h - k, lo = x_k, hi = x_{min(k+1, n-1)}
+ * (both exact), value = lo + (hi - lo) g if g < 0.5 else hi - (hi - lo) (1 - g) — numpy's quantile(method="linear").  An empty
+ * population, or a direction the call did not evaluate, has n = 0 and NaN values.  Exact and deterministic for any world:
+ * only integer counts cross ranks.
+ * The loop (as me_icp_begin .. me_icp_end): me_nn_quantile_begin checks the arguments and the records and runs pass 0;
+ * me_nn_quantile_block hands out the running pass's SUM-reducible block (*n fp64 counts, the same length on every rank and
+ * in every pass), which the caller all-reduces in place (after me_synchronize); me_nn_quantile_step reads the reduced block
+ * and runs the next pass (*done = 1 after the last one); me_nn_quantile_end fills the result.  A call that changes the clouds
+ * between begin and end makes step and end fail.  me_nn_quantiles: the whole loop, world must be 1.
+ * me_quantile_finalize (host only): value[k] from n, p[k] and lo_hi[2k] = lo, lo_hi[2k + 1] = hi, by the rule above. */
+#define ME_QUANTILE_MAX_PROBS 64
+enum { ME_DIST_KEPT = 0, ME_DIST_NN = 1 };
+typedef struct {
+  int64_t n;                                    /* population size                                           */
+  double  min, max;                             /* x_0, x_{n-1}; max is the one-sided Hausdorff distance (ME_DIST_NN) */
+  int64_t rank[ME_QUANTILE_MAX_PROBS];          /* k = floor((n - 1) p)                                      */
+  double  lo[ME_QUANTILE_MAX_PROBS], hi[ME_QUANTILE_MAX_PROBS], value[ME_QUANTILE_MAX_PROBS];
+} me_quantile_dir;
+typedef struct {
+  int32_t population, n_probs;
+  double  p[ME_QUANTILE_MAX_PROBS];
+  me_quantile_dir est_to_gt, gt_to_est;
+  double  hausdorff;                            /* ME_DIST_NN, both directions: max of the two maxima; else NaN */
+} me_quantile_result;
+ME_API int  me_nn_quantile_begin(me_ctx *ctx, int32_t population, const double *p, int32_t n_probs);
+ME_API int  me_nn_quantile_block(me_ctx *ctx, double **device_block, int32_t *n);
+ME_API int  me_nn_quantile_step(me_ctx *ctx, int32_t *done);
+ME_API int  me_nn_quantile_end(me_ctx *ctx, me_quantile_result *out);
+ME_API int  me_nn_quantiles(me_ctx *ctx, int32_t population, const double *p, int32_t n_probs, me_quantile_result *out);
+ME_API int  me_quantile_finalize(int64_t n, const double *p, int32_t n_probs, const double *lo_hi, double *values);  /* host only */
+
 /* replaces: ComputeMeanMapEntropyUsingNormalTBB / ...UsingNormal (min_neighbors 10, map_eval.cpp:1608-1737, 1538-1606),
  * ComputeMeanMapEntropy (min_neighbors 5, :1438-1535), ComputeEntropy (:1433-1436) and the min/max side effect of
  * ColorPointCloudByMME (:697-701).  entropies_host (nullable) receives N fp64, zeros where invalid. */
