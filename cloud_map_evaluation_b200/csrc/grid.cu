@@ -1049,12 +1049,14 @@ __global__ void __launch_bounds__(kThreads) transform_kernel(double *__restrict_
   }
 }
 
-// PointCloud::TransformNormals: n' = T.block<3,3>(0,0) n
+// PointCloud::TransformNormals: n' = T.block<3,3>(0,0) n, every product and sum rounded like Eigen's product in a build
+// without FMA, in the order of transform_kernel: (T0 x + T1 y) + T2 z.  The plain expression would be contracted to FMAs.
 __global__ void __launch_bounds__(kThreads) rotate_normals_kernel(double *__restrict__ nrm, long long n, Mat16 T) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const double x = nrm[3 * i], y = nrm[3 * i + 1], z = nrm[3 * i + 2];
 #pragma unroll
-    for (int r = 0; r < 3; ++r) nrm[3 * i + r] = T.t[r * 4] * x + T.t[r * 4 + 1] * y + T.t[r * 4 + 2] * z;
+    for (int r = 0; r < 3; ++r)
+      nrm[3 * i + r] = __dadd_rn(__dadd_rn(__dmul_rn(T.t[r * 4], x), __dmul_rn(T.t[r * 4 + 1], y)), __dmul_rn(T.t[r * 4 + 2], z));
   }
 }
 
