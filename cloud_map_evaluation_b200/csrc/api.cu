@@ -578,39 +578,86 @@ int me_build_grid(me_ctx *ctx, int which) {
 
 }  // extern "C"
 
-// a successful me_eval_nn*: its records serve me_nn_curve* until the clouds change (e, g == NULL: the accumulators are in
-// the device block)
-static void remember_nn(me_ctx *ctx, const me_nn_params *p, const me_nn_accum *e, const me_nn_accum *g) {
+// ---- accumulators: sweep -> d_block -> (all-reduce on the device by the caller) -> one fetch per pass ------------------------
+// The block is the only encoding of the accumulators: me_eval_*_accum decode their sections right after the sweep.
+
+// the arguments of me_eval_nn_accum* that the sweep reads
+static int check_nn_params(me_ctx *ctx, const me_nn_params *p) {
+  if (!p) return fail(ctx, ME_ERR_INVALID, "null params");
+  if (p->cutoff_mode != ME_CUTOFF_SQDIST_LE_R && p->cutoff_mode != ME_CUTOFF_DIST_LT_R) return fail(ctx, ME_ERR_INVALID, "bad cutoff_mode");
+  if (p->pairing != ME_PAIRING_AS_WRITTEN && p->pairing != ME_PAIRING_GEOMETRIC) return fail(ctx, ME_ERR_INVALID, "bad pairing");
+  return ME_OK;
+}
+
+// the NN sweeps of the requested directions into their sections of the block; on success the records serve me_nn_curve* and
+// me_nn_quantile* until the clouds change
+static int eval_nn_block(me_ctx *ctx, const me_nn_params *p) {
+  ctx->curve_valid = false;
+  ME_TRY(run_nn(ctx, p, true));
   ctx->curve_valid = true;
   ctx->curve_gen = ctx->cloud_gen;
   ctx->curve_p = *p;
-  ctx->curve_acc_host = e || g;
-  std::memset(ctx->curve_acc, 0, sizeof(ctx->curve_acc));
-  if (e) ctx->curve_acc[0] = *e;
-  if (g) ctx->curve_acc[1] = *g;
+  return ME_OK;
+}
+
+// the block, copied to the pinned host scratch once the stream has finished with it
+static int fetch_block(me_ctx *ctx, const double **h_out) {
+  static_assert(4096 + kBlkTotal * sizeof(double) <= kScratchBytes, "the accumulator block fits the pinned scratch");
+  double *h = (double *)((char *)ctx->h_pinned + 4096);
+  ME_CUDA(ctx, cudaMemcpyAsync(h, ctx->d_block, kBlkTotal * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  *h_out = h;
+  return ME_OK;
+}
+
+// the block's NN and MME sections (host copy) -> the accumulator structs; a NULL struct is skipped.  Counts come back
+// through fp64 exactly (below 2^53), the entropy minimum through an exact negation.
+static void decode_block(const double *h, me_nn_accum *est_to_gt, me_nn_accum *gt_to_est, me_mme_accum *mme_est, me_mme_accum *mme_gt) {
+  auto i64 = [](double v) { return (int64_t)std::llround(v); };
+  me_nn_accum *dirs[2] = {est_to_gt, gt_to_est};
+  for (int d = 0; d < 2; ++d) {
+    me_nn_accum *a = dirs[d];
+    if (!a) continue;
+    const double *b = h + d * kBlkNN;
+    a->n_query = i64(b[0]); a->n_corr = i64(b[1]);
+    for (int k = 0; k < 5; ++k) a->n_inlier[k] = i64(b[2 + k]);
+    a->n_ub = i64(b[7]); a->n_far = i64(b[8]);
+    for (int k = 0; k < 5; ++k) { a->sum_d[k] = b[9 + k]; a->sum_d2[k] = b[14 + k]; }
+    a->sum_d_all = b[19]; a->sum_d2_all = b[20]; a->sum_nn_dist = b[21];
+    for (int r = 0; r < ME_MAX_WORLD; ++r) {
+      a->rank_n[r] = b[kBlkMoments + r]; a->rank_mean[r] = b[kBlkMoments + ME_MAX_WORLD + r];
+      a->rank_m2[r] = b[kBlkMoments + 2 * ME_MAX_WORLD + r];
+    }
+  }
+  me_mme_accum *mm[2] = {mme_est, mme_gt};
+  for (int w = 0; w < 2; ++w) {
+    me_mme_accum *m = mm[w];
+    if (!m) continue;
+    const double *b = h + kBlkMmeSum + 3 * w, *x = h + kBlkMax + 2 * w;
+    m->n_query = i64(b[0]); m->n_valid = i64(b[1]); m->sum_entropy = b[2];
+    m->max_entropy = x[0]; m->min_entropy = -x[1];
+  }
 }
 
 extern "C" {
 
-int me_eval_nn_accum(me_ctx *ctx, const me_nn_params *p, me_nn_accum *est_to_gt, me_nn_accum *gt_to_est) {
-  ME_ENTER(ctx);
-  if (!p) return fail(ctx, ME_ERR_INVALID, "null params");
-  if (p->cutoff_mode != ME_CUTOFF_SQDIST_LE_R && p->cutoff_mode != ME_CUTOFF_DIST_LT_R) return fail(ctx, ME_ERR_INVALID, "bad cutoff_mode");
-  if (p->pairing != ME_PAIRING_AS_WRITTEN && p->pairing != ME_PAIRING_GEOMETRIC) return fail(ctx, ME_ERR_INVALID, "bad pairing");
-  const int dirs = p->directions ? p->directions : 3;
-  if (((dirs & 1) && !est_to_gt) || ((dirs & 2) && !gt_to_est)) return fail(ctx, ME_ERR_INVALID, "null accumulator for a requested direction");
-  ctx->curve_valid = false;
-  ME_TRY(run_nn(ctx, p, est_to_gt, gt_to_est));
-  remember_nn(ctx, p, est_to_gt, gt_to_est);
-  return ME_OK;
-}
-
-// ---- device-resident accumulators: sweep -> (all-reduce on the device by the caller) -> one fetch per pass ----------------
 __global__ void block_init_kernel(double *blk) {
   for (int t = threadIdx.x; t < me::kBlkTotal; t += blockDim.x) blk[t] = t < me::kBlkSumCount ? 0.0 : -INFINITY;
 }
 
-extern "C" {
+int me_eval_nn_accum(me_ctx *ctx, const me_nn_params *p, me_nn_accum *est_to_gt, me_nn_accum *gt_to_est) {
+  ME_ENTER(ctx);
+  ME_TRY(check_nn_params(ctx, p));
+  const int dirs = p->directions ? p->directions : 3;
+  if (((dirs & 1) && !est_to_gt) || ((dirs & 2) && !gt_to_est)) return fail(ctx, ME_ERR_INVALID, "null accumulator for a requested direction");
+  if (est_to_gt) std::memset(est_to_gt, 0, sizeof(*est_to_gt));      // a direction not requested stays zero
+  if (gt_to_est) std::memset(gt_to_est, 0, sizeof(*gt_to_est));
+  ME_TRY(eval_nn_block(ctx, p));
+  const double *h = nullptr;
+  ME_TRY(fetch_block(ctx, &h));
+  decode_block(h, (dirs & 1) ? est_to_gt : nullptr, (dirs & 2) ? gt_to_est : nullptr, nullptr, nullptr);
+  return ME_OK;
+}
 
 int me_accum_reset(me_ctx *ctx) {
   ME_ENTER(ctx);
@@ -621,19 +668,14 @@ int me_accum_reset(me_ctx *ctx) {
 
 int me_eval_nn_accum_device(me_ctx *ctx, const me_nn_params *p) {
   ME_ENTER(ctx);
-  if (!p) return fail(ctx, ME_ERR_INVALID, "null params");
-  if (p->cutoff_mode != ME_CUTOFF_SQDIST_LE_R && p->cutoff_mode != ME_CUTOFF_DIST_LT_R) return fail(ctx, ME_ERR_INVALID, "bad cutoff_mode");
-  if (p->pairing != ME_PAIRING_AS_WRITTEN && p->pairing != ME_PAIRING_GEOMETRIC) return fail(ctx, ME_ERR_INVALID, "bad pairing");
-  ctx->curve_valid = false;
-  ME_TRY(run_nn(ctx, p, nullptr, nullptr, true));
-  remember_nn(ctx, p, nullptr, nullptr);
-  return ME_OK;
+  ME_TRY(check_nn_params(ctx, p));
+  return eval_nn_block(ctx, p);
 }
 
 int me_eval_mme_accum_device(me_ctx *ctx, int which, double radius, int32_t min_neighbors) {
   ME_ENTER(ctx);
   if (which != ME_CLOUD_EST && which != ME_CLOUD_GT) return fail(ctx, ME_ERR_INVALID, "bad arguments");
-  return run_mme(ctx, which, radius, min_neighbors, nullptr, true);
+  return run_mme(ctx, which, radius, min_neighbors);
 }
 
 int me_accum_block(me_ctx *ctx, double **device_block, int32_t *n_sum, int32_t *n_max) {
@@ -663,54 +705,19 @@ int me_voxel_finish_accum_device(me_ctx *ctx, int32_t scs_radius) {
 int me_accum_fetch_awd(me_ctx *ctx, me_awd_result *out) {
   ME_ENTER(ctx);
   if (!out) return fail(ctx, ME_ERR_INVALID, "null result");
-  double *h = (double *)((char *)ctx->h_pinned + 4096);
-  ME_CUDA(ctx, cudaMemcpyAsync(h, ctx->d_block + kBlkAwd, 8 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-  ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  auto i64 = [](double v) { return (int64_t)std::llround(v); };
-  std::memset(out, 0, sizeof(*out));
-  out->n_pairs = i64(h[0]); out->n_scs = i64(h[1]);
-  out->n_voxels_est = i64(h[2]); out->n_voxels_gt = i64(h[3]);
-  out->n_active = i64(h[4]); out->n_new = i64(h[5]);
-  out->n_old = out->n_voxels_gt - out->n_active;
-  out->awd = h[6] / (double)out->n_pairs;        // 0/0 -> NaN as map_eval.cpp:324
-  out->scs = h[7] / (double)out->n_scs;          // map_eval.cpp:387
+  const double *h = nullptr;
+  ME_TRY(fetch_block(ctx, &h));
+  awd_result(h + kBlkAwd, out);
   return ME_OK;
 }
 
 int me_accum_fetch(me_ctx *ctx, me_nn_accum *est_to_gt, me_nn_accum *gt_to_est, me_mme_accum *mme_est, me_mme_accum *mme_gt) {
   ME_ENTER(ctx);
-  static_assert(4096 + kBlkTotal * sizeof(double) <= kScratchBytes, "the accumulator block fits the pinned scratch");
-  double *h = (double *)((char *)ctx->h_pinned + 4096);
-  ME_CUDA(ctx, cudaMemcpyAsync(h, ctx->d_block, kBlkTotal * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-  ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  auto i64 = [](double v) { return (int64_t)std::llround(v); };
-  me_nn_accum *dirs[2] = {est_to_gt, gt_to_est};
-  for (int d = 0; d < 2; ++d) {
-    me_nn_accum *a = dirs[d];
-    if (!a) continue;
-    const double *b = h + d * kBlkNN;
-    a->n_query = i64(b[0]); a->n_corr = i64(b[1]);
-    for (int k = 0; k < 5; ++k) a->n_inlier[k] = i64(b[2 + k]);
-    a->n_ub = i64(b[7]); a->n_far = i64(b[8]);
-    for (int k = 0; k < 5; ++k) { a->sum_d[k] = b[9 + k]; a->sum_d2[k] = b[14 + k]; }
-    a->sum_d_all = b[19]; a->sum_d2_all = b[20]; a->sum_nn_dist = b[21];
-    for (int r = 0; r < ME_MAX_WORLD; ++r) {
-      a->rank_n[r] = b[kBlkMoments + r]; a->rank_mean[r] = b[kBlkMoments + ME_MAX_WORLD + r];
-      a->rank_m2[r] = b[kBlkMoments + 2 * ME_MAX_WORLD + r];
-    }
-  }
-  me_mme_accum *mm[2] = {mme_est, mme_gt};
-  for (int w = 0; w < 2; ++w) {
-    me_mme_accum *m = mm[w];
-    if (!m) continue;
-    const double *b = h + kBlkMmeSum + 3 * w, *x = h + kBlkMax + 2 * w;
-    m->n_query = i64(b[0]); m->n_valid = i64(b[1]); m->sum_entropy = b[2];
-    m->max_entropy = x[0]; m->min_entropy = -x[1];
-  }
+  const double *h = nullptr;
+  ME_TRY(fetch_block(ctx, &h));
+  decode_block(h, est_to_gt, gt_to_est, mme_est, mme_gt);
   return ME_OK;
 }
-
-}  // extern "C"
 
 // the per-level arithmetic of me_nn_finalize, shared with me_nn_curve_finalize so that a level both compute is one expression
 struct DirMoments {           // one direction's accumulator, reduced over the ranks
@@ -850,8 +857,7 @@ int me_nn_curve(me_ctx *ctx, const double *tau, int32_t n_tau, me_curve_row *row
   int32_t n = 0;
   ME_TRY(me_nn_curve_accum_device(ctx, tau, n_tau, &d_blk, &n));
   me_nn_accum acc[2];
-  if (ctx->curve_acc_host) { acc[0] = ctx->curve_acc[0]; acc[1] = ctx->curve_acc[1]; }
-  else ME_TRY(me_accum_fetch(ctx, &acc[0], &acc[1], nullptr, nullptr));
+  ME_TRY(me_accum_fetch(ctx, &acc[0], &acc[1], nullptr, nullptr));
   std::vector<double> h((size_t)n);
   ME_CUDA(ctx, cudaMemcpyAsync(h.data(), d_blk, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -934,7 +940,11 @@ int me_get_nn(me_ctx *ctx, int which_query, int32_t *nn_index, double *nn_sqdist
 int me_eval_mme_accum(me_ctx *ctx, int which, double radius, int32_t min_neighbors, me_mme_accum *out) {
   ME_ENTER(ctx);
   if ((which != ME_CLOUD_EST && which != ME_CLOUD_GT) || !out) return fail(ctx, ME_ERR_INVALID, "bad arguments");
-  return run_mme(ctx, which, radius, min_neighbors, out);
+  ME_TRY(run_mme(ctx, which, radius, min_neighbors));
+  const double *h = nullptr;
+  ME_TRY(fetch_block(ctx, &h));
+  decode_block(h, nullptr, nullptr, which == ME_CLOUD_EST ? out : nullptr, which == ME_CLOUD_GT ? out : nullptr);
+  return ME_OK;
 }
 
 int me_mme_finalize(const me_mme_accum *acc, int64_t n_total, me_mme_result *out) {

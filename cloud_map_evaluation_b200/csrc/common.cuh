@@ -246,7 +246,7 @@ struct me_ctx {
   size_t scratch_bytes = 0;
   void *h_pinned = nullptr;         // pinned host mirror of the scratch
   void *stage = nullptr;            // pinned bounce buffers + streams of the pageable-memory upload path (api.cu)
-  double *d_block = nullptr;        // device-resident accumulator block of the *_device calls (ME_BLOCK_* layout, api.cu)
+  double *d_block = nullptr;        // device-resident accumulator block of the me_eval_*_accum* calls (kBlk* layout below)
   // large device scratch (scan partials, far list, voxel tables)
   void *d_work = nullptr;
   size_t work_bytes = 0;
@@ -272,8 +272,6 @@ struct me_ctx {
   bool curve_valid = false;            // the last me_eval_nn* succeeded
   unsigned long long curve_gen = 0;    // cloud_gen at that call
   me_nn_params curve_p{};              // its parameters
-  bool curve_acc_host = false;         // its accumulators are curve_acc (me_eval_nn_accum), else in d_block (the _device call)
-  me_nn_accum curve_acc[2];
   double *d_curve = nullptr;           // the curve block (both directions), then the levels
   long long cap_curve = 0;
   me::QuantRun quant;                  // distance quantiles (me_nn_quantile*), from the same records
@@ -374,8 +372,9 @@ int exclusive_scan_inplace(me_ctx *ctx, uint32_t *a, long long n, unsigned long 
 int voxel_downsample(me_ctx *ctx, int which, double voxel_size, int64_t *n_out);
 int radix_sort_pairs(me_ctx *ctx, unsigned long long *keys, uint32_t *vals, unsigned long long *keys_tmp, uint32_t *vals_tmp,
                      long long n, int key_bits, unsigned long long **keys_sorted, uint32_t **vals_sorted);
-// sweep_only: the per-query results only (d_nn_idx / d_nn_d2), no accumulators handed out (registration)
-int run_nn(me_ctx *ctx, const me_nn_params *p, me_nn_accum *e2g, me_nn_accum *g2e, bool to_block = false, bool sweep_only = false);
+// pack: the accumulators of every evaluated direction into its section of d_block; false: the per-query results only
+// (d_nn_idx / d_nn_d2, registration)
+int run_nn(me_ctx *ctx, const me_nn_params *p, bool pack);
 int unsort_nn(me_ctx *ctx, int which_query, int32_t *h_idx, double *h_d2);
 // the curve block of the last me_eval_nn* at the K levels tau (host memory, checked by the caller) — me_nn_curve_accum_device
 int nn_curve(me_ctx *ctx, const double *tau, int K, double **device_block, int32_t *n);
@@ -385,7 +384,8 @@ int nn_quantile_block(me_ctx *ctx, double **device_block, int32_t *n);
 int nn_quantile_step(me_ctx *ctx, int32_t *done);
 int nn_quantile_end(me_ctx *ctx, me_quantile_result *out);
 void nn_quantile_free(me_ctx *ctx);
-int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors, me_mme_accum *out, bool to_block = false);
+// the accumulators go to the cloud's MME section of d_block
+int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors);
 
 // layout of me_ctx::d_block (fp64): the SUM-reducible part first, then the MAX-reducible part.  Counts ride as fp64 (exact
 // below 2^53, so their sums are exact and order-independent).
@@ -403,6 +403,8 @@ static constexpr int kBlkTotal = kBlkSumCount + kBlkMaxCount;
 int unsort_entropy(me_ctx *ctx, int which, double *h_entropy);
 int run_awd(me_ctx *ctx, double voxel_size, int min_points, int scs_radius, me_awd_result *out, int64_t *n_rows,
             double **rows27);
+// the voxel stage's eight values in the order of the block's AWD section -> the result (map_eval.cpp:324,387)
+void awd_result(const double v[8], me_awd_result *out);
 bool plan_lattice_host(const double bmin[3], const double bmax[3], long long n, const double *obmin, const double *obmax,
                        long long other_n, double v_req, double h_target, long long budget, bool allow_sparse, Lattice *out);
 static constexpr double kSlabMaxShare = 0.75;      // a slab cut whose busiest rank lays out more than this share is not worth it

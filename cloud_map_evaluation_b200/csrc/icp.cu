@@ -555,7 +555,7 @@ static int icp_sweep(me_ctx *ctx) {
   p.pairing = ME_PAIRING_GEOMETRIC;
   p.want_full_cd = 0;
   p.directions = 1;
-  ME_TRY(run_nn(ctx, &p, nullptr, nullptr, false, true));      // lays the moved cloud out again, then sweeps this rank's queries
+  ME_TRY(run_nn(ctx, &p, false));      // lays the moved cloud out again, then sweeps this rank's queries
   const long long qb = E.nn_b, qe = E.nn_e;
   const int blocks = (int)std::max(1ll, std::min<long long>((qe - qb + kThreads - 1) / kThreads, (long long)ctx->sm_count * 8));
   double *blk = icp_block_dev(ctx);

@@ -621,7 +621,7 @@ static int launch_flat(me_ctx *ctx, Cloud &c, long long qb, long long qe, const 
   return ME_OK;
 }
 
-// MME accumulators -> the context's fp64 block (me_eval_mme_accum_device)
+// MME accumulators -> the context's fp64 block (me_eval_mme_accum*)
 __global__ void pack_mme_kernel(const MmeAcc *__restrict__ a, double *__restrict__ sum3, double *__restrict__ max2) {
   if (threadIdx.x != 0) return;
   sum3[0] = (double)a->n_query; sum3[1] = (double)a->n_valid; sum3[2] = a->sum;
@@ -637,7 +637,7 @@ __global__ void unsort_f64_kernel(const P4 *__restrict__ S, long long n, const d
   }
 }
 
-int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors, me_mme_accum *out, bool to_block) {
+int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors) {
   Cloud &c = ctx->cloud[which];
   if (c.n <= 0) return fail(ctx, ME_ERR_EMPTY, "cloud is empty");
   if (!(radius > 0)) return fail(ctx, ME_ERR_INVALID, "nn_radius must be > 0");
@@ -738,19 +738,8 @@ int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors, me_mme_acc
       trace_kernel(ctx, ME_KBIT_MME_GENERIC);
     }
   }
-  if (to_block) {
-    pack_mme_kernel<<<1, 32, 0, ctx->stream>>>(acc, ctx->d_block + kBlkMmeSum + 3 * which, ctx->d_block + kBlkMax + 2 * which);
-    ME_LAUNCH_CHECK(ctx);
-  } else {
-    MmeAcc *h = (MmeAcc *)ctx->h_pinned;
-    ME_CUDA(ctx, cudaMemcpyAsync(h, acc, sizeof(MmeAcc), cudaMemcpyDeviceToHost, ctx->stream));
-    ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    out->n_query = (int64_t)h->n_query;
-    out->n_valid = (int64_t)h->n_valid;
-    out->sum_entropy = h->sum;
-    out->min_entropy = dec_ordered(h->min_enc);
-    out->max_entropy = dec_ordered(h->max_enc);
-  }
+  pack_mme_kernel<<<1, 32, 0, ctx->stream>>>(acc, ctx->d_block + kBlkMmeSum + 3 * which, ctx->d_block + kBlkMax + 2 * which);
+  ME_LAUNCH_CHECK(ctx);
   c.entropy_valid = true;
   c.entropy_caller_valid = false;
   if (c.grid_solo) {      // the solo lattice (and with it the sorted order of d_entropy) does not survive the next build

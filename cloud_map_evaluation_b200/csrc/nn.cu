@@ -1146,7 +1146,7 @@ __global__ void __launch_bounds__(kThreads) merge_moments_kernel(const double *_
   if (threadIdx.x == 0) { acc->mean_all = m; acc->m2_all = m2; acc->sum_d_all = n * m; acc->sum_d2_all = m2 + n * m * m; }
 }
 
-// accumulator block of one direction -> the context's fp64 block (me_eval_nn_accum_device): no host round trip.  The
+// accumulator block of one direction -> the context's fp64 block (me_eval_nn_accum*): no host round trip.  The
 // moments go to this rank's slot; the other ranks' slots are zeroed, so that the SUM all-reduce gathers them.
 __global__ void pack_nn_kernel(const AccBlock *__restrict__ a, const unsigned long long *__restrict__ n_eval, long long n_query,
                                int rank, double *__restrict__ blk) {
@@ -1173,7 +1173,7 @@ static void set_cutoff(NNConst &C, const me_nn_params *p) {
   C.cutoff = p->cutoff_mode == ME_CUTOFF_SQDIST_LE_R ? p->icp_max_distance : p->icp_max_distance * p->icp_max_distance;
 }
 
-static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, me_nn_accum *out, int stage, bool to_block) {
+static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, int stage, bool pack) {
   Cloud &Qc = ctx->cloud[qwhich];
   Cloud &Rc = ctx->cloud[1 - qwhich];
   StageTimer timer(ctx, stage);
@@ -1312,34 +1312,15 @@ static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, me_nn_a
   }
   Qc.nn_b = use_tile ? 0 : qb;
   Qc.nn_e = use_tile ? Qc.n : qe;
-  if (!out && !to_block) {      // sweep only: the caller reads the per-query results
-    Qc.nn_valid = true;
-    return ME_OK;
-  }
-  if (sharded && use_tile) {
-    count_marked_kernel<<<fill_blocks, kThreads, 0, ctx->stream>>>(Qc.d_nn_idx, Qc.n, n_eval);
-    ME_LAUNCH_CHECK(ctx);
-  }
-  if (to_block) {      // the accumulators stay on the device (all-reduced there, fetched once per pass)
+  if (pack) {      // the accumulators stay on the device (all-reduced there, fetched once per pass)
+    if (sharded && use_tile) {
+      count_marked_kernel<<<fill_blocks, kThreads, 0, ctx->stream>>>(Qc.d_nn_idx, Qc.n, n_eval);
+      ME_LAUNCH_CHECK(ctx);
+    }
     pack_nn_kernel<<<1, 32, 0, ctx->stream>>>(acc, (sharded && use_tile) ? n_eval : nullptr, Qc.slab ? Qc.n_owned : (sharded ? qe - qb : Qc.n),
                                               ctx->rank, ctx->d_block + (qwhich == ME_CLOUD_EST ? 0 : kBlkNN));
     ME_LAUNCH_CHECK(ctx);
-    Qc.nn_valid = true;
-    return ME_OK;
   }
-  AccBlock *h = (AccBlock *)ctx->h_pinned;
-  unsigned long long *h_eval = (unsigned long long *)((char *)ctx->h_pinned + 1024);
-  ME_CUDA(ctx, cudaMemcpyAsync(h, acc, sizeof(AccBlock), cudaMemcpyDeviceToHost, ctx->stream));
-  if (sharded && use_tile) ME_CUDA(ctx, cudaMemcpyAsync(h_eval, n_eval, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
-  ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  std::memset(out, 0, sizeof(*out));
-  out->n_query = !sharded ? Qc.n : (use_tile ? (int64_t)*h_eval : (Qc.slab ? Qc.n_owned : qe - qb));
-  out->n_corr = (int64_t)h->n_corr;
-  for (int k = 0; k < 5; ++k) { out->n_inlier[k] = (int64_t)h->n_inl[k]; out->sum_d[k] = h->sum_d[k]; out->sum_d2[k] = h->sum_d2[k]; }
-  out->n_ub = (int64_t)h->n_ub;
-  out->n_far = (int64_t)h->n_far;
-  out->sum_d_all = h->sum_d_all; out->sum_d2_all = h->sum_d2_all; out->sum_nn_dist = h->sum_nn;
-  out->rank_n[ctx->rank] = (double)h->n_corr; out->rank_mean[ctx->rank] = h->mean_all; out->rank_m2[ctx->rank] = h->m2_all;
   Qc.nn_valid = true;
   return ME_OK;
 }
@@ -1354,16 +1335,13 @@ int build_both(me_ctx *ctx) {
   return fail(ctx, ME_ERR_RANGE, "could not lay both clouds out on a common lattice");
 }
 
-int run_nn(me_ctx *ctx, const me_nn_params *p, me_nn_accum *e2g, me_nn_accum *g2e, bool to_block, bool sweep_only) {
+int run_nn(me_ctx *ctx, const me_nn_params *p, bool pack) {
   if (ctx->cloud[0].n <= 0 || ctx->cloud[1].n <= 0)
     return fail(ctx, ME_ERR_EMPTY, "both clouds must be set (map_eval.cpp:32-35)");
   ME_TRY(build_both(ctx));
   const int dirs = p->directions ? p->directions : 3;
-  if (e2g) std::memset(e2g, 0, sizeof(*e2g));
-  if (g2e) std::memset(g2e, 0, sizeof(*g2e));
-  if (sweep_only) { e2g = g2e = nullptr; to_block = false; }
-  if ((dirs & 1) && (e2g || to_block || sweep_only)) ME_TRY(run_direction(ctx, ME_CLOUD_EST, p, e2g, 2, to_block));
-  if ((dirs & 2) && (g2e || to_block || sweep_only)) ME_TRY(run_direction(ctx, ME_CLOUD_GT, p, g2e, 3, to_block));
+  if (dirs & 1) ME_TRY(run_direction(ctx, ME_CLOUD_EST, p, 2, pack));
+  if (dirs & 2) ME_TRY(run_direction(ctx, ME_CLOUD_GT, p, 3, pack));
   return ME_OK;
 }
 

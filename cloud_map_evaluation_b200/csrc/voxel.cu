@@ -503,6 +503,17 @@ int voxel_finish_block(me_ctx *ctx, int scs_radius) {
   return ME_OK;
 }
 
+void awd_result(const double v[8], me_awd_result *out) {
+  auto i64 = [](double x) { return (int64_t)std::llround(x); };
+  std::memset(out, 0, sizeof(*out));
+  out->n_pairs = i64(v[0]); out->n_scs = i64(v[1]);
+  out->n_voxels_est = i64(v[2]); out->n_voxels_gt = i64(v[3]);
+  out->n_active = i64(v[4]); out->n_new = i64(v[5]);
+  out->n_old = out->n_voxels_gt - out->n_active;
+  out->awd = v[6] / (double)out->n_pairs;        // 0/0 -> NaN as map_eval.cpp:324
+  out->scs = v[7] / (double)out->n_scs;          // map_eval.cpp:387
+}
+
 int run_awd(me_ctx *ctx, double voxel_size, int min_points, int scs_radius, me_awd_result *out, int64_t *n_rows,
             double **rows27) {
   std::memset(out, 0, sizeof(*out));
@@ -521,15 +532,10 @@ int run_awd(me_ctx *ctx, double voxel_size, int min_points, int scs_radius, me_a
   Host *h = (Host *)ctx->h_pinned;
   ME_CUDA(ctx, cudaMemcpyAsync(h, ctx->d_scratch, sizeof(Host), cudaMemcpyDeviceToHost, ctx->stream));
   ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  out->n_pairs = (int64_t)h->a.n_pairs;
-  out->n_scs = (int64_t)h->a.n_scs;
-  out->n_voxels_est = (int64_t)h->occ[0];
-  out->n_voxels_gt = (int64_t)h->occ[1];
-  out->n_active = (int64_t)h->a.n_active;
-  out->n_new = (int64_t)h->a.n_new;
-  out->n_old = out->n_voxels_gt - out->n_active;
-  out->awd = h->a.sum_w / (double)h->a.n_pairs;        // 0/0 -> NaN as map_eval.cpp:324
-  out->scs = h->a.sum_scs / (double)h->a.n_scs;        // map_eval.cpp:387
+  // the values pack_awd_kernel would write (counts exact in fp64 below 2^53); no launch on this single-GPU path
+  const double v[8] = {(double)h->a.n_pairs, (double)h->a.n_scs, (double)h->occ[0], (double)h->occ[1],
+                       (double)h->a.n_active, (double)h->a.n_new, h->a.sum_w, h->a.sum_scs};
+  awd_result(v, out);
   if (n_rows) *n_rows = out->n_pairs;
   if (rows27) {
     size_t bytes = (size_t)std::max<int64_t>(out->n_pairs, 1) * 27 * sizeof(double);

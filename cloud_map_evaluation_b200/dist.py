@@ -1,78 +1,14 @@
 """Multi-GPU plumbing: one process per GPU; the evaluated cloud's query ranges sharded by rank with both lattices laid out whole
 (replicated layout), or every rank laying out and evaluating only its voxel layers (slab layout, MapEvalB200.set_layout); ONE
-all-reduce of the sum-reducible accumulators (plus a MAX pair for the entropy extrema; on a slab layout a MAX all-reduce of
-the voxel stage's W table).
+in-place all-reduce of the device accumulator block's sum-reducible values (plus a MAX all-reduce of its entropy extrema;
+on a slab layout a MAX all-reduce of the voxel stage's W table).  allreduce_block is the one way to reduce accumulators:
+the *_accum_device sweeps fill the block, accum_fetch decodes it.
 
 The reference is single-process (SURVEY.md §5); this is the H100-native equivalent of its TBB/OpenMP reductions
 (map_eval.cpp:1411,1420,1704-1708).  torch.distributed is used for the collectives only: backend "nccl" on GPUs
 (NVLink / NVSwitch), "gloo" in the CPU tests.
 """
 from . import _abi as A
-
-_NN_I = A.ME_NN_ACCUM_I64
-_NN_F = A.ME_NN_ACCUM_F64
-
-
-def pack(nn_e, nn_g, mme_list):
-    """Flatten the accumulators into (int64 list, fp64 list, min list, max list)."""
-    ints, flts, mins, maxs = [], [], [], []
-    for a in (nn_e, nn_g):
-        ints += [a.n_query, a.n_corr] + list(a.n_inlier) + [a.n_ub, a.n_far]
-        flts += list(a.sum_d) + list(a.sum_d2) + [a.sum_d_all, a.sum_d2_all, a.sum_nn_dist] + list(a.rank_n) + list(a.rank_mean) + list(a.rank_m2)
-    for m in mme_list:
-        ints += [m.n_query, m.n_valid]
-        flts += [m.sum_entropy]
-        mins.append(m.min_entropy)
-        maxs.append(m.max_entropy)
-    return ints, flts, mins, maxs
-
-
-def unpack(ints, flts, mins, maxs, nn_e, nn_g, mme_list):
-    ii = fi = 0
-    for a in (nn_e, nn_g):
-        a.n_query, a.n_corr = int(ints[ii]), int(ints[ii + 1])
-        for k in range(5):
-            a.n_inlier[k] = int(ints[ii + 2 + k])
-        a.n_ub, a.n_far = int(ints[ii + 7]), int(ints[ii + 8])
-        ii += _NN_I
-        for k in range(5):
-            a.sum_d[k] = float(flts[fi + k])
-            a.sum_d2[k] = float(flts[fi + 5 + k])
-        a.sum_d_all, a.sum_d2_all, a.sum_nn_dist = float(flts[fi + 10]), float(flts[fi + 11]), float(flts[fi + 12])
-        W = A.ME_MAX_WORLD
-        for r in range(W):
-            a.rank_n[r] = float(flts[fi + 13 + r])
-            a.rank_mean[r] = float(flts[fi + 13 + W + r])
-            a.rank_m2[r] = float(flts[fi + 13 + 2 * W + r])
-        fi += _NN_F
-    for j, m in enumerate(mme_list):
-        m.n_query, m.n_valid = int(ints[ii]), int(ints[ii + 1])
-        ii += 2
-        m.sum_entropy = float(flts[fi])
-        fi += 1
-        m.min_entropy, m.max_entropy = float(mins[j]), float(maxs[j])
-
-
-def allreduce_accumulators(nn_e, nn_g, mme_list, device=None, group=None):
-    """In-place all-reduce of the partial accumulators of every rank: ONE SUM all-reduce over the whole block (the
-    integer counts ride along as fp64 — they stay below 2^53, so their sum is exact and order-independent: the reduced
-    inlier counts are bit-exact for any world size; fp64 sums differ from the 1-GPU run by rounding only), plus one MAX
-    all-reduce over [max entropy, -min entropy] when MME was evaluated (map_eval.cpp:697-701)."""
-    import torch
-    import torch.distributed as dist
-    ints, flts, mins, maxs = pack(nn_e, nn_g, mme_list)
-    assert all(abs(v) < 2 ** 53 for v in ints)
-    t = torch.tensor([float(v) for v in ints] + flts, dtype=torch.float64, device=device)
-    dist.all_reduce(t, group=group)
-    out = t.cpu().tolist()
-    ri, rf = [int(round(v)) for v in out[:len(ints)]], out[len(ints):]
-    rmin, rmax = [], []
-    if mins:
-        tx = torch.tensor(list(maxs) + [-v for v in mins], dtype=torch.float64, device=device)
-        dist.all_reduce(tx, op=dist.ReduceOp.MAX, group=group)
-        ox = tx.cpu().tolist()
-        rmax, rmin = ox[:len(maxs)], [-v for v in ox[len(maxs):]]
-    unpack(ri, rf, rmin, rmax, nn_e, nn_g, mme_list)
 
 
 def shard_range(n, rank, world):

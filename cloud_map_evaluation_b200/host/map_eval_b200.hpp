@@ -329,7 +329,7 @@ class MapEvalB200 {
   std::string simulationSummary() const;
   int renderEntropy(int which, int64_t n, render::ColoredCloud *out);
   int renderDistances(bool cutoff_strict);
-  int accuracyCurve(const me_nn_params &p, const std::vector<me_nn_accum> &e2g, const std::vector<me_nn_accum> &g2e);
+  int accuracyCurve(const me_nn_params &p, const me_nn_accum &e2g, const me_nn_accum &g2e);
   int distanceQuantiles();
   GpuGroup gpus_;            // one context per GPU; rank r evaluates the r-th shard of every sweep's query range
   me_ctx *ctx_ = nullptr;    // = gpus_.ctx(0): the voxel stage and the single-GPU calls
@@ -561,11 +561,11 @@ inline int MapEvalB200::computeMME() {
   if (!param_.evaluate_mme_) return 0;
   // use_tbb_mme only selects between two CPU threadings of the same arithmetic in the reference (:153-157)
   auto eval_mme = [&](int which, int min_neighbors, int64_t n_total, me_mme_result *out) -> int {
-    std::vector<me_mme_accum> acc(gpus_.size());
-    if (gpus_.for_each([&](int r, me_ctx *c) { return me_eval_mme_accum(c, which, param_.nn_radius_, min_neighbors, &acc[r]); }) != ME_OK)
+    me_mme_accum acc;
+    if (!gpus_.reduce_accum([&](me_ctx *c) { return me_eval_mme_accum_device(c, which, param_.nn_radius_, min_neighbors); }, nullptr,
+                            nullptr, which == ME_CLOUD_EST ? &acc : nullptr, which == ME_CLOUD_GT ? &acc : nullptr))
       return -1;
-    if (!gpus_.reduce_mme(acc)) return -1;
-    return me_mme_finalize(&acc[0], n_total, out) == ME_OK ? 0 : -1;
+    return me_mme_finalize(&acc, n_total, out) == ME_OK ? 0 : -1;
   };
   if (eval_mme(ME_CLOUD_EST, 10, n_est_, &mme_est_res_) != 0) return fail("me_eval_mme(est)");
   if (param_.save_immediate_result_ && renderEntropy(ME_CLOUD_EST, n_est_, &map_3d_entropy_) != 0) return -1;   // :179
@@ -601,14 +601,15 @@ inline int MapEvalB200::calculateMetricsWithInitialMatrix() {
   // so they are produced and reported on stdout, while the results file keeps the reference's value
   p.want_full_cd = 1;
   p.directions = 3;
-  std::vector<me_nn_accum> e2g(gpus_.size()), g2e(gpus_.size());
-  if (gpus_.for_each([&](int r, me_ctx *c) {
-        int rc = me_transform(c, ME_CLOUD_EST, param_.initial_matrix_);      // map_3d_->Transform(initial_matrix), :1206
-        return rc != ME_OK ? rc : me_eval_nn_accum(c, &p, &e2g[r], &g2e[r]);
-      }) != ME_OK)
-    return fail("me_transform / me_eval_nn_accum");
-  if (!gpus_.reduce_nn(e2g, g2e)) return fail("all-reduce of the NN accumulators");
-  if (me_nn_finalize(&p, &e2g[0], &g2e[0], n_est_, n_gt_, &nn_) != ME_OK) return fail("me_nn_finalize");
+  me_nn_accum e2g, g2e;
+  if (!gpus_.reduce_accum(
+          [&](me_ctx *c) {
+            int rc = me_transform(c, ME_CLOUD_EST, param_.initial_matrix_);      // map_3d_->Transform(initial_matrix), :1206
+            return rc != ME_OK ? rc : me_eval_nn_accum_device(c, &p);
+          },
+          &e2g, &g2e, nullptr, nullptr))
+    return fail("me_transform / me_eval_nn_accum_device / all-reduce of the NN accumulators");
+  if (me_nn_finalize(&p, &e2g, &g2e, n_est_, n_gt_, &nn_) != ME_OK) return fail("me_nn_finalize");
   t_acc = tic.toc() / 1000.0;
   if (param_.accuracy_curve_steps_ > 0 && accuracyCurve(p, e2g, g2e) != 0) return -1;
   if (!param_.distance_quantiles_.empty() && distanceQuantiles() != 0) return -1;
@@ -628,7 +629,7 @@ inline int MapEvalB200::calculateMetricsWithInitialMatrix() {
 
 // accuracy curve: the pass's NN records at accuracy_curve_steps levels (me_nn_curve_accum_device on every GPU, one NCCL
 // all-reduce of the blocks, me_nn_curve_finalize with the reduced accumulators) -> accuracy_curve.txt next to map_results.txt
-inline int MapEvalB200::accuracyCurve(const me_nn_params &p, const std::vector<me_nn_accum> &e2g, const std::vector<me_nn_accum> &g2e) {
+inline int MapEvalB200::accuracyCurve(const me_nn_params &p, const me_nn_accum &e2g, const me_nn_accum &g2e) {
   const int K = param_.accuracy_curve_steps_;
   std::vector<double> tau(K);
   for (int k = 1; k <= K; ++k) tau[k - 1] = (param_.accuracy_curve_max_ * (double)k) / (double)K;
@@ -642,7 +643,7 @@ inline int MapEvalB200::accuracyCurve(const me_nn_params &p, const std::vector<m
   std::vector<double> blk((size_t)len[0]);
   if (!gpus_.reduce_curve(ptr, blk)) return fail("all-reduce of the accuracy curve");
   std::vector<me_curve_row> rows(K);
-  if (me_nn_curve_finalize(&p, &e2g[0], &g2e[0], blk.data(), tau.data(), K, n_est_, n_gt_, rows.data()) != ME_OK)
+  if (me_nn_curve_finalize(&p, &e2g, &g2e, blk.data(), tau.data(), K, n_est_, n_gt_, rows.data()) != ME_OK)
     return fail("me_nn_curve_finalize");
   const std::string path = results_subfolder + "accuracy_curve.txt";
   std::ofstream f(path);
@@ -809,10 +810,10 @@ inline int MapEvalB200::performRegistration() {
   p.pairing = ME_PAIRING_GEOMETRIC;
   p.want_full_cd = 1;
   p.directions = 3;
-  std::vector<me_nn_accum> e2g(gpus_.size()), g2e(gpus_.size());
-  if (gpus_.for_each([&](int r, me_ctx *c) { return me_eval_nn_accum(c, &p, &e2g[r], &g2e[r]); }) != ME_OK) return fail("me_eval_nn_accum");
-  if (!gpus_.reduce_nn(e2g, g2e)) return fail("all-reduce of the NN accumulators");
-  if (me_nn_finalize(&p, &e2g[0], &g2e[0], n_est_, n_gt_, &nn_) != ME_OK) return fail("me_nn_finalize");
+  me_nn_accum e2g, g2e;
+  if (!gpus_.reduce_accum([&](me_ctx *c) { return me_eval_nn_accum_device(c, &p); }, &e2g, &g2e, nullptr, nullptr))
+    return fail("me_eval_nn_accum_device / all-reduce of the NN accumulators");
+  if (me_nn_finalize(&p, &e2g, &g2e, n_est_, n_gt_, &nn_) != ME_OK) return fail("me_nn_finalize");
   t_acc = tic.toc() / 1000.0;
   if (param_.accuracy_curve_steps_ > 0 && accuracyCurve(p, e2g, g2e) != 0) return -1;
   if (!param_.distance_quantiles_.empty() && distanceQuantiles() != 0) return -1;

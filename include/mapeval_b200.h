@@ -15,9 +15,10 @@
  *   - clouds are N x 3 fp64, array-of-structs — the layout of Open3D's
  *     `std::vector<Eigen::Vector3d> points_` that the reference reads.
  *   - one me_ctx = one GPU = one caller thread at a time.  Multi-GPU = one
- *     context per process/GPU with {rank, world} set; the *_accum entry points
- *     return sum-reducible partial accumulators for this rank's query range,
- *     the caller all-reduces them (NCCL) and calls the host-side *_finalize.
+ *     context per process/GPU with {rank, world} set; the *_accum_device entry
+ *     points leave this rank's partial accumulators in the context's device
+ *     block, the caller all-reduces it in place (NCCL), fetches it once
+ *     (me_accum_fetch) and calls the host-side *_finalize.
  *   - there is NO CPU fallback in this library: without a usable CUDA device
  *     me_create fails with ME_ERR_NO_DEVICE.
  */
@@ -379,7 +380,9 @@ ME_API int me_get_features(me_ctx *ctx, int which, double *xyz, double *normals,
 ME_API int me_get_correspondences(me_ctx *ctx, int32_t *est_idx, int32_t *gt_idx, int64_t capacity, int64_t *n);
 
 /* replaces: MapEval::calculateMetricsWithInitialMatrix (map_eval.cpp:1204-1260), getDiffRegResultWithCorrespondence
- * (:1069-1145), the metric half of calculateMetrics (:1147-1202) and computeChamferDistance (:1398-1431). */
+ * (:1069-1145), the metric half of calculateMetrics (:1147-1202) and computeChamferDistance (:1398-1431).
+ * me_eval_nn_accum: this rank's accumulators of the requested directions (the others zeroed), through the accumulator
+ * block: it overwrites the block's NN sections of those directions, the sections me_eval_nn_accum_device writes. */
 ME_API int  me_eval_nn_accum(me_ctx *ctx, const me_nn_params *p, me_nn_accum *est_to_gt, me_nn_accum *gt_to_est);
 ME_API int  me_nn_finalize(const me_nn_params *p, const me_nn_accum *est_to_gt, const me_nn_accum *gt_to_est,
                     int64_t n_est, int64_t n_gt, me_nn_result *out);      /* host only, no device work */
@@ -458,7 +461,9 @@ ME_API int  me_quantile_finalize(int64_t n, const double *p, int32_t n_probs, co
 
 /* replaces: ComputeMeanMapEntropyUsingNormalTBB / ...UsingNormal (min_neighbors 10, map_eval.cpp:1608-1737, 1538-1606),
  * ComputeMeanMapEntropy (min_neighbors 5, :1438-1535), ComputeEntropy (:1433-1436) and the min/max side effect of
- * ColorPointCloudByMME (:697-701).  entropies_host (nullable) receives N fp64, zeros where invalid. */
+ * ColorPointCloudByMME (:697-701).  entropies_host (nullable) receives N fp64, zeros where invalid.
+ * me_eval_mme_accum goes through the accumulator block: it overwrites the MME section of cloud `which`, the section
+ * me_eval_mme_accum_device writes for that cloud. */
 ME_API int  me_eval_mme_accum(me_ctx *ctx, int which, double radius, int32_t min_neighbors, me_mme_accum *out);
 ME_API int  me_mme_finalize(const me_mme_accum *acc, int64_t n_total, me_mme_result *out);   /* host only */
 ME_API int  me_eval_mme(me_ctx *ctx, int which, double radius, int32_t min_neighbors, me_mme_result *out,
@@ -467,7 +472,9 @@ ME_API int  me_get_entropies(me_ctx *ctx, int which, double *entropies_host);
 
 /* Device-resident accumulators, for multi-GPU passes without host round trips: me_accum_reset clears the context's
  * accumulator block; the *_device calls run the same sweeps as me_eval_nn_accum / me_eval_mme_accum but leave the partial
- * accumulators in that block (fp64; counts ride as fp64, exact below 2^53); me_accum_block hands out its DEVICE address:
+ * accumulators in that block (fp64; counts ride as fp64, exact below 2^53) — each call writes only its own sections (NN: those of
+ * the evaluated directions; MME: the cloud's), as do me_eval_nn_accum / me_eval_mme_accum, so a section survives calls that
+ * write other sections; me_accum_block hands out its DEVICE address:
  * the first *n_sum values are SUM-reducible, the following *n_max values MAX-reducible (entropy maximum and negated
  * minimum per cloud) — the caller all-reduces them in place (ncclAllReduce / torch.distributed on the context's stream);
  * me_accum_fetch copies the block back ONCE and fills the accumulator structs (any of them may be NULL), ready for

@@ -1,6 +1,6 @@
 """N > 1 host logic on CPU: world_size-2 (and 3) gloo processes each own a shard of the queries, build the partial
-accumulators for it, all-reduce them through cloud_map_evaluation_b200.dist and finalise with the library's host-only
-me_nn_finalize / me_mme_finalize.  The result must equal the unsharded oracle run (counts exactly)."""
+accumulators for it, all-reduce them and finalise with the library's host-only me_nn_finalize / me_mme_finalize.  The
+result must equal the unsharded oracle run (counts exactly)."""
 import ctypes as C
 import os
 import socket
@@ -39,6 +39,21 @@ def _partial_nn(query, ref, qb, qe, tau, R, slot=None):
     return a
 
 
+def _allreduce(nn_e, nn_g, m):
+    """the partial accumulators of every rank, reduced in place: SUM of each NN struct's int64 and fp64 fields and of the MME
+    counts and entropy sum, MAX / MIN of the entropy extrema"""
+    def field_sum(ctype, n, obj, offset=0):
+        dist.all_reduce(torch.from_numpy(np.ctypeslib.as_array((ctype * n).from_buffer(obj, offset))))
+    for a in (nn_e, nn_g):
+        field_sum(C.c_int64, A.ME_NN_ACCUM_I64, a)
+        field_sum(C.c_double, A.ME_NN_ACCUM_F64, a, 8 * A.ME_NN_ACCUM_I64)
+    field_sum(C.c_int64, 2, m)
+    t = torch.tensor([m.sum_entropy, m.min_entropy, m.max_entropy], dtype=torch.float64)
+    for op, sl in ((dist.ReduceOp.SUM, t[0:1]), (dist.ReduceOp.MIN, t[1:2]), (dist.ReduceOp.MAX, t[2:3])):
+        dist.all_reduce(sl, op=op)
+    m.sum_entropy, m.min_entropy, m.max_entropy = t.tolist()
+
+
 def _worker(rank, world, port, out_dir, moments=False):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     dist.init_process_group("gloo", rank=rank, world_size=world)
@@ -60,7 +75,7 @@ def _worker(rank, world, port, out_dir, moments=False):
         nz = mine[mine != 0]
         m.n_query, m.n_valid, m.sum_entropy = len(mine), int((mine != 0).sum()), float(mine.sum())
         m.min_entropy, m.max_entropy = (float(nz.min()), float(nz.max())) if len(nz) else (np.inf, -np.inf)
-        mdist.allreduce_accumulators(nn_e, nn_g, [m])
+        _allreduce(nn_e, nn_g, m)
         res = A.me_nn_result()
         assert L.me_nn_finalize(C.byref(p), C.byref(nn_e), C.byref(nn_g), len(est), len(gt), C.byref(res)) == 0
         mres = A.me_mme_result()
@@ -86,7 +101,10 @@ def _worker(rank, world, port, out_dir, moments=False):
 
 
 @pytest.mark.parametrize("world", [2, 3])
-def test_sharded_accumulators_allreduce_gloo(world, tmp_path):
+def test_sharded_partials_finalize_to_the_unsharded_result_gloo(world, tmp_path):
+    """partial accumulators of each rank's shard, summed over the ranks: me_nn_finalize / me_mme_finalize give the
+    unsharded result"""
+    assert mdist.shard_range(10, 0, 3) == (0, 3) and mdist.shard_range(10, 2, 3) == (6, 10)
     if not os.path.exists(_lib.LIB_PATH):
         import __graft_entry__ as g
         g.build()
@@ -101,8 +119,8 @@ def test_sharded_accumulators_allreduce_gloo(world, tmp_path):
 
 
 @pytest.mark.parametrize("world", [2, 3])
-def test_sharded_moments_allreduce_gloo(world, tmp_path):
-    """the per-rank (n, mean, M2) slots through the same single SUM all-reduce: me_nn_finalize merges them into sigma"""
+def test_sharded_moment_slots_merge_in_finalize_gloo(world, tmp_path):
+    """the per-rank (n, mean, M2) slots through the same SUM over the ranks: me_nn_finalize merges them into sigma"""
     if not os.path.exists(_lib.LIB_PATH):
         import __graft_entry__ as g
         g.build()
@@ -113,23 +131,6 @@ def test_sharded_moments_allreduce_gloo(world, tmp_path):
         port = s.getsockname()[1]
     mp.spawn(_worker, args=(world, port, str(tmp_path), True), nprocs=world, join=True)
     assert os.path.exists(tmp_path / "ok")
-
-def test_pack_unpack_roundtrip():
-    a, b, m = A.me_nn_accum(), A.me_nn_accum(), A.me_mme_accum()
-    rng = np.random.RandomState(0)
-    for acc in (a, b):
-        acc.n_query, acc.n_corr, acc.n_ub, acc.n_far = [int(x) for x in rng.randint(0, 1 << 40, 4)]
-        for k in range(5):
-            acc.n_inlier[k] = int(rng.randint(0, 1 << 40))
-            acc.sum_d[k], acc.sum_d2[k] = rng.rand(2)
-        acc.sum_d_all, acc.sum_d2_all, acc.sum_nn_dist = rng.rand(3)
-    m.n_query, m.n_valid, m.sum_entropy, m.min_entropy, m.max_entropy = 10, 7, -55.5, -9.0, -6.0
-    packed = mdist.pack(a, b, [m])
-    assert len(packed[0]) == 2 * A.ME_NN_ACCUM_I64 + 2 and len(packed[1]) == 2 * A.ME_NN_ACCUM_F64 + 1
-    a2, b2, m2 = A.me_nn_accum(), A.me_nn_accum(), A.me_mme_accum()
-    mdist.unpack(*packed, a2, b2, [m2])
-    assert bytes(a) == bytes(a2) and bytes(b) == bytes(b2) and bytes(m) == bytes(m2)
-    assert mdist.shard_range(10, 0, 3) == (0, 3) and mdist.shard_range(10, 2, 3) == (6, 10)
 
 
 # ---------------------------------------------------------------------------------------------------------------

@@ -520,7 +520,8 @@ def test_small_lattice_budget(api, O):
 
 
 def test_device_resident_accumulators_equal_the_host_path(api, O):
-    """me_eval_*_accum_device + me_accum_fetch (what bench.py and the multi-GPU pass use) = me_eval_*_accum"""
+    """me_eval_*_accum_device + me_accum_fetch (what bench.py and the multi-GPU pass use) = me_eval_*_accum; a *_device MME
+    section survives a later me_eval_nn_accum, which writes only the NN sections of the block"""
     est, gt, cfg = synth.make_pair("C2", scale=0.1)
     p = A.make_nn_params(cfg["tau"], 1.0)
     with _ctx(api, est, gt, vmd_voxel_size=cfg["vmd_voxel_size"]) as ctx:
@@ -530,6 +531,8 @@ def test_device_resident_accumulators_equal_the_host_path(api, O):
         ctx.accum_reset()
         ctx.eval_mme_accum_device(A.ME_CLOUD_EST, cfg["nn_radius"], 10)
         ctx.eval_mme_accum_device(A.ME_CLOUD_GT, cfg["nn_radius"], 5)
+        ctx.eval_nn_accum(p)
+        _, _, (m_e3, m_g3) = ctx.accum_fetch(want_mme=(True, True))
         ctx.eval_nn_accum_device(p)
         ptr, n_sum, n_max = ctx.accum_block()
         assert ptr and n_sum == 2 * (A.ME_NN_ACCUM_I64 + A.ME_NN_ACCUM_F64) + 14 and n_max == 4
@@ -541,7 +544,7 @@ def test_device_resident_accumulators_equal_the_host_path(api, O):
         for k in ("sum_d", "sum_d2", "sum_d_all", "sum_d2_all", "sum_nn_dist", "rank_mean", "rank_m2"):
             np.testing.assert_allclose(da[k], db[k], rtol=1e-12)
         assert da["rank_n"] == db["rank_n"] == [da["n_corr"]] + [0.0] * (A.ME_MAX_WORLD - 1)
-    for a, b in ((m_e, m_e2), (m_g, m_g2)):
+    for a, b in ((m_e, m_e2), (m_g, m_g2), (m_e, m_e3), (m_g, m_g3)):
         assert (a.n_query, a.n_valid) == (b.n_query, b.n_valid)
         np.testing.assert_allclose([a.sum_entropy, a.min_entropy, a.max_entropy], [b.sum_entropy, b.min_entropy, b.max_entropy], rtol=1e-12)
 
