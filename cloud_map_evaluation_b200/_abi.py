@@ -155,6 +155,24 @@ class me_quantile_result(C.Structure):
                 ("est_to_gt", me_quantile_dir), ("gt_to_est", me_quantile_dir), ("hausdorff", C.c_double)]
 
 
+# AC / COM / CD / F1 / IoU per region (me_nn_region*)
+ME_REGION_MAX_REGIONS = 1 << 21
+ME_REGION_SUM_FIELDS = 18      # per region and direction: n_query n_corr n_inlier[5] sum_d[5] sum_d2[5] sum_nn_dist
+ME_REGION_MAX_FIELDS = 2       # per region and direction: max_d max_nn
+
+
+class me_region_dir(C.Structure):
+    _fields_ = [("n_query", C.c_int64), ("n_corr", C.c_int64), ("n_inlier", C.c_int64 * 5), ("sum_d", C.c_double * 5),
+                ("sum_d2", C.c_double * 5), ("sum_nn_dist", C.c_double), ("max_d", C.c_double), ("max_nn", C.c_double),
+                ("mean", C.c_double * 5), ("rmse", C.c_double * 5), ("fitness", C.c_double * 5), ("mean_nn", C.c_double)]
+
+
+class me_region_row(C.Structure):
+    _fields_ = [("index", C.c_int64 * 3), ("min", C.c_double * 3), ("max", C.c_double * 3), ("n_est", C.c_int64),
+                ("n_gt", C.c_int64), ("est_to_gt", me_region_dir), ("gt_to_est", me_region_dir), ("cd", C.c_double * 5),
+                ("f1", C.c_double * 5), ("iou", C.c_double * 5)]
+
+
 class me_mme_accum(C.Structure):
     _fields_ = [("n_query", C.c_int64), ("n_valid", C.c_int64), ("sum_entropy", C.c_double),
                 ("min_entropy", C.c_double), ("max_entropy", C.c_double)]

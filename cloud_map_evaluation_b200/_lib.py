@@ -27,6 +27,7 @@ SYMBOLS = (
     "me_nn_curve_accum_device", "me_nn_curve_finalize", "me_nn_curve",
     "me_nn_quantile_begin", "me_nn_quantile_block", "me_nn_quantile_step", "me_nn_quantile_end", "me_nn_quantiles",
     "me_quantile_finalize",
+    "me_nn_region_begin", "me_nn_region_block", "me_nn_region_end", "me_nn_regions", "me_region_finalize",
 )
 
 _lib = None
@@ -124,6 +125,12 @@ def load():
     L.me_nn_quantile_end.argtypes = [ctx, C.POINTER(A.me_quantile_result)]
     L.me_nn_quantiles.argtypes = [ctx, C.c_int32, dp, C.c_int32, C.POINTER(A.me_quantile_result)]
     L.me_quantile_finalize.argtypes = [C.c_int64, dp, C.c_int32, dp, dp]
+    i64p = C.POINTER(C.c_int64)
+    L.me_nn_region_begin.argtypes = [ctx, C.c_double, i64p]
+    L.me_nn_region_block.argtypes = [ctx, C.POINTER(dp), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    L.me_nn_region_end.argtypes = [ctx, C.POINTER(A.me_region_row), C.c_int64]
+    L.me_nn_regions.argtypes = [ctx, C.c_double, C.POINTER(C.POINTER(A.me_region_row)), i64p]
+    L.me_region_finalize.argtypes = [C.c_int64, C.c_double, i64p, i64p, i64p, dp, C.POINTER(A.me_region_row)]
     L.me_kernel_trace.argtypes = [ctx, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.c_int32]
     if L.me_abi_version() != A.ME_ABI_VERSION:
         raise RuntimeError("libmapeval_b200.so ABI version mismatch")

@@ -104,6 +104,51 @@ def quantile_dict(res):
     return out
 
 
+_REGION_DIR_DT = np.dtype([("n_query", "<i8"), ("n_corr", "<i8"), ("n_inlier", "<i8", 5), ("sum_d", "<f8", 5), ("sum_d2", "<f8", 5),
+                           ("sum_nn_dist", "<f8"), ("max_d", "<f8"), ("max_nn", "<f8"), ("mean", "<f8", 5), ("rmse", "<f8", 5),
+                           ("fitness", "<f8", 5), ("mean_nn", "<f8")])
+# me_region_row as a numpy record (8-byte fields only, so no padding): the rows convert without a per-row Python step
+_REGION_ROW_DT = np.dtype([("index", "<i8", 3), ("min", "<f8", 3), ("max", "<f8", 3), ("n_est", "<i8"), ("n_gt", "<i8"),
+                           ("est_to_gt", _REGION_DIR_DT), ("gt_to_est", _REGION_DIR_DT), ("cd", "<f8", 5), ("f1", "<f8", 5),
+                           ("iou", "<f8", 5)])
+assert _REGION_ROW_DT.itemsize == C.sizeof(A.me_region_row) and _REGION_DIR_DT.names == tuple(f[0] for f in A.me_region_dir._fields_)
+
+
+def region_dict(a):
+    """me_region_row records (numpy, _REGION_ROW_DT) -> {'index' (n, 3) int64, 'min' / 'max' (n, 3), 'n_est', 'n_gt',
+    'cd' / 'f1' / 'iou' (n, 5), 'est_to_gt' / 'gt_to_est': {field: array}}, one entry per field"""
+    out = {name: np.array(a[name]) for name in ("index", "min", "max", "n_est", "n_gt", "cd", "f1", "iou")}
+    for name in ("est_to_gt", "gt_to_est"):
+        out[name] = {f: np.array(a[name][f]) for f in _REGION_DIR_DT.names}
+    return out
+
+
+def _region_rows(n):
+    """zeroed records for n rows and the pointer the C-ABI takes"""
+    rows = np.zeros(max(int(n), 1), _REGION_ROW_DT)
+    return rows, rows.ctypes.data_as(C.POINTER(A.me_region_row))
+
+
+def region_finalize(region_size, index, n_est, n_gt, block):
+    """me_region_finalize (host only): the rows of n regions from a reduced host block (ME_REGION_SUM_FIELDS x 2 SUM values per
+    region, then ME_REGION_MAX_FIELDS x 2 MAX values), index (n, 3) and the per-region point counts; as region_dict"""
+    L = _lib.load()
+    idx = np.ascontiguousarray(index, dtype=np.int64).reshape(-1, 3)
+    n = idx.shape[0]
+    ne = np.ascontiguousarray(n_est, dtype=np.int64).reshape(-1)
+    ng = np.ascontiguousarray(n_gt, dtype=np.int64).reshape(-1)
+    blk = np.ascontiguousarray(block, dtype=np.float64).reshape(-1)
+    if ne.size != n or ng.size != n or blk.size != 2 * (A.ME_REGION_SUM_FIELDS + A.ME_REGION_MAX_FIELDS) * n:
+        raise ValueError("one index triple, one n_est / n_gt and 2 x (ME_REGION_SUM_FIELDS + ME_REGION_MAX_FIELDS) values per region")
+    rows, rows_p = _region_rows(n)
+    i64 = C.POINTER(C.c_int64)
+    rc = L.me_region_finalize(n, float(region_size), idx.ctypes.data_as(i64), ne.ctypes.data_as(i64), ng.ctypes.data_as(i64),
+                              blk.ctypes.data_as(C.POINTER(C.c_double)), rows_p)
+    if rc != A.ME_OK:
+        raise MapEvalError(rc, "me_region_finalize: n >= 0, region_size finite and > 0")
+    return region_dict(rows[:n])
+
+
 class MapEvalB200:
     """One context = one GPU.  rank/world select this context's contiguous query range (multi-GPU sharding)."""
 
@@ -406,6 +451,41 @@ class MapEvalB200:
         out = A.me_quantile_result()
         self._check(self._L.me_nn_quantile_end(self._ctx, C.byref(out)))
         return quantile_dict(out)
+
+    def region_errors(self, region_size):
+        """AC / COM / CD / F1 / IoU per occupied region floor(x / region_size) of the last NN evaluation's records, both
+        directions (me_nn_regions, world 1).  Returns region_dict's dict of arrays, rows ascending by (ix, iy, iz).
+        Multi-GPU: dist.regions_distributed."""
+        rows = C.POINTER(A.me_region_row)()
+        n = C.c_int64(0)
+        self._check(self._L.me_nn_regions(self._ctx, float(region_size), C.byref(rows), C.byref(n)))
+        try:
+            nb = n.value * _REGION_ROW_DT.itemsize
+            a = np.frombuffer((C.c_char * nb).from_address(C.addressof(rows.contents)), _REGION_ROW_DT) if nb else \
+                np.zeros(0, _REGION_ROW_DT)
+            return region_dict(a.copy())
+        finally:
+            self._L.me_free(rows)
+
+    def region_begin(self, region_size):
+        """me_nn_region_begin: lists the occupied regions and folds this rank's records; returns the region count"""
+        n = C.c_int64(0)
+        self._check(self._L.me_nn_region_begin(self._ctx, float(region_size), C.byref(n)))
+        return n.value
+
+    def region_block(self):
+        """(device pointer, n_sum, n_max) of the block: SUM-reduce its first n_sum values and MAX-reduce the next n_max in place
+        (after synchronize())"""
+        ptr = C.POINTER(C.c_double)()
+        n_sum, n_max = C.c_int32(0), C.c_int32(0)
+        self._check(self._L.me_nn_region_block(self._ctx, C.byref(ptr), C.byref(n_sum), C.byref(n_max)))
+        return C.cast(ptr, C.c_void_p).value, n_sum.value, n_max.value
+
+    def region_end(self, n_regions):
+        """the rows from the reduced block, as region_errors"""
+        rows, rows_p = _region_rows(n_regions)
+        self._check(self._L.me_nn_region_end(self._ctx, rows_p, int(n_regions)))
+        return region_dict(rows[:int(n_regions)])
 
     def get_nn(self, which_query):
         n = self.n[which_query]

@@ -231,6 +231,7 @@ void me_destroy(me_ctx *ctx) {
   if (ctx->stream) cudaStreamSynchronize(ctx->stream);
   icp_close(ctx, false);
   nn_quantile_free(ctx);
+  nn_region_free(ctx);
   if (ctx->copy_stream) { cudaStreamSynchronize(ctx->copy_stream); cudaStreamDestroy(ctx->copy_stream); }
   if (ctx->compute_mark) cudaEventDestroy(ctx->compute_mark);
   for (Cloud &c : ctx->cloud) free_cloud(c);
@@ -920,6 +921,87 @@ int me_nn_quantiles(me_ctx *ctx, int32_t population, const double *p, int32_t n_
   int32_t done = 0;
   while (!done) ME_TRY(me_nn_quantile_step(ctx, &done));
   return me_nn_quantile_end(ctx, out);
+}
+
+int me_region_finalize(int64_t n_regions, double region_size, const int64_t *index, const int64_t *n_est, const int64_t *n_gt,
+                       const double *host_block, me_region_row *rows) {
+  if (n_regions < 0 || !(std::isfinite(region_size) && region_size > 0.0)) return ME_ERR_INVALID;
+  if (n_regions > 0 && (!index || !n_est || !n_gt || !host_block || !rows)) return ME_ERR_INVALID;
+  const int F = ME_REGION_SUM_FIELDS;
+  const double *mx = host_block + (size_t)2 * F * n_regions;
+  me_nn_accum none;
+  std::memset(&none, 0, sizeof(none));
+  for (int64_t r = 0; r < n_regions; ++r) {
+    me_region_row &R = rows[r];
+    std::memset(&R, 0, sizeof(R));
+    for (int a = 0; a < 3; ++a) {
+      R.index[a] = index[3 * r + a];
+      R.min[a] = (double)R.index[a] * region_size;
+      R.max[a] = (double)(R.index[a] + 1) * region_size;
+    }
+    R.n_est = n_est[r];
+    R.n_gt = n_gt[r];
+    for (int q = 0; q < 2; ++q) {
+      const double *v = host_block + ((size_t)r * 2 + q) * F;
+      me_region_dir &D = q == 0 ? R.est_to_gt : R.gt_to_est;
+      D.n_query = (int64_t)v[0];
+      D.n_corr = (int64_t)v[1];
+      for (int k = 0; k < 5; ++k) { D.n_inlier[k] = (int64_t)v[2 + k]; D.sum_d[k] = v[7 + k]; D.sum_d2[k] = v[12 + k]; }
+      D.sum_nn_dist = v[17];
+      D.max_d = mx[((size_t)r * 2 + q) * ME_REGION_MAX_FIELDS];
+      D.max_nn = mx[((size_t)r * 2 + q) * ME_REGION_MAX_FIELDS + 1];
+      // no sigma per region (DESIGN §3.12): dir_level's sigma output is dropped, so the moments it would read do not matter
+      const DirMoments M{&none, (double)D.n_corr, true, 0.0, 0.0};
+      double sigma;
+      for (int k = 0; k < 5; ++k)
+        dir_level(M, D.n_inlier[k], D.sum_d[k], D.sum_d2[k], q == 0 ? R.n_est : R.n_gt, &D.mean[k], &D.rmse[k], &D.fitness[k], &sigma);
+      D.mean_nn = D.sum_nn_dist / (double)D.n_query;
+    }
+    for (int k = 0; k < 5; ++k)
+      pair_level(R.est_to_gt.fitness[k], R.est_to_gt.rmse[k], R.est_to_gt.n_inlier[k], R.gt_to_est.rmse[k], R.n_est, R.n_gt, &R.cd[k],
+                 &R.f1[k], &R.iou[k]);
+  }
+  return ME_OK;
+}
+
+int me_nn_region_begin(me_ctx *ctx, double region_size, int64_t *n_regions) {
+  ME_ENTER(ctx);
+  if (!n_regions) return fail(ctx, ME_ERR_INVALID, "null argument");
+  if (!(std::isfinite(region_size) && region_size > 0.0)) return fail(ctx, ME_ERR_INVALID, "me_nn_region*: region_size must be finite and > 0");
+  return nn_region_begin(ctx, region_size, n_regions);
+}
+
+int me_nn_region_block(me_ctx *ctx, double **device_block, int32_t *n_sum, int32_t *n_max) {
+  ME_ENTER(ctx);
+  if (!device_block || !n_sum || !n_max) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return nn_region_block(ctx, device_block, n_sum, n_max);
+}
+
+int me_nn_region_end(me_ctx *ctx, me_region_row *rows, int64_t capacity) {
+  ME_ENTER(ctx);
+  if (!rows) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return nn_region_end(ctx, rows, capacity);
+}
+
+int me_nn_regions(me_ctx *ctx, double region_size, me_region_row **rows, int64_t *n_regions) {
+  ME_ENTER(ctx);
+  if (!rows || !n_regions) return fail(ctx, ME_ERR_INVALID, "null argument");
+  *rows = nullptr;
+  *n_regions = 0;
+  if (ctx->world != 1)
+    return fail(ctx, ME_ERR_INVALID, "me_nn_regions needs world == 1; use me_nn_region_begin / _block + all-reduce / _end");
+  int64_t n = 0;
+  ME_TRY(me_nn_region_begin(ctx, region_size, &n));
+  me_region_row *r = (me_region_row *)std::malloc((size_t)std::max<int64_t>(n, 1) * sizeof(me_region_row));
+  if (!r) return fail(ctx, ME_ERR_NOMEM, "me_nn_regions: host allocation of the rows failed");
+  const int rc = me_nn_region_end(ctx, r, n);
+  if (rc != ME_OK) {
+    std::free(r);
+    return rc;
+  }
+  *rows = r;
+  *n_regions = n;
+  return ME_OK;
 }
 
 int me_eval_nn(me_ctx *ctx, const me_nn_params *p, me_nn_result *out) {

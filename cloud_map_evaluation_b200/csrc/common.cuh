@@ -193,6 +193,20 @@ struct QuantRun {
   std::vector<double> h_blk;
 };
 
+// the per-region table (me_nn_region_begin .. me_nn_region_end, region.cu): the occupied list and the block, the same
+// length on every rank
+struct RegionRun {
+  bool open = false;
+  unsigned long long gen = 0;          // cloud_gen at me_nn_region_begin
+  double s = 0.0;
+  long long n = 0;                     // occupied regions
+  std::vector<int64_t> index, n_est, n_gt;   // 3 per region; per region
+  double *d_blk = nullptr;             // SUM part (ME_REGION_SUM_FIELDS x 2 per region), then MAX part (ME_REGION_MAX_FIELDS x 2)
+  long long cap_blk = 0;
+  double *d_part = nullptr;            // the fold's per-chunk values
+  long long cap_part = 0;
+};
+
 // numpy's method="linear" position of probability p among n sorted values: h = (n - 1) p, k = floor(h), g = h - k
 inline void quantile_rank(long long n, double p, long long *k, double *g) {
   const double h = (double)(n - 1) * p;
@@ -275,6 +289,7 @@ struct me_ctx {
   double *d_curve = nullptr;           // the curve block (both directions), then the levels
   long long cap_curve = 0;
   me::QuantRun quant;                  // distance quantiles (me_nn_quantile*), from the same records
+  me::RegionRun region;                // the per-region table (me_nn_region*), from the same records
   std::string err;
 };
 
@@ -384,6 +399,11 @@ int nn_quantile_block(me_ctx *ctx, double **device_block, int32_t *n);
 int nn_quantile_step(me_ctx *ctx, int32_t *done);
 int nn_quantile_end(me_ctx *ctx, me_quantile_result *out);
 void nn_quantile_free(me_ctx *ctx);
+// the per-region table of the last me_eval_nn*'s records (region_size checked by the caller) — me_nn_region_* (region.cu)
+int nn_region_begin(me_ctx *ctx, double s, int64_t *n_regions);
+int nn_region_block(me_ctx *ctx, double **device_block, int32_t *n_sum, int32_t *n_max);
+int nn_region_end(me_ctx *ctx, me_region_row *rows, int64_t capacity);
+void nn_region_free(me_ctx *ctx);
 // the accumulators go to the cloud's MME section of d_block
 int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors);
 

@@ -18,6 +18,7 @@
 //   nn_tile_kernel   lattices the flat kernel cannot index (>= 2^24 cells along x or points per run): one CTA per
 //                    4x4x4-cell query tile, 6x6x6-cell region staged with TMA bulk copies.  ME_NN_TILE (env) forces it.
 #include "common.cuh"
+#include "records.cuh"
 #include "tile.cuh"
 #include "flat.cuh"
 #include <algorithm>
@@ -27,19 +28,6 @@
 namespace me {
 
 static constexpr int kThreads = 256;
-
-struct NNConst {
-  double tau[5];
-  double cutoff;        // R (mode 0) or R*R (mode 1)
-  int cutoff_mode;
-  int accumulate;       // accumulate pair statistics in the sweep (0 for ME_PAIRING_AS_WRITTEN gt->est)
-  int want_full_cd;
-  double max_d2;        // nothing beyond this squared distance matters (inf when full CD is wanted)
-  double ref_maxabs;    // max |coordinate| of the reference cloud (slack of the face test)
-  // slab layout: only the planes [cov_lo, cov_hi) of the reference lattice along axis cov_axis (1: y, 2: z; 0: everything)
-  // are laid out on this rank
-  int cov_axis, cov_lo, cov_hi, cov_dim;
-};
 
 // distance (in cells) from lattice coordinate (uy, uz) to the nearest plane of the reference lattice that is NOT laid out on
 // this rank: beyond it the cloud is unknown, not empty
@@ -78,25 +66,6 @@ struct LocalAcc {
   __device__ __forceinline__ void nn_dist(double d) { sum_nn += d; }
   __device__ __forceinline__ void ub() { n_ub++; }
 };
-
-
-__device__ __forceinline__ bool keep_pair(double d2, const NNConst &c) {
-  return c.cutoff_mode == ME_CUTOFF_SQDIST_LE_R ? (d2 <= c.cutoff) : (d2 < c.cutoff);
-}
-
-// the distance d of a kept pair, map_eval.cpp:1095: sqrt of Eigen's squaredNorm
-__device__ __forceinline__ double pair_dist(double sq) { return __dsqrt_rn(sq); }
-
-// map_eval.cpp:1095-1123 for one kept pair (source - target)
-// sq = Eigen's squaredNorm of (source - target), x*x + (y*y + z*z)
-template <class Acc>
-__device__ __forceinline__ void accum_sq(double sq, const NNConst &c, Acc &a) {
-  double nd = pair_dist(sq);
-  a.pair(nd, sq);
-#pragma unroll
-  for (int k = 0; k < 5; ++k)
-    if (nd <= c.tau[k]) a.inlier(k, nd, sq);
-}
 
 // (n, mean, M2) of the whole block from every thread's (n, mean, M2), valid in thread 0; every thread of the block calls it
 __device__ void block_moments(double &n, double &m, double &m2) {
@@ -854,30 +823,8 @@ nn_stats_kernel(long long i_begin, long long i_end, const int32_t *__restrict__ 
   flush_acc(a, acc, mom);
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// ME_PAIRING_AS_WRITTEN: map_eval.cpp:1233 stores (nn_est, i_gt); :1241 passes (source = gt, target = est), so
-// :1093-1094 reads gt[nn_est] and est[i_gt].  Reproduced verbatim; out-of-range (UB in the reference) is counted.
-// Walks every gt point; points this rank did not evaluate carry the marker -2.
-// ---------------------------------------------------------------------------------------------------------------
-enum { kAwNone = 0, kAwOutOfRange = 1, kAwPair = 2 };
-// gt query i (sorted order): kAwNone (no kept pair), kAwOutOfRange (counted in n_ub) or kAwPair with sq = Eigen's
-// squaredNorm of gt[nn_est] - est[i_gt]
-__device__ __forceinline__ int as_written_pair(const P4 *__restrict__ Qgt, long long i, const int32_t *__restrict__ nn_idx,
-                                               const double *__restrict__ nn_d2, const double *__restrict__ gt_xyz, long long n_gt,
-                                               const double *__restrict__ est_xyz, long long n_est, const NNConst &C, double &sq) {
-  const int32_t nn_est = nn_idx[i];
-  if (nn_est < 0) return kAwNone;
-  if (!keep_pair(nn_d2[i], C)) return kAwNone;
-  const long long i_gt = orig_of(__double_as_longlong(__ldg(reinterpret_cast<const double *>(Qgt + i) + 3)));
-  const long long s = nn_est, t = i_gt;          // source index into gt, target index into est
-  if (s >= n_gt || t >= n_est) return kAwOutOfRange;
-  const double dx = __dsub_rn(__ldg(gt_xyz + 3 * s), __ldg(est_xyz + 3 * t));
-  const double dy = __dsub_rn(__ldg(gt_xyz + 3 * s + 1), __ldg(est_xyz + 3 * t + 1));
-  const double dz = __dsub_rn(__ldg(gt_xyz + 3 * s + 2), __ldg(est_xyz + 3 * t + 2));
-  sq = sqnorm_eigen(dx, dy, dz);
-  return kAwPair;
-}
-
+// ME_PAIRING_AS_WRITTEN gt->est (as_written_pair, records.cuh).  Walks every gt point; points this rank did not evaluate
+// carry the marker -2.
 __global__ void __launch_bounds__(kThreads, 4)      // as nn_stats_kernel
 pair_as_written_kernel(const P4 *__restrict__ Qgt, long long n, const int32_t *__restrict__ nn_idx,
                        const double *__restrict__ nn_d2, const double *__restrict__ gt_xyz, long long n_gt,
@@ -905,31 +852,6 @@ pair_as_written_kernel(const P4 *__restrict__ Qgt, long long n, const int32_t *_
 // ---------------------------------------------------------------------------------------------------------------
 static constexpr int kCurveThreads = 256;
 static constexpr int kCurveWarps = kCurveThreads / 32;
-
-struct CurveSrc {           // the per-query records of one direction
-  long long b, e;           // sorted range the sweep filled (entries < 0 in it: no neighbour / another rank's query)
-  const int32_t *nn_idx;
-  const double *nn_d2, *nn_sq;
-  int as_written;           // ME_PAIRING_AS_WRITTEN gt->est: the distance comes from the swapped indices
-  const P4 *Qgt;
-  const double *gt_xyz, *est_xyz;
-  long long n_gt, n_est;
-};
-
-// the kept-pair rule of the five-level pass on record i of S (me_nn_curve* and me_nn_quantile* share it): true with sq = the
-// pair's squared norm, whose pair_dist is d; an out-of-range ME_PAIRING_AS_WRITTEN pair adds one to ub and is not kept
-__device__ __forceinline__ bool kept_record(const CurveSrc &S, const NNConst &C, long long i, double &sq, unsigned int &ub) {
-  if (S.as_written) {
-    const int r = as_written_pair(S.Qgt, i, S.nn_idx, S.nn_d2, S.gt_xyz, S.n_gt, S.est_xyz, S.n_est, C, sq);
-    ub += r == kAwOutOfRange;
-    return r == kAwPair;
-  }
-  if (__ldg(S.nn_idx + i) >= 0 && keep_pair(__ldg(S.nn_d2 + i), C)) {
-    sq = __ldg(S.nn_sq + i);
-    return true;
-  }
-  return false;
-}
 
 // first k in [0, K) with d <= tau[k], K if none (tau non-decreasing)
 __device__ __forceinline__ int curve_bin(const double *tau, int K, double d) {
@@ -1168,7 +1090,7 @@ __global__ void pack_nn_kernel(const AccBlock *__restrict__ a, const unsigned lo
 // ---------------------------------------------------------------------------------------------------------------
 // host driver
 // ---------------------------------------------------------------------------------------------------------------
-static void set_cutoff(NNConst &C, const me_nn_params *p) {
+void set_cutoff(NNConst &C, const me_nn_params *p) {
   C.cutoff_mode = p->cutoff_mode;
   C.cutoff = p->cutoff_mode == ME_CUTOFF_SQDIST_LE_R ? p->icp_max_distance : p->icp_max_distance * p->icp_max_distance;
 }
@@ -1347,7 +1269,7 @@ int run_nn(me_ctx *ctx, const me_nn_params *p, bool pack) {
 
 // the records of the last me_eval_nn* still describe the clouds: no call has changed them since, and every direction that
 // call evaluated holds its records.  `who` names the caller in the message.
-static int nn_records_fresh(me_ctx *ctx, const char *who) {
+int nn_records_fresh(me_ctx *ctx, const char *who) {
   const me_nn_params *p = &ctx->curve_p;
   const int dirs = p->directions ? p->directions : 3;
   bool fresh = ctx->curve_valid && ctx->curve_gen == ctx->cloud_gen;
@@ -1359,7 +1281,7 @@ static int nn_records_fresh(me_ctx *ctx, const char *who) {
 }
 
 // the records of direction q (query cloud q) over the ranges nn_stats_kernel / pair_as_written_kernel walk
-static CurveSrc record_src(const me_ctx *ctx, int q) {
+CurveSrc record_src(const me_ctx *ctx, int q) {
   const me_nn_params *p = &ctx->curve_p;
   const Cloud &Qc = ctx->cloud[q], &Rc = ctx->cloud[1 - q];
   CurveSrc S;

@@ -49,6 +49,23 @@ def allreduce_curve(ctx, tau, device, group=None):
     return t.cpu().numpy().copy()
 
 
+def regions_distributed(ctx, region_size, device, group=None):
+    """AC / COM / CD / F1 / IoU per region over every rank of the job (MapEvalB200.region_errors for world > 1): every rank
+    lists the same occupied regions and folds its own records, then ONE in-place SUM all-reduce of the block's sums (counts
+    ride as fp64, exact) and ONE MAX all-reduce of its maxima.  Every rank returns the same table."""
+    import torch
+    import torch.distributed as dist
+    n = ctx.region_begin(region_size)
+    if dist.is_initialized() and dist.get_world_size(group) > 1:
+        ptr, n_sum, n_max = ctx.region_block()
+        ctx.synchronize()
+        t = torch.as_tensor(_DeviceBlock(ptr, n_sum + n_max), device=device)
+        dist.all_reduce(t[:n_sum], group=group)
+        dist.all_reduce(t[n_sum:], op=dist.ReduceOp.MAX, group=group)
+        torch.cuda.current_stream(device).synchronize()
+    return ctx.region_end(n)
+
+
 def quantiles_distributed(ctx, device, p, population=A.ME_DIST_KEPT, group=None):
     """Exact distance quantiles of the last NN evaluation over every rank of the job (MapEvalB200.distance_quantiles for
     world > 1): the selection loop with ONE in-place SUM all-reduce of the pass's integer counts (as fp64, exact) per pass.

@@ -94,6 +94,9 @@ struct Param {   // map_eval.h:60-116
   // exact distance quantiles at these probabilities and the Hausdorff distance, written to distance_quantiles.txt
   // (me_nn_quantile*: no new sweep); absent or empty = off
   std::vector<double> distance_quantiles_;
+  // AC / COM / CD / F1 / IoU per region floor(x / region_size), written to region_errors.txt (me_nn_region*: no new sweep);
+  // absent or 0 = off.  region_size = vmd_voxel_size lines the rows up with voxel_errors.txt
+  double region_size_ = 0.0;
 };
 
 // map_eval_main.cpp:120-208
@@ -159,6 +162,11 @@ inline Param loadParametersFromYAML(const std::string &yaml_file_path) {
     if (config["distance_quantiles"])
       for (size_t i = 0; i < config["distance_quantiles"].size(); ++i)
         param.distance_quantiles_.push_back(config["distance_quantiles"][i].as<double>());
+    if (config["region_size"]) {
+      param.region_size_ = config["region_size"].as<double>();
+      if (!(std::isfinite(param.region_size_) && param.region_size_ >= 0.0))
+        throw std::runtime_error("region_size must be finite and >= 0 (0 = off), not " + config["region_size"].as<std::string>());
+    }
     return param;
   } catch (const std::exception &e) {
     std::cerr << "Error loading parameters: " << e.what() << std::endl;
@@ -189,7 +197,7 @@ inline void dumpParam(const Param &p, std::ostream &os) {
      << "\naccuracy_curve_steps=" << p.accuracy_curve_steps_ << "\naccuracy_curve_max=" << p.accuracy_curve_max_
      << "\ndistance_quantiles=";
   for (size_t i = 0; i < p.distance_quantiles_.size(); ++i) os << (i ? "," : "") << p.distance_quantiles_[i];
-  os << "\n";
+  os << "\nregion_size=" << p.region_size_ << "\n";
 }
 
 // Eigen's default IOFormat for `vec.transpose()`: coefficients right-aligned to a common width, one space apart
@@ -331,6 +339,7 @@ class MapEvalB200 {
   int renderDistances(bool cutoff_strict);
   int accuracyCurve(const me_nn_params &p, const me_nn_accum &e2g, const me_nn_accum &g2e);
   int distanceQuantiles();
+  int regionErrors();
   GpuGroup gpus_;            // one context per GPU; rank r evaluates the r-th shard of every sweep's query range
   me_ctx *ctx_ = nullptr;    // = gpus_.ctx(0): the voxel stage and the single-GPU calls
   std::vector<double> map_3d_, gt_3d_;   // N x 3 fp64, the layout of open3d PointCloud::points_ (as loaded)
@@ -613,6 +622,7 @@ inline int MapEvalB200::calculateMetricsWithInitialMatrix() {
   t_acc = tic.toc() / 1000.0;
   if (param_.accuracy_curve_steps_ > 0 && accuracyCurve(p, e2g, g2e) != 0) return -1;
   if (!param_.distance_quantiles_.empty() && distanceQuantiles() != 0) return -1;
+  if (param_.region_size_ > 0.0 && regionErrors() != 0) return -1;
   if (nn_.gt_to_est.n_ub > 0)
     std::cerr << "WARNING: " << nn_.gt_to_est.n_ub << " gt->est pairs index past the end of a cloud (the reference reads out of "
                  "bounds there, map_eval.cpp:1233 vs :1093-1094: undefined behaviour); they are left out of the gt->est statistics, "
@@ -712,6 +722,58 @@ inline int MapEvalB200::distanceQuantiles() {
   f << "hausdorff_est_to_gt " << nn.est_to_gt.max << "\nhausdorff_gt_to_est " << nn.gt_to_est.max << "\nhausdorff " << nn.hausdorff << "\n";
   std::cout << "INFO: Hausdorff distance: " << nn.hausdorff << " (est->gt " << nn.est_to_gt.max << ", gt->est " << nn.gt_to_est.max
             << "); distance quantiles saved to " << path << std::endl;
+  return 0;
+}
+
+// per-region table: the pass's NN records split by region floor(x / region_size) (me_nn_region_begin on every GPU, one grouped
+// NCCL SUM all-reduce of the block's sums and one MAX all-reduce of its maxima) -> region_errors.txt next to map_results.txt
+inline int MapEvalB200::regionErrors() {
+  const double s = param_.region_size_;
+  std::vector<int64_t> n(gpus_.size(), 0);
+  std::vector<double *> ptr(gpus_.size(), nullptr), ptr_max(gpus_.size(), nullptr);
+  std::vector<int32_t> n_sum(gpus_.size(), 0), n_max(gpus_.size(), 0);
+  if (gpus_.for_each([&](int r, me_ctx *c) {
+        int rc = me_nn_region_begin(c, s, &n[r]);
+        if (rc == ME_OK) rc = me_nn_region_block(c, &ptr[r], &n_sum[r], &n_max[r]);
+        ptr_max[r] = ptr[r] + n_sum[r];
+        return rc != ME_OK ? rc : me_synchronize(c);
+      }) != ME_OK)
+    return fail("me_nn_region_begin");
+  if (!gpus_.allreduce_device(ptr, (size_t)n_sum[0], ncclSum) || !gpus_.allreduce_device(ptr_max, (size_t)n_max[0], ncclMax))
+    return fail("all-reduce of the region block");
+  std::vector<me_region_row> rows((size_t)n[0]);
+  if (me_nn_region_end(ctx_, rows.data(), n[0]) != ME_OK) return fail("me_nn_region_end");
+  const std::string path = results_subfolder + "region_errors.txt";
+  std::ofstream f(path);
+  if (!f.is_open()) {
+    std::cerr << "ERROR: cannot write " << path << std::endl;
+    return -1;
+  }
+  f << "min_x min_y min_z max_x max_y max_z n_est n_gt";
+  for (const char *d : {"e2g", "g2e"}) {
+    f << " " << d << "_n_corr";
+    for (const char *field : {"n_inlier", "mean", "rmse", "fitness"})
+      for (int k = 1; k <= 5; ++k) f << " " << d << "_" << field << "_" << k;
+    f << " " << d << "_max_d " << d << "_mean_nn";
+  }
+  for (const char *field : {"cd", "f1", "iou"})
+    for (int k = 1; k <= 5; ++k) f << " " << field << "_" << k;
+  f << "\n" << std::fixed << std::setprecision(15);
+  for (const me_region_row &r : rows) {
+    f << r.min[0] << " " << r.min[1] << " " << r.min[2] << " " << r.max[0] << " " << r.max[1] << " " << r.max[2] << " " << r.n_est
+      << " " << r.n_gt;
+    for (const me_region_dir *d : {&r.est_to_gt, &r.gt_to_est}) {
+      f << " " << d->n_corr;
+      for (int k = 0; k < 5; ++k) f << " " << d->n_inlier[k];
+      for (const double *v : {d->mean, d->rmse, d->fitness})
+        for (int k = 0; k < 5; ++k) f << " " << v[k];
+      f << " " << d->max_d << " " << d->mean_nn;
+    }
+    for (const double *v : {r.cd, r.f1, r.iou})
+      for (int k = 0; k < 5; ++k) f << " " << v[k];
+    f << "\n";
+  }
+  std::cout << "INFO: errors of " << n[0] << " regions of edge " << s << " saved to " << path << std::endl;
   return 0;
 }
 
@@ -817,6 +879,7 @@ inline int MapEvalB200::performRegistration() {
   t_acc = tic.toc() / 1000.0;
   if (param_.accuracy_curve_steps_ > 0 && accuracyCurve(p, e2g, g2e) != 0) return -1;
   if (!param_.distance_quantiles_.empty() && distanceQuantiles() != 0) return -1;
+  if (param_.region_size_ > 0.0 && regionErrors() != 0) return -1;
   if (param_.save_immediate_result_ && renderDistances(true) != 0) return -1;
   full_chamfer_dist = nn_.full_cd;
   t_fcd = t_acc;

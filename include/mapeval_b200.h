@@ -459,6 +459,51 @@ ME_API int  me_nn_quantile_end(me_ctx *ctx, me_quantile_result *out);
 ME_API int  me_nn_quantiles(me_ctx *ctx, int32_t population, const double *p, int32_t n_probs, me_quantile_result *out);
 ME_API int  me_quantile_finalize(int64_t n, const double *p, int32_t n_probs, const double *lo_hi, double *values);  /* host only */
 
+/* ---- AC / COM / CD / F1 / IoU per region ----------------------------------------------------------------------------------
+ * From the per-query records of the LAST me_eval_nn* call (stale as for me_nn_curve*), the five-level statistics split by the
+ * region of the query point.  For region edge s (finite, > 0) a point's region is (ix, iy, iz) = floor(x / s) per axis (IEEE
+ * division, as the voxel index of the AWD stage), taken from the clouds as they are now; every index must satisfy
+ * |index| < 2^20 (else ME_ERR_INVALID, naming the axis and the smallest s that fits).  The occupied regions — those holding a
+ * point of either whole cloud — are listed ascending by (ix, iy, iz), at most ME_REGION_MAX_REGIONS (else ME_ERR_INVALID);
+ * the list and n_est / n_gt per region are the same on every rank.  A record counts in the region of its query point and is
+ * kept exactly as the five-level pass keeps it (cut-off modes, ME_PAIRING_AS_WRITTEN gt->est distances).
+ * Device block: n_sum = ME_REGION_SUM_FIELDS * 2 * n_regions SUM-reducible values, [region][direction][field] with the fields
+ *   n_query n_corr n_inlier[5] sum_d[5] sum_d2[5] sum_nn_dist   (counts as fp64; sum_nn_dist only after want_full_cd = 1)
+ * then n_max = ME_REGION_MAX_FIELDS * 2 * n_regions MAX-reducible values, [region][direction][max_d, max_nn] (0 when the set is
+ * empty; max_nn only after want_full_cd = 1).  The same length on every rank.  No floating-point atomics: two calls on the
+ * same device, world and layout give the same bits; counts and maxima are the same for any world and layout.
+ * The loop: me_nn_region_begin lists the regions and folds this rank's records into the block; me_nn_region_block hands the
+ * block out (all-reduce the SUM part with SUM and the MAX part with MAX, in place, after me_synchronize); me_nn_region_end
+ * reads the reduced block and fills rows[0 .. n_regions - 1] (capacity >= n_regions).  A call that changes the clouds between
+ * begin and end makes block and end fail.  me_nn_regions: the whole loop at world 1, rows allocated by the library (me_free).
+ * me_region_finalize (host only): rows from a reduced host block (SUM part, then MAX part), the region indices (3 per region)
+ * and the counts — mean / rmse / fitness per direction and level as me_nn_finalize forms them with n_source = the region's
+ * point count of the query cloud, cd / f1 / iou with the region's n_est / n_gt, mean_nn = sum_nn_dist / n_query.  There is no
+ * sigma per region (DESIGN §3.12). */
+#define ME_REGION_MAX_REGIONS (1 << 21)
+#define ME_REGION_SUM_FIELDS 18
+#define ME_REGION_MAX_FIELDS 2
+typedef struct {
+  int64_t n_query, n_corr, n_inlier[5];
+  double  sum_d[5], sum_d2[5], sum_nn_dist;
+  double  max_d, max_nn;                        /* largest kept d, largest sqrt(d2); 0 for an empty set */
+  double  mean[5], rmse[5], fitness[5];
+  double  mean_nn;                              /* sum_nn_dist / n_query */
+} me_region_dir;
+typedef struct {
+  int64_t index[3];                             /* (ix, iy, iz) */
+  double  min[3], max[3];                       /* index * s, (index + 1) * s */
+  int64_t n_est, n_gt;                          /* points of each whole cloud in the region */
+  me_region_dir est_to_gt, gt_to_est;
+  double  cd[5], f1[5], iou[5];
+} me_region_row;
+ME_API int  me_nn_region_begin(me_ctx *ctx, double region_size, int64_t *n_regions);
+ME_API int  me_nn_region_block(me_ctx *ctx, double **device_block, int32_t *n_sum, int32_t *n_max);
+ME_API int  me_nn_region_end(me_ctx *ctx, me_region_row *rows, int64_t capacity);
+ME_API int  me_nn_regions(me_ctx *ctx, double region_size, me_region_row **rows, int64_t *n_regions);
+ME_API int  me_region_finalize(int64_t n_regions, double region_size, const int64_t *index, const int64_t *n_est,
+                               const int64_t *n_gt, const double *host_block, me_region_row *rows);   /* host only */
+
 /* replaces: ComputeMeanMapEntropyUsingNormalTBB / ...UsingNormal (min_neighbors 10, map_eval.cpp:1608-1737, 1538-1606),
  * ComputeMeanMapEntropy (min_neighbors 5, :1438-1535), ComputeEntropy (:1433-1436) and the min/max side effect of
  * ColorPointCloudByMME (:697-701).  entropies_host (nullable) receives N fp64, zeros where invalid.
