@@ -173,6 +173,20 @@ class me_region_row(C.Structure):
                 ("f1", C.c_double * 5), ("iou", C.c_double * 5)]
 
 
+# drift per region (me_drift*)
+ME_DRIFT_CONVERGED = 0
+ME_DRIFT_ITERATION_LIMIT = 1
+ME_DRIFT_TOO_FEW = 2
+
+
+class me_drift_row(C.Structure):
+    _fields_ = [("index", C.c_int64 * 3), ("min", C.c_double * 3), ("max", C.c_double * 3), ("n_est", C.c_int64),
+                ("n_corr_before", C.c_int64), ("fitness_before", C.c_double), ("rmse_before", C.c_double),
+                ("n_corr", C.c_int64), ("fitness", C.c_double), ("rmse", C.c_double), ("T", C.c_double * 16),
+                ("centroid", C.c_double * 3), ("shift", C.c_double * 3), ("shift_norm", C.c_double), ("angle", C.c_double),
+                ("iterations", C.c_int32), ("status", C.c_int32)]
+
+
 class me_mme_accum(C.Structure):
     _fields_ = [("n_query", C.c_int64), ("n_valid", C.c_int64), ("sum_entropy", C.c_double),
                 ("min_entropy", C.c_double), ("max_entropy", C.c_double)]

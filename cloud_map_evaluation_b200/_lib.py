@@ -28,6 +28,7 @@ SYMBOLS = (
     "me_nn_quantile_begin", "me_nn_quantile_block", "me_nn_quantile_step", "me_nn_quantile_end", "me_nn_quantiles",
     "me_quantile_finalize",
     "me_nn_region_begin", "me_nn_region_block", "me_nn_region_end", "me_nn_regions", "me_region_finalize",
+    "me_drift_begin", "me_drift_block", "me_drift_step", "me_drift_end", "me_drift",
 )
 
 _lib = None
@@ -131,6 +132,11 @@ def load():
     L.me_nn_region_end.argtypes = [ctx, C.POINTER(A.me_region_row), C.c_int64]
     L.me_nn_regions.argtypes = [ctx, C.c_double, C.POINTER(C.POINTER(A.me_region_row)), i64p]
     L.me_region_finalize.argtypes = [C.c_int64, C.c_double, i64p, i64p, i64p, dp, C.POINTER(A.me_region_row)]
+    L.me_drift_begin.argtypes = [ctx, C.c_double, C.c_double, C.c_int32, C.c_double, C.c_double, i64p]
+    L.me_drift_block.argtypes = [ctx, C.POINTER(dp), C.POINTER(C.c_int32)]
+    L.me_drift_step.argtypes = [ctx, C.POINTER(C.c_int32)]
+    L.me_drift_end.argtypes = [ctx, C.POINTER(A.me_drift_row), C.c_int64]
+    L.me_drift.argtypes = [ctx, C.c_double, C.c_double, C.c_int32, C.c_double, C.c_double, C.POINTER(C.POINTER(A.me_drift_row)), i64p]
     L.me_kernel_trace.argtypes = [ctx, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.c_int32]
     if L.me_abi_version() != A.ME_ABI_VERSION:
         raise RuntimeError("libmapeval_b200.so ABI version mismatch")

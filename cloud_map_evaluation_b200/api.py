@@ -149,6 +149,21 @@ def region_finalize(region_size, index, n_est, n_gt, block):
     return region_dict(rows[:n])
 
 
+# me_drift_row as a numpy record (8-byte fields, then two int32: no padding)
+_DRIFT_ROW_DT = np.dtype([("index", "<i8", 3), ("min", "<f8", 3), ("max", "<f8", 3), ("n_est", "<i8"), ("n_corr_before", "<i8"),
+                          ("fitness_before", "<f8"), ("rmse_before", "<f8"), ("n_corr", "<i8"), ("fitness", "<f8"), ("rmse", "<f8"),
+                          ("T", "<f8", 16), ("centroid", "<f8", 3), ("shift", "<f8", 3), ("shift_norm", "<f8"), ("angle", "<f8"),
+                          ("iterations", "<i4"), ("status", "<i4")])
+assert _DRIFT_ROW_DT.itemsize == C.sizeof(A.me_drift_row) and _DRIFT_ROW_DT.names == tuple(f[0] for f in A.me_drift_row._fields_)
+
+
+def drift_dict(a):
+    """me_drift_row records (numpy, _DRIFT_ROW_DT) -> {field: array}, one entry per row field, 'T' as (n, 4, 4)"""
+    out = {name: np.array(a[name]) for name in _DRIFT_ROW_DT.names}
+    out["T"] = out["T"].reshape(-1, 4, 4)
+    return out
+
+
 class MapEvalB200:
     """One context = one GPU.  rank/world select this context's contiguous query range (multi-GPU sharding)."""
 
@@ -486,6 +501,54 @@ class MapEvalB200:
         rows, rows_p = _region_rows(n_regions)
         self._check(self._L.me_nn_region_end(self._ctx, rows_p, int(n_regions)))
         return region_dict(rows[:int(n_regions)])
+
+    def region_drift(self, region_size, max_correspondence_distance, max_iteration=30, relative_fitness=1e-6,
+                     relative_rmse=1e-6):
+        """Aligns every occupied region floor(x / region_size) of the estimated cloud to the ground truth on its own: one
+        point-to-point ICP per region, all in one pass per iteration (me_drift, world 1).  Returns drift_dict's dict of
+        arrays, rows ascending by (ix, iy, iz): the transform T (R x 4 x 4) that moves the region onto the ground truth, its
+        centroid shift and rotation angle, and the fitness / rmse before and after.  The estimated cloud is unchanged
+        afterwards.  Multi-GPU: dist.drift_distributed."""
+        rows = C.POINTER(A.me_drift_row)()
+        n = C.c_int64(0)
+        self._check(self._L.me_drift(self._ctx, float(region_size), float(max_correspondence_distance), int(max_iteration),
+                                     float(relative_fitness), float(relative_rmse), C.byref(rows), C.byref(n)))
+        try:
+            nb = n.value * _DRIFT_ROW_DT.itemsize
+            a = np.frombuffer((C.c_char * nb).from_address(C.addressof(rows.contents)), _DRIFT_ROW_DT) if nb else \
+                np.zeros(0, _DRIFT_ROW_DT)
+            return drift_dict(a.copy())
+        finally:
+            self._L.me_free(rows)
+
+    def drift_begin(self, region_size, max_correspondence_distance, max_iteration=30, relative_fitness=1e-6,
+                    relative_rmse=1e-6):
+        """me_drift_begin: lists the regions, keeps a copy of the estimated cloud, runs the first sweep and fold; returns
+        the region count"""
+        n = C.c_int64(0)
+        self._check(self._L.me_drift_begin(self._ctx, float(region_size), float(max_correspondence_distance),
+                                           int(max_iteration), float(relative_fitness), float(relative_rmse), C.byref(n)))
+        return n.value
+
+    def drift_block(self):
+        """(device pointer, n_sum) of the block, ME_ICP_BLOCK_P2P values per region: SUM-reduce it in place (after
+        synchronize())"""
+        ptr = C.POINTER(C.c_double)()
+        n_sum = C.c_int32(0)
+        self._check(self._L.me_drift_block(self._ctx, C.byref(ptr), C.byref(n_sum)))
+        return C.cast(ptr, C.c_void_p).value, n_sum.value
+
+    def drift_step(self):
+        """reads the reduced block, updates every running region, moves and sweeps again; True when every region is done"""
+        done = C.c_int32(0)
+        self._check(self._L.me_drift_step(self._ctx, C.byref(done)))
+        return bool(done.value)
+
+    def drift_end(self, n_regions):
+        """the rows, as region_drift; the estimated cloud is back as it was at drift_begin"""
+        rows = np.zeros(max(int(n_regions), 1), _DRIFT_ROW_DT)
+        self._check(self._L.me_drift_end(self._ctx, rows.ctypes.data_as(C.POINTER(A.me_drift_row)), int(n_regions)))
+        return drift_dict(rows[:int(n_regions)])
 
     def get_nn(self, which_query):
         n = self.n[which_query]

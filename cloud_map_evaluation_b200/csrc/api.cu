@@ -232,6 +232,7 @@ void me_destroy(me_ctx *ctx) {
   icp_close(ctx, false);
   nn_quantile_free(ctx);
   nn_region_free(ctx);
+  drift_close(ctx, false);
   if (ctx->copy_stream) { cudaStreamSynchronize(ctx->copy_stream); cudaStreamDestroy(ctx->copy_stream); }
   if (ctx->compute_mark) cudaEventDestroy(ctx->compute_mark);
   for (Cloud &c : ctx->cloud) free_cloud(c);
@@ -468,9 +469,18 @@ int me_get_cloud(me_ctx *ctx, int which, double *xyz_host, int64_t capacity_poin
   return ME_OK;
 }
 
+// a registration cannot start while a drift loop moves the estimated cloud; refused before the call stales anything, so the
+// drift loop stays open
+static bool drift_blocks_icp(me_ctx *ctx) {
+  if (!ctx->drift.open) return false;
+  fail(ctx, ME_ERR_INVALID, "me_icp_begin while a drift loop is open (me_drift_end first)");
+  return true;
+}
+
 int me_icp_point_to_point(me_ctx *ctx, double max_correspondence_distance, int32_t max_iteration, double relative_fitness,
                           double relative_rmse, const double T_init[16], me_icp_result *out) {
   ME_ENTER(ctx);
+  if (drift_blocks_icp(ctx)) return ME_ERR_INVALID;
   ctx->cloud_gen++;      // stales the NN records (me_nn_curve*)
   if (!T_init || !out) return fail(ctx, ME_ERR_INVALID, "null argument");
   return run_icp(ctx, ME_ICP_POINT_TO_POINT, max_correspondence_distance, max_iteration, relative_fitness, relative_rmse, T_init, out);
@@ -479,6 +489,7 @@ int me_icp_point_to_point(me_ctx *ctx, double max_correspondence_distance, int32
 int me_icp(me_ctx *ctx, int32_t method, double max_correspondence_distance, int32_t max_iteration, double relative_fitness,
            double relative_rmse, const double T_init[16], me_icp_result *out) {
   ME_ENTER(ctx);
+  if (drift_blocks_icp(ctx)) return ME_ERR_INVALID;
   ctx->cloud_gen++;      // stales the NN records (me_nn_curve*)
   if (!T_init || !out) return fail(ctx, ME_ERR_INVALID, "null argument");
   return run_icp(ctx, method, max_correspondence_distance, max_iteration, relative_fitness, relative_rmse, T_init, out);
@@ -487,6 +498,7 @@ int me_icp(me_ctx *ctx, int32_t method, double max_correspondence_distance, int3
 int me_icp_begin(me_ctx *ctx, int32_t method, double max_correspondence_distance, int32_t max_iteration, double relative_fitness,
                  double relative_rmse, const double T_init[16]) {
   ME_ENTER(ctx);
+  if (drift_blocks_icp(ctx)) return ME_ERR_INVALID;
   ctx->cloud_gen++;      // stales the NN records (me_nn_curve*)
   if (!T_init) return fail(ctx, ME_ERR_INVALID, "null argument");
   return icp_begin(ctx, method, max_correspondence_distance, max_iteration, relative_fitness, relative_rmse, T_init);
@@ -995,6 +1007,68 @@ int me_nn_regions(me_ctx *ctx, double region_size, me_region_row **rows, int64_t
   me_region_row *r = (me_region_row *)std::malloc((size_t)std::max<int64_t>(n, 1) * sizeof(me_region_row));
   if (!r) return fail(ctx, ME_ERR_NOMEM, "me_nn_regions: host allocation of the rows failed");
   const int rc = me_nn_region_end(ctx, r, n);
+  if (rc != ME_OK) {
+    std::free(r);
+    return rc;
+  }
+  *rows = r;
+  *n_regions = n;
+  return ME_OK;
+}
+
+int me_drift_begin(me_ctx *ctx, double region_size, double max_correspondence_distance, int32_t max_iteration,
+                   double relative_fitness, double relative_rmse, int64_t *n_regions) {
+  ME_ENTER(ctx);
+  // bad arguments are refused before anything is staled: an open drift loop stays open
+  if (!n_regions) return fail(ctx, ME_ERR_INVALID, "null argument");
+  *n_regions = 0;
+  if (!(std::isfinite(region_size) && region_size > 0.0)) return fail(ctx, ME_ERR_INVALID, "me_drift_begin: region_size must be finite and > 0");
+  if (!(std::isfinite(max_correspondence_distance) && max_correspondence_distance > 0.0))
+    return fail(ctx, ME_ERR_INVALID, "me_drift_begin: max_correspondence_distance must be finite and > 0");
+  if (max_iteration < 0) return fail(ctx, ME_ERR_INVALID, "me_drift_begin: max_iteration must be >= 0");
+  ctx->cloud_gen++;      // stales the NN records (me_nn_curve*)
+  return drift_begin(ctx, region_size, max_correspondence_distance, max_iteration, relative_fitness, relative_rmse, n_regions);
+}
+
+int me_drift_block(me_ctx *ctx, double **device_block, int32_t *n_sum) {
+  ME_ENTER(ctx);
+  if (!device_block || !n_sum) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return drift_block(ctx, device_block, n_sum);
+}
+
+int me_drift_step(me_ctx *ctx, int32_t *done) {
+  ME_ENTER(ctx);
+  if (!done) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return drift_step(ctx, done);
+}
+
+int me_drift_end(me_ctx *ctx, me_drift_row *rows, int64_t capacity) {
+  ME_ENTER(ctx);
+  if (!rows) return fail(ctx, ME_ERR_INVALID, "null argument");
+  const int rc = drift_end(ctx, rows, capacity);
+  ctx->cloud_gen++;      // the estimated cloud is back as it was: records of the moved cloud are stale
+  return rc;
+}
+
+int me_drift(me_ctx *ctx, double region_size, double max_correspondence_distance, int32_t max_iteration, double relative_fitness,
+             double relative_rmse, me_drift_row **rows, int64_t *n_regions) {
+  ME_ENTER(ctx);
+  if (!rows || !n_regions) return fail(ctx, ME_ERR_INVALID, "null argument");
+  *rows = nullptr;
+  *n_regions = 0;
+  if (ctx->world != 1)
+    return fail(ctx, ME_ERR_INVALID, "me_drift needs world == 1; use me_drift_begin / _block + all-reduce / _step / _end");
+  int64_t n = 0;
+  ME_TRY(me_drift_begin(ctx, region_size, max_correspondence_distance, max_iteration, relative_fitness, relative_rmse, &n));
+  int32_t done = 0;
+  while (!done) ME_TRY(me_drift_step(ctx, &done));
+  me_drift_row *r = (me_drift_row *)std::malloc((size_t)std::max<int64_t>(n, 1) * sizeof(me_drift_row));
+  if (!r) {
+    drift_close(ctx, true);
+    ctx->cloud_gen++;
+    return fail(ctx, ME_ERR_NOMEM, "me_drift: host allocation of the rows failed");
+  }
+  const int rc = me_drift_end(ctx, r, n);
   if (rc != ME_OK) {
     std::free(r);
     return rc;

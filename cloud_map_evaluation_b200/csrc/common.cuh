@@ -207,6 +207,47 @@ struct RegionRun {
   long long cap_part = 0;
 };
 
+// the occupied regions floor(x / s) of est ++ gt, or of est alone (list_regions, region.cu).  The device arrays live in
+// d_work until its next user: val = caller ids sorted by region (stable: caller order inside a region, est before gt),
+// pos = the scanned heads (sorted point j lies in region pos[j + 1] - 1), seg[r] / est_end[r] = first sorted position and one
+// past the last est point of region r (seg[R] = n), chunks = the scanned chunk counts per direction ((R + 1) each), pos_of =
+// scratch for record_positions (max(n_est, n_gt) entries)
+static constexpr int kRegionChunk = 1024;      // points per warp of the region folds (region.cu, drift.cu): the unit of `chunks`
+struct RegionList {
+  long long R = 0, n = 0;
+  uint32_t *val = nullptr, *pos = nullptr, *pos_of = nullptr, *seg = nullptr, *est_end = nullptr, *chunks = nullptr;
+  uint32_t n_chunks[2] = {0, 0};
+  std::vector<int64_t> index, n_est, n_gt;   // 3 per region; per region
+};
+
+// an open drift loop (me_drift_begin .. me_drift_end, drift.cu): one point-to-point ICP per region of the estimated cloud,
+// the same state on every rank
+struct DriftRun {
+  bool open = false;
+  unsigned long long gen = 0;          // cloud_gen at me_drift_begin
+  double s = 0, max_dist = 0, rel_fitness = 0, rel_rmse = 0;
+  int max_iter = 0;
+  long long R = 0, n_chunks = 0;
+  const double *xyz = nullptr;         // the estimated cloud's buffer and size at me_drift_begin
+  long long n_est = 0;
+  double *orig = nullptr;              // the estimated cloud as handed in
+  uint32_t *d_rid = nullptr;           // caller index -> region
+  uint32_t *d_val = nullptr;           // caller ids sorted by region, caller order inside a region
+  uint32_t *d_pos_of = nullptr;        // caller index -> record position after the last re-layout
+  uint32_t *d_seg = nullptr;           // R + 1 first positions in d_val
+  uint32_t *d_chunk_off = nullptr;     // R + 1 scanned chunk counts
+  double *d_T = nullptr;               // 16 per region, row-major
+  double *d_c = nullptr;               // 3 per region: the centre the sums are taken about
+  double *d_blk = nullptr;             // ME_ICP_BLOCK_P2P per region
+  double *d_part = nullptr;            // the fold's per-chunk values
+  bool have_prev = false;
+  std::vector<int64_t> index, n_est_r;
+  std::vector<double> c, T, centroid, fitness, rmse, fitness0, rmse0;
+  std::vector<int64_t> n_corr, n_corr0;
+  std::vector<int32_t> it, status;     // status < 0: running
+  std::vector<double> h_blk;
+};
+
 // numpy's method="linear" position of probability p among n sorted values: h = (n - 1) p, k = floor(h), g = h - k
 inline void quantile_rank(long long n, double p, long long *k, double *g) {
   const double h = (double)(n - 1) * p;
@@ -290,6 +331,7 @@ struct me_ctx {
   long long cap_curve = 0;
   me::QuantRun quant;                  // distance quantiles (me_nn_quantile*), from the same records
   me::RegionRun region;                // the per-region table (me_nn_region*), from the same records
+  me::DriftRun drift;                  // the per-region drift loop (me_drift*)
   std::string err;
 };
 
@@ -404,6 +446,14 @@ int nn_region_begin(me_ctx *ctx, double s, int64_t *n_regions);
 int nn_region_block(me_ctx *ctx, double **device_block, int32_t *n_sum, int32_t *n_max);
 int nn_region_end(me_ctx *ctx, me_region_row *rows, int64_t capacity);
 void nn_region_free(me_ctx *ctx);
+int list_regions(me_ctx *ctx, const char *who, double s, bool with_gt, RegionList *L);
+int record_positions(me_ctx *ctx, int which, uint32_t *pos_of);
+// one point-to-point ICP per region of the estimated cloud (arguments checked by the caller) — me_drift_* (drift.cu)
+int drift_begin(me_ctx *ctx, double s, double max_dist, int max_iter, double rel_fitness, double rel_rmse, int64_t *n_regions);
+int drift_block(me_ctx *ctx, double **device_block, int32_t *n_sum);
+int drift_step(me_ctx *ctx, int32_t *done);
+int drift_end(me_ctx *ctx, me_drift_row *rows, int64_t capacity);
+void drift_close(me_ctx *ctx, bool restore);
 // the accumulators go to the cloud's MME section of d_block
 int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors);
 

@@ -27,7 +27,6 @@
 namespace me {
 
 static constexpr int kThreads = 256;
-static constexpr int kRegionChunk = 1024;                                  // query points per warp of the fold
 static constexpr double kAxisLimit = 1048576.0;                            // |index| < 2^20 per axis
 static constexpr int kSumF = ME_REGION_SUM_FIELDS, kMaxF = ME_REGION_MAX_FIELDS;
 static constexpr int kPart = kSumF + kMaxF;                                // values per chunk: the SUM fields, then the MAX fields
@@ -220,26 +219,24 @@ static std::string num(double x) {
   return b;
 }
 
-int nn_region_begin(me_ctx *ctx, double s, int64_t *n_regions) {
-  RegionRun &G = ctx->region;
-  G.open = false;
-  *n_regions = 0;
-  ME_TRY(nn_records_fresh(ctx, "me_nn_region*"));
+// The occupied list of est ++ gt (with_gt = false: of est alone), in d_work.  The size checks and their messages are the
+// same for every caller; `who` names the call in them.
+int list_regions(me_ctx *ctx, const char *who, double s, bool with_gt, RegionList *L) {
   const Cloud &E = ctx->cloud[ME_CLOUD_EST], &T = ctx->cloud[ME_CLOUD_GT];
   ME_TRY(compute_bbox(ctx, ME_CLOUD_EST));
-  ME_TRY(compute_bbox(ctx, ME_CLOUD_GT));
+  if (with_gt) ME_TRY(compute_bbox(ctx, ME_CLOUD_GT));
   RegionGeom g;
   g.s = s;
   double mn[3], mx[3];
   for (int a = 0; a < 3; ++a) {
-    mn[a] = std::min(E.bbox_min[a], T.bbox_min[a]);
-    mx[a] = std::max(E.bbox_max[a], T.bbox_max[a]);
+    mn[a] = with_gt ? std::min(E.bbox_min[a], T.bbox_min[a]) : E.bbox_min[a];
+    mx[a] = with_gt ? std::max(E.bbox_max[a], T.bbox_max[a]) : E.bbox_max[a];
   }
   for (int a = 0; a < 3; ++a) {
     if (axis_fits(mn[a], mx[a], s)) continue;
     double s_fit = 0.0;      // the smallest size that fits along every axis
     for (int b = 0; b < 3; ++b) s_fit = std::max(s_fit, smallest_fit(mn[b], mx[b]));
-    return fail(ctx, ME_ERR_INVALID, std::string("me_nn_region_begin: region_size ") + num(s) + " puts region indices along " +
+    return fail(ctx, ME_ERR_INVALID, std::string(who) + ": region_size " + num(s) + " puts region indices along " +
                                          "xyz"[a] + " outside |index| < 2^20 (" + num(std::floor(mn[a] / s)) + " .. " +
                                          num(std::floor(mx[a] / s)) + "); the smallest region_size that fits is " + num(s_fit));
   }
@@ -252,13 +249,13 @@ int nn_region_begin(me_ctx *ctx, double s, int64_t *n_regions) {
     g.bits[a] = b;
     key_bits += b;
   }
-  const long long n_est = E.n, n = E.n + T.n;
-  if (n >= 0xffffffffll) return fail(ctx, ME_ERR_RANGE, "me_nn_region_begin: more than 2^32 - 1 points in the two clouds");
+  const long long n_est = E.n, n_gt = with_gt ? T.n : 0, n = n_est + n_gt;
+  if (n >= 0xffffffffll) return fail(ctx, ME_ERR_RANGE, std::string(who) + ": more than 2^32 - 1 points in the two clouds");
   const long long r_cap = std::min<long long>(n, ME_REGION_MAX_REGIONS);
   auto align = [](size_t x) { return (x + 255) & ~(size_t)255; };
   const size_t o_key0 = 0, o_key1 = o_key0 + align((size_t)n * 8), o_val0 = o_key1 + align((size_t)n * 8),
                o_val1 = o_val0 + align((size_t)n * 4), o_pos = o_val1 + align((size_t)n * 4),
-               o_pos_of = o_pos + align((size_t)(n + 1) * 4), o_seg = o_pos_of + align((size_t)std::max(E.n, T.n) * 4),
+               o_pos_of = o_pos + align((size_t)(n + 1) * 4), o_seg = o_pos_of + align((size_t)std::max(n_est, n_gt) * 4),
                o_ee = o_seg + align((size_t)(r_cap + 1) * 4), o_rkey = o_ee + align((size_t)r_cap * 4),
                o_cnt = o_rkey + align((size_t)r_cap * 8), o_chunks = o_cnt + align((size_t)2 * r_cap * 4),
                total = o_chunks + align((size_t)2 * (r_cap + 1) * 4);
@@ -266,12 +263,11 @@ int nn_region_begin(me_ctx *ctx, double s, int64_t *n_regions) {
   char *base = (char *)ctx->d_work;
   unsigned long long *key0 = (unsigned long long *)(base + o_key0), *key1 = (unsigned long long *)(base + o_key1);
   uint32_t *val0 = (uint32_t *)(base + o_val0), *val1 = (uint32_t *)(base + o_val1), *pos = (uint32_t *)(base + o_pos);
-  uint32_t *pos_of = (uint32_t *)(base + o_pos_of), *seg = (uint32_t *)(base + o_seg), *est_end = (uint32_t *)(base + o_ee);
+  uint32_t *seg = (uint32_t *)(base + o_seg), *est_end = (uint32_t *)(base + o_ee);
   unsigned long long *rkey = (unsigned long long *)(base + o_rkey);
   uint32_t *cnt = (uint32_t *)(base + o_cnt), *chunks = (uint32_t *)(base + o_chunks);
   const int blocks = (int)std::min<long long>((n + kThreads) / kThreads, (long long)ctx->sm_count * 16);
 
-  // the occupied list
   region_key_kernel<<<blocks, kThreads, 0, ctx->stream>>>(E.d_xyz, n_est, T.d_xyz, n, g, key0, val0);
   ME_LAUNCH_CHECK(ctx);
   unsigned long long *ks = nullptr;
@@ -285,7 +281,7 @@ int nn_region_begin(me_ctx *ctx, double s, int64_t *n_regions) {
   ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   const long long R = (long long)h[0];
   if (R > ME_REGION_MAX_REGIONS)
-    return fail(ctx, ME_ERR_INVALID, "me_nn_region_begin: " + std::to_string(R) + " occupied regions at region_size " + num(s) +
+    return fail(ctx, ME_ERR_INVALID, std::string(who) + ": " + std::to_string(R) + " occupied regions at region_size " + num(s) +
                                          ", at most ME_REGION_MAX_REGIONS = 2^21; choose a larger region_size");
   ME_CUDA(ctx, cudaMemsetAsync(est_end, 0, (size_t)R * 4, ctx->stream));
   region_list_kernel<<<blocks, kThreads, 0, ctx->stream>>>(ks, vs, pos, n, n_est, seg, est_end, rkey);
@@ -297,31 +293,60 @@ int nn_region_begin(me_ctx *ctx, double s, int64_t *n_regions) {
   ME_TRY(exclusive_scan_inplace(ctx, chunks + R + 1, R + 1));
   std::vector<unsigned long long> hkey((size_t)R);
   std::vector<uint32_t> hcnt((size_t)2 * R);
-  uint32_t n_chunks[2];
   ME_CUDA(ctx, cudaMemcpyAsync(hkey.data(), rkey, (size_t)R * 8, cudaMemcpyDeviceToHost, ctx->stream));
   ME_CUDA(ctx, cudaMemcpyAsync(hcnt.data(), cnt, (size_t)2 * R * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  ME_CUDA(ctx, cudaMemcpyAsync(&n_chunks[0], chunks + R, 4, cudaMemcpyDeviceToHost, ctx->stream));
-  ME_CUDA(ctx, cudaMemcpyAsync(&n_chunks[1], chunks + 2 * R + 1, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  ME_CUDA(ctx, cudaMemcpyAsync(&L->n_chunks[0], chunks + R, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  ME_CUDA(ctx, cudaMemcpyAsync(&L->n_chunks[1], chunks + 2 * R + 1, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  L->R = R;
+  L->n = n;
+  L->val = vs; L->pos = pos; L->pos_of = (uint32_t *)(base + o_pos_of); L->seg = seg; L->est_end = est_end; L->chunks = chunks;
+  L->index.resize((size_t)3 * R);
+  L->n_est.resize((size_t)R);
+  L->n_gt.resize((size_t)R);
+  for (long long r = 0; r < R; ++r) {
+    unsigned long long k = hkey[r];
+    for (int a = 2; a >= 0; --a) {
+      L->index[3 * r + a] = g.lo[a] + (long long)(g.bits[a] ? k & ((1ull << g.bits[a]) - 1) : 0ull);
+      k = g.bits[a] ? k >> g.bits[a] : k;
+    }
+    L->n_est[r] = hcnt[r];
+    L->n_gt[r] = hcnt[R + r];
+  }
+  return ME_OK;
+}
+
+// pos_of[caller index] = position of the point's record in the cloud's cell-sorted layout (~0u: not laid out here)
+int record_positions(me_ctx *ctx, int which, uint32_t *pos_of) {
+  const Cloud &Qc = ctx->cloud[which];
+  ME_CUDA(ctx, cudaMemsetAsync(pos_of, 0xff, (size_t)Qc.n * 4, ctx->stream));
+  const int qblocks = (int)std::min<long long>((Qc.ns + kThreads - 1) / kThreads + 1, (long long)ctx->sm_count * 16);
+  record_pos_kernel<<<qblocks, kThreads, 0, ctx->stream>>>(Qc.d_sorted, Qc.ns, pos_of);
+  ME_LAUNCH_CHECK(ctx);
+  return ME_OK;
+}
+
+int nn_region_begin(me_ctx *ctx, double s, int64_t *n_regions) {
+  RegionRun &G = ctx->region;
+  G.open = false;
+  *n_regions = 0;
+  ME_TRY(nn_records_fresh(ctx, "me_nn_region*"));
+  RegionList RL;
+  ME_TRY(list_regions(ctx, "me_nn_region_begin", s, true, &RL));
+  const long long R = RL.R, n_est = ctx->cloud[ME_CLOUD_EST].n;
+  const uint32_t *n_chunks = RL.n_chunks;
+  uint32_t *vs = RL.val, *pos_of = RL.pos_of, *seg = RL.seg, *est_end = RL.est_end, *chunks = RL.chunks;
+  const int rblocks = (int)std::min<long long>((R + kThreads) / kThreads, (long long)ctx->sm_count * 16);
 
   // the block: zero for a direction the last me_eval_nn* did not evaluate
   const long long n_blk = (long long)(2 * kSumF + 2 * kMaxF) * R;
   ME_TRY(ensure(ctx, (void **)&G.d_blk, &G.cap_blk, n_blk, sizeof(double)));
   ME_CUDA(ctx, cudaMemsetAsync(G.d_blk, 0, (size_t)n_blk * sizeof(double), ctx->stream));
-  ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   G.s = s;
   G.n = R;
-  G.index.resize((size_t)3 * R);
-  G.n_est.resize((size_t)R);
-  G.n_gt.resize((size_t)R);
-  for (long long r = 0; r < R; ++r) {
-    unsigned long long k = hkey[r];
-    for (int a = 2; a >= 0; --a) {
-      G.index[3 * r + a] = g.lo[a] + (long long)(g.bits[a] ? k & ((1ull << g.bits[a]) - 1) : 0ull);
-      k = g.bits[a] ? k >> g.bits[a] : k;
-    }
-    G.n_est[r] = hcnt[r];
-    G.n_gt[r] = hcnt[R + r];
-  }
+  G.index = std::move(RL.index);
+  G.n_est = std::move(RL.n_est);
+  G.n_gt = std::move(RL.n_gt);
 
   // the record fold, per evaluated direction
   const me_nn_params *p = &ctx->curve_p;
@@ -331,10 +356,7 @@ int nn_region_begin(me_ctx *ctx, double s, int64_t *n_regions) {
   for (int q = 0; q < 2; ++q) {
     if (!(dirs & (1 << q)) || n_chunks[q] == 0) continue;
     const Cloud &Qc = ctx->cloud[q];
-    ME_CUDA(ctx, cudaMemsetAsync(pos_of, 0xff, (size_t)Qc.n * 4, ctx->stream));
-    const int qblocks = (int)std::min<long long>((Qc.ns + kThreads - 1) / kThreads + 1, (long long)ctx->sm_count * 16);
-    record_pos_kernel<<<qblocks, kThreads, 0, ctx->stream>>>(Qc.d_sorted, Qc.ns, pos_of);
-    ME_LAUNCH_CHECK(ctx);
+    ME_TRY(record_positions(ctx, q, pos_of));
     NNConst C{};
     for (int k = 0; k < 5; ++k) C.tau[k] = p->tau[k];
     set_cutoff(C, p);

@@ -124,6 +124,28 @@ def icp_distributed(ctx, device, max_correspondence_distance, T_init=None, max_i
     return ctx.icp_end()
 
 
+def drift_distributed(ctx, device, region_size, max_correspondence_distance, max_iteration=30, relative_fitness=1e-6,
+                      relative_rmse=1e-6, group=None):
+    """The drift per region on every rank of the job (MapEvalB200.region_drift for world > 1): the clouds are replicated,
+    every rank lists the same regions and folds the pairs of its query range, then ONE in-place SUM all-reduce of the
+    17-value block per region per iteration; every rank applies the same updates to the same reduced doubles, so every rank
+    returns the same rows."""
+    import torch
+    import torch.distributed as dist
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    n = ctx.drift_begin(region_size, max_correspondence_distance, max_iteration, relative_fitness, relative_rmse)
+    ptr, n_sum = ctx.drift_block()
+    blk = torch.as_tensor(_DeviceBlock(ptr, n_sum), device=device) if world > 1 and n_sum > 0 else None
+    done = False
+    while not done:
+        if blk is not None:
+            ctx.synchronize()
+            dist.all_reduce(blk, group=group)
+            torch.cuda.current_stream(device).synchronize()
+        done = ctx.drift_step()
+    return ctx.drift_end(n)
+
+
 def allreduce_voxel_w(ctx, device, group=None):
     """Slab layout, between MapEvalB200.voxel_begin and voxel_finish_accum_device: MAX-all-reduce of the W table over the
     estimated cloud's voxels in place (-1 = no pair; every voxel has one owner), so that the SCS sweep of every rank sees

@@ -97,6 +97,9 @@ struct Param {   // map_eval.h:60-116
   // AC / COM / CD / F1 / IoU per region floor(x / region_size), written to region_errors.txt (me_nn_region*: no new sweep);
   // absent or 0 = off.  region_size = vmd_voxel_size lines the rows up with voxel_errors.txt
   double region_size_ = 0.0;
+  // drift per region: every region floor(x / drift_region_size) of the estimate aligned to the ground truth on its own
+  // (me_drift*: point-to-point ICP per region, R = icp_max_distance, ICP's criteria), written to region_drift.txt; absent or 0 = off
+  double drift_region_size_ = 0.0;
 };
 
 // map_eval_main.cpp:120-208
@@ -167,6 +170,12 @@ inline Param loadParametersFromYAML(const std::string &yaml_file_path) {
       if (!(std::isfinite(param.region_size_) && param.region_size_ >= 0.0))
         throw std::runtime_error("region_size must be finite and >= 0 (0 = off), not " + config["region_size"].as<std::string>());
     }
+    if (config["drift_region_size"]) {
+      param.drift_region_size_ = config["drift_region_size"].as<double>();
+      if (!(std::isfinite(param.drift_region_size_) && param.drift_region_size_ >= 0.0))
+        throw std::runtime_error("drift_region_size must be finite and >= 0 (0 = off), not " +
+                                 config["drift_region_size"].as<std::string>());
+    }
     return param;
   } catch (const std::exception &e) {
     std::cerr << "Error loading parameters: " << e.what() << std::endl;
@@ -197,7 +206,7 @@ inline void dumpParam(const Param &p, std::ostream &os) {
      << "\naccuracy_curve_steps=" << p.accuracy_curve_steps_ << "\naccuracy_curve_max=" << p.accuracy_curve_max_
      << "\ndistance_quantiles=";
   for (size_t i = 0; i < p.distance_quantiles_.size(); ++i) os << (i ? "," : "") << p.distance_quantiles_[i];
-  os << "\nregion_size=" << p.region_size_ << "\n";
+  os << "\nregion_size=" << p.region_size_ << "\ndrift_region_size=" << p.drift_region_size_ << "\n";
 }
 
 // Eigen's default IOFormat for `vec.transpose()`: coefficients right-aligned to a common width, one space apart
@@ -340,6 +349,7 @@ class MapEvalB200 {
   int accuracyCurve(const me_nn_params &p, const me_nn_accum &e2g, const me_nn_accum &g2e);
   int distanceQuantiles();
   int regionErrors();
+  int regionDrift();
   GpuGroup gpus_;            // one context per GPU; rank r evaluates the r-th shard of every sweep's query range
   me_ctx *ctx_ = nullptr;    // = gpus_.ctx(0): the voxel stage and the single-GPU calls
   std::vector<double> map_3d_, gt_3d_;   // N x 3 fp64, the layout of open3d PointCloud::points_ (as loaded)
@@ -629,6 +639,7 @@ inline int MapEvalB200::calculateMetricsWithInitialMatrix() {
                  "so the CD vector / gt->est lines are not comparable with a reference run.  geometric_gt_pairing: true pairs "
                  "the points geometrically instead." << std::endl;
   if (param_.save_immediate_result_ && renderDistances(false) != 0) return -1;
+  if (param_.drift_region_size_ > 0.0 && regionDrift() != 0) return -1;
   std::cout << "INFO: Chamfer Distance: " << eigenRow(nn_.cd, 5, 6) << std::endl;
   std::cout << "INFO: F1 Score: " << eigenRow(nn_.f1, 5, 6) << std::endl;
   std::cout << "INFO: est-gt MME: " << mme_est << " " << mme_gt << std::endl;
@@ -777,6 +788,66 @@ inline int MapEvalB200::regionErrors() {
   return 0;
 }
 
+// drift per region: every region floor(x / drift_region_size) of the estimate aligned to the ground truth on its own (the
+// me_drift_* loop on every GPU, one grouped NCCL SUM all-reduce of the 17 values per region per iteration, as the multi-GPU
+// loop of performRegistration) -> region_drift.txt next to map_results.txt.  The estimate is restored bit for bit afterwards,
+// so it runs after the consumers of the pass's NN records, which it stales.
+inline int MapEvalB200::regionDrift() {
+  const double s = param_.drift_region_size_;
+  const int G = gpus_.size();
+  std::vector<int64_t> n(G, 0);
+  std::vector<double *> ptr(G, nullptr);
+  std::vector<int32_t> n_sum(G, 0), done(G, 0);
+  if (gpus_.for_each([&](int r, me_ctx *c) {
+        int rc = me_drift_begin(c, s, param_.icp_max_distance_, 30, 1e-6, 1e-6, &n[r]);
+        if (rc == ME_OK) rc = me_drift_block(c, &ptr[r], &n_sum[r]);
+        return rc != ME_OK ? rc : me_synchronize(c);
+      }) != ME_OK)
+    return fail("me_drift_begin");
+  while (!done[0]) {
+    if (!gpus_.allreduce_device(ptr, (size_t)n_sum[0], ncclSum)) return fail("all-reduce of the drift block");
+    if (gpus_.for_each([&](int r, me_ctx *c) {
+          const int rc = me_drift_step(c, &done[r]);
+          return rc != ME_OK ? rc : me_synchronize(c);
+        }) != ME_OK)
+      return fail("me_drift_step");
+  }
+  std::vector<std::vector<me_drift_row>> rows(G, std::vector<me_drift_row>((size_t)std::max<int64_t>(n[0], 1)));
+  if (gpus_.for_each([&](int r, me_ctx *c) { return me_drift_end(c, rows[r].data(), n[0]); }) != ME_OK) return fail("me_drift_end");
+  rows[0].resize((size_t)n[0]);
+  const std::string path = results_subfolder + "region_drift.txt";
+  std::ofstream f(path);
+  if (!f.is_open()) {
+    std::cerr << "ERROR: cannot write " << path << std::endl;
+    return -1;
+  }
+  f << "min_x min_y min_z max_x max_y max_z n_est n_corr_before fitness_before rmse_before n_corr fitness rmse shift_x shift_y "
+       "shift_z shift_norm angle_rad iterations status";
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 4; ++j) f << " T" << i << j;
+  f << "\n" << std::fixed << std::setprecision(15);
+  int64_t converged = 0, worst = -1;
+  for (size_t k = 0; k < rows[0].size(); ++k) {
+    const me_drift_row &r = rows[0][k];
+    f << r.min[0] << " " << r.min[1] << " " << r.min[2] << " " << r.max[0] << " " << r.max[1] << " " << r.max[2] << " " << r.n_est
+      << " " << r.n_corr_before << " " << r.fitness_before << " " << r.rmse_before << " " << r.n_corr << " " << r.fitness << " "
+      << r.rmse << " " << r.shift[0] << " " << r.shift[1] << " " << r.shift[2] << " " << r.shift_norm << " " << r.angle << " "
+      << r.iterations << " " << r.status;
+    for (int i = 0; i < 12; ++i) f << " " << r.T[i];
+    f << "\n";
+    converged += r.status == ME_DRIFT_CONVERGED;
+    if (worst < 0 || r.shift_norm > rows[0][(size_t)worst].shift_norm) worst = (int64_t)k;
+  }
+  std::cout << "INFO: drift of " << n[0] << " regions of edge " << s << " (" << converged << " converged) saved to " << path;
+  if (worst >= 0) {
+    const me_drift_row &w = rows[0][(size_t)worst];
+    std::cout << "; largest shift " << w.shift_norm << " in [" << w.min[0] << ", " << w.max[0] << "] x [" << w.min[1] << ", "
+              << w.max[1] << "] x [" << w.min[2] << ", " << w.max[2] << "]";
+  }
+  std::cout << std::endl;
+  return 0;
+}
+
 // global_registration: FPFH + RANSAC on context 0 (me_global_registration) on the loaded, down-sampled clouds.  The result
 // is a pure function of the clouds, the parameters and the seed, so every context of a multi-GPU run uses context 0's T
 // without a collective.  It replaces initial_matrix: path A's transform, path B's T_init.
@@ -881,6 +952,7 @@ inline int MapEvalB200::performRegistration() {
   if (!param_.distance_quantiles_.empty() && distanceQuantiles() != 0) return -1;
   if (param_.region_size_ > 0.0 && regionErrors() != 0) return -1;
   if (param_.save_immediate_result_ && renderDistances(true) != 0) return -1;
+  if (param_.drift_region_size_ > 0.0 && regionDrift() != 0) return -1;
   full_chamfer_dist = nn_.full_cd;
   t_fcd = t_acc;
   t5 = tic_toc.toc();

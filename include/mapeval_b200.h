@@ -504,6 +504,57 @@ ME_API int  me_nn_regions(me_ctx *ctx, double region_size, me_region_row **rows,
 ME_API int  me_region_finalize(int64_t n_regions, double region_size, const int64_t *index, const int64_t *n_est,
                                const int64_t *n_gt, const double *host_block, me_region_row *rows);   /* host only */
 
+/* ---- drift per region: every region of the estimated cloud aligned to the ground truth on its own --------------------------
+ * Separates a region that is shifted or turned as a whole (drift) from one that is noisy or smeared (damage): a rigid
+ * point-to-point ICP per region, all of them in one pass over the cloud per iteration.
+ * Regions: an est point's region is floor(x / s) per axis (IEEE division), the rule of me_nn_region_begin, taken from the
+ * estimated cloud as it is at me_drift_begin; only regions holding est points are listed, ascending by (ix, iy, iz), with
+ * the limits and messages of me_nn_region_begin (|index| < 2^20, at most ME_REGION_MAX_REGIONS).  Membership is fixed at
+ * begin.  Region r has a transform T_r, I at first.  Each iteration:
+ *   1. every est point i := T_{r(i)} x_i (original coordinates, me_transform's rounding: never compounded on moved points);
+ *   2. one est->gt sweep as registration runs it (ME_CUTOFF_DIST_LT_R, geometric pairing, est->gt only);
+ *   3. per region the ME_ICP_BLOCK_P2P sums of its kept pairs (nn >= 0, d2 < R^2), about the region centre
+ *      c_r = ((ix + 0.5) s, (iy + 0.5) s, (iz + 0.5) s);
+ *   4. every region not done: fitness = n_corr / n_est, rmse = sqrt(sum d2 / n_corr) (0 without pairs), me_icp_step's
+ *      convergence test, then update = me_icp_update(ME_ICP_POINT_TO_POINT, block_r, c_r) and T_r := update T_r.
+ * A region is done when it converged (ME_DRIFT_CONVERGED), made max_iteration updates (ME_DRIFT_ITERATION_LIMIT), or an update
+ * was due with fewer than 3 pairs (ME_DRIFT_TOO_FEW, T_r kept).  The loop ends when every region is done.
+ * Device block: n_sum = ME_ICP_BLOCK_P2P * n_regions SUM-reducible values, [region][count, sum p (3), sum q (3), sum q p^T (9),
+ * sum d2].  Folded in caller order per region with a fixed shuffle tree and every product and sum rounded on its own; no
+ * floating-point atomics, so two calls give the same bits.
+ * The loop (as me_icp_begin .. me_icp_end; every rank the same calls): me_drift_begin checks, lists the regions, keeps a copy
+ * of the estimated cloud and runs the first sweep; me_drift_block hands out the block (SUM-all-reduce it in place after
+ * me_synchronize); me_drift_step reads the reduced block, updates, moves and sweeps (*done = 1: nothing left to reduce);
+ * me_drift_end fills rows[0 .. n_regions - 1] (capacity >= n_regions).  After me_drift_end, and after any failure while the
+ * loop is open, the estimated cloud's points and normals are as they were at begin; the NN records are stale.  Refused: s or R
+ * not finite and > 0, max_iteration < 0, an empty cloud, a borrowed estimated cloud, world > 1 with ME_LAYOUT_SLAB requested,
+ * begin while a registration or drift loop is open (and me_icp_begin while a drift loop is open), calls out of order, and a
+ * cloud changed during the loop (the next loop call fails and closes the loop; an estimated cloud set into the same buffer is
+ * overwritten by the one held at begin).  Arguments are checked before anything else, so a begin refused for them leaves an
+ * open loop running.  me_drift: the whole loop at world 1, rows allocated by the library (me_free). */
+enum { ME_DRIFT_CONVERGED = 0, ME_DRIFT_ITERATION_LIMIT = 1, ME_DRIFT_TOO_FEW = 2 };
+typedef struct {
+  int64_t index[3];                             /* (ix, iy, iz) */
+  double  min[3], max[3];                       /* index * s, (index + 1) * s */
+  int64_t n_est;                                /* est points in the region */
+  int64_t n_corr_before;                        /* the first sweep, T_r = I */
+  double  fitness_before, rmse_before;
+  int64_t n_corr;                               /* the sweep at the final T_r */
+  double  fitness, rmse;
+  double  T[16];                                /* row-major: moves the region onto the ground truth */
+  double  centroid[3];                          /* mean of the region's original est points */
+  double  shift[3], shift_norm;                 /* T_r centroid - centroid, and its length */
+  double  angle;                                /* rotation angle of T_r in radians */
+  int32_t iterations, status;                   /* updates applied; ME_DRIFT_* */
+} me_drift_row;
+ME_API int  me_drift_begin(me_ctx *ctx, double region_size, double max_correspondence_distance, int32_t max_iteration,
+                           double relative_fitness, double relative_rmse, int64_t *n_regions);
+ME_API int  me_drift_block(me_ctx *ctx, double **device_block, int32_t *n_sum);
+ME_API int  me_drift_step(me_ctx *ctx, int32_t *done);
+ME_API int  me_drift_end(me_ctx *ctx, me_drift_row *rows, int64_t capacity);
+ME_API int  me_drift(me_ctx *ctx, double region_size, double max_correspondence_distance, int32_t max_iteration,
+                     double relative_fitness, double relative_rmse, me_drift_row **rows, int64_t *n_regions);
+
 /* replaces: ComputeMeanMapEntropyUsingNormalTBB / ...UsingNormal (min_neighbors 10, map_eval.cpp:1608-1737, 1538-1606),
  * ComputeMeanMapEntropy (min_neighbors 5, :1438-1535), ComputeEntropy (:1433-1436) and the min/max side effect of
  * ColorPointCloudByMME (:697-701).  entropies_host (nullable) receives N fp64, zeros where invalid.
