@@ -173,6 +173,23 @@ class me_region_row(C.Structure):
                 ("f1", C.c_double * 5), ("iou", C.c_double * 5)]
 
 
+# point-to-plane metrics and normal consistency (me_nn_surface*)
+# the SUM part: both directions laid out as the NN section of the accumulator block, then per direction n_no_normal
+# n_no_normal_nn n_nc sum_c; the MAX part: per direction max_e max_e_nn
+ME_SURFACE_BLOCK_SUM = 2 * (ME_NN_ACCUM_I64 + ME_NN_ACCUM_F64) + 8
+ME_SURFACE_BLOCK_MAX = 4
+
+
+class me_surface_dir(C.Structure):
+    _fields_ = [("n_no_normal", C.c_int64), ("n_no_normal_nn", C.c_int64), ("n_nc", C.c_int64),
+                ("normal_consistency", C.c_double), ("max_e", C.c_double), ("max_e_nn", C.c_double)]
+
+
+class me_surface_result(C.Structure):
+    _fields_ = [("plane", me_nn_result), ("est_to_gt", me_surface_dir), ("gt_to_est", me_surface_dir),
+                ("normal_consistency", C.c_double)]
+
+
 # drift per region (me_drift*)
 ME_DRIFT_CONVERGED = 0
 ME_DRIFT_ITERATION_LIMIT = 1

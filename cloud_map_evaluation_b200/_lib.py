@@ -29,6 +29,8 @@ SYMBOLS = (
     "me_quantile_finalize",
     "me_nn_region_begin", "me_nn_region_block", "me_nn_region_end", "me_nn_regions", "me_region_finalize",
     "me_drift_begin", "me_drift_block", "me_drift_step", "me_drift_end", "me_drift",
+    "me_nn_surface_begin", "me_nn_surface_normals_slice", "me_nn_surface_block", "me_nn_surface_end", "me_nn_surface",
+    "me_surface_finalize",
 )
 
 _lib = None
@@ -137,6 +139,12 @@ def load():
     L.me_drift_step.argtypes = [ctx, C.POINTER(C.c_int32)]
     L.me_drift_end.argtypes = [ctx, C.POINTER(A.me_drift_row), C.c_int64]
     L.me_drift.argtypes = [ctx, C.c_double, C.c_double, C.c_int32, C.c_double, C.c_double, C.POINTER(C.POINTER(A.me_drift_row)), i64p]
+    L.me_nn_surface_begin.argtypes = [ctx, C.c_int32]
+    L.me_nn_surface_normals_slice.argtypes = [ctx, C.c_int, C.POINTER(dp), i64p, C.POINTER(C.c_int32)]
+    L.me_nn_surface_block.argtypes = [ctx, C.POINTER(dp), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    L.me_nn_surface_end.argtypes = [ctx, C.POINTER(A.me_surface_result)]
+    L.me_nn_surface.argtypes = [ctx, C.c_int32, C.POINTER(A.me_surface_result)]
+    L.me_surface_finalize.argtypes = [C.POINTER(A.me_nn_params), dp, C.c_int64, C.c_int64, C.POINTER(A.me_surface_result)]
     L.me_kernel_trace.argtypes = [ctx, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.c_int32]
     if L.me_abi_version() != A.ME_ABI_VERSION:
         raise RuntimeError("libmapeval_b200.so ABI version mismatch")

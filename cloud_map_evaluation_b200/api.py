@@ -149,6 +149,36 @@ def region_finalize(region_size, index, n_est, n_gt, block):
     return region_dict(rows[:n])
 
 
+def surface_dict(res):
+    """me_surface_result -> {'cd' / 'f1' / 'iou' (5,), 'full_cd', 'normal_consistency', 'est_to_gt' / 'gt_to_est': {the
+    me_dir_result fields of the point-to-plane table, then the me_surface_dir fields}}; arrays for the five levels"""
+    def _v(x):
+        return np.array(x[:]) if isinstance(x, C.Array) else x
+    out = {name: np.array(getattr(res.plane, name)[:]) for name in ("cd", "f1", "iou")}
+    out["full_cd"] = res.plane.full_cd
+    out["normal_consistency"] = res.normal_consistency
+    for name in ("est_to_gt", "gt_to_est"):
+        p, s = getattr(res.plane, name), getattr(res, name)
+        d = {f[0]: _v(getattr(p, f[0])) for f in A.me_dir_result._fields_}
+        d.update({f[0]: getattr(s, f[0]) for f in A.me_surface_dir._fields_})
+        out[name] = d
+    return out
+
+
+def surface_finalize(params, block, n_est, n_gt):
+    """me_surface_finalize (host only): the point-to-plane result from a reduced host block (ME_SURFACE_BLOCK_SUM SUM values,
+    then ME_SURFACE_BLOCK_MAX MAX values) with the NN evaluation's parameters and the cloud sizes; as surface_dict"""
+    L = _lib.load()
+    blk = np.ascontiguousarray(block, dtype=np.float64).reshape(-1)
+    if blk.size != A.ME_SURFACE_BLOCK_SUM + A.ME_SURFACE_BLOCK_MAX:
+        raise ValueError("ME_SURFACE_BLOCK_SUM + ME_SURFACE_BLOCK_MAX values")
+    out = A.me_surface_result()
+    rc = L.me_surface_finalize(C.byref(params), blk.ctypes.data_as(C.POINTER(C.c_double)), int(n_est), int(n_gt), C.byref(out))
+    if rc != A.ME_OK:
+        raise MapEvalError(rc, "me_surface_finalize")
+    return surface_dict(out)
+
+
 # me_drift_row as a numpy record (8-byte fields, then two int32: no padding)
 _DRIFT_ROW_DT = np.dtype([("index", "<i8", 3), ("min", "<f8", 3), ("max", "<f8", 3), ("n_est", "<i8"), ("n_corr_before", "<i8"),
                           ("fitness_before", "<f8"), ("rmse_before", "<f8"), ("n_corr", "<i8"), ("fitness", "<f8"), ("rmse", "<f8"),
@@ -501,6 +531,41 @@ class MapEvalB200:
         rows, rows_p = _region_rows(n_regions)
         self._check(self._L.me_nn_region_end(self._ctx, rows_p, int(n_regions)))
         return region_dict(rows[:int(n_regions)])
+
+    def surface_metrics(self, knn=0):
+        """Point-to-plane AC / COM / CD / F1 / IoU and normal consistency from the last NN evaluation's records (me_nn_surface,
+        world 1): the distance of every query point to the tangent plane of its nearest neighbour, and |n_p . n_t| per pair.
+        knn = 0 uses the clouds' own normals; knn in 1..64 estimates k-NN normals for a cloud without them as a working copy
+        (the cloud still has none afterwards).  Returns surface_dict's dict.  Multi-GPU: dist.surface_distributed."""
+        out = A.me_surface_result()
+        self._check(self._L.me_nn_surface(self._ctx, int(knn), C.byref(out)))
+        return surface_dict(out)
+
+    def surface_begin(self, knn=0):
+        """me_nn_surface_begin: checks the records, the normals and knn"""
+        self._check(self._L.me_nn_surface_begin(self._ctx, int(knn)))
+
+    def surface_normals_slice(self, which):
+        """(device pointer of the world * slice * 3 fp64 normal buffer or None, slice points, pending): pending = True when
+        the caller must all-gather the buffer in place (this rank filled rows [rank * slice, (rank + 1) * slice))"""
+        ptr = C.POINTER(C.c_double)()
+        s, pend = C.c_int64(0), C.c_int32(0)
+        self._check(self._L.me_nn_surface_normals_slice(self._ctx, int(which), C.byref(ptr), C.byref(s), C.byref(pend)))
+        return C.cast(ptr, C.c_void_p).value, s.value, bool(pend.value)
+
+    def surface_block(self):
+        """(device pointer, n_sum, n_max) of the block; the first call folds this rank's records.  SUM-reduce the first n_sum
+        values and MAX-reduce the next n_max in place (after synchronize())"""
+        ptr = C.POINTER(C.c_double)()
+        n_sum, n_max = C.c_int32(0), C.c_int32(0)
+        self._check(self._L.me_nn_surface_block(self._ctx, C.byref(ptr), C.byref(n_sum), C.byref(n_max)))
+        return C.cast(ptr, C.c_void_p).value, n_sum.value, n_max.value
+
+    def surface_end(self):
+        """the result from the reduced block, as surface_metrics"""
+        out = A.me_surface_result()
+        self._check(self._L.me_nn_surface_end(self._ctx, C.byref(out)))
+        return surface_dict(out)
 
     def region_drift(self, region_size, max_correspondence_distance, max_iteration=30, relative_fitness=1e-6,
                      relative_rmse=1e-6):

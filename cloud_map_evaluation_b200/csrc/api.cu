@@ -232,6 +232,7 @@ void me_destroy(me_ctx *ctx) {
   icp_close(ctx, false);
   nn_quantile_free(ctx);
   nn_region_free(ctx);
+  nn_surface_free(ctx);
   drift_close(ctx, false);
   if (ctx->copy_stream) { cudaStreamSynchronize(ctx->copy_stream); cudaStreamDestroy(ctx->copy_stream); }
   if (ctx->compute_mark) cudaEventDestroy(ctx->compute_mark);
@@ -1014,6 +1015,68 @@ int me_nn_regions(me_ctx *ctx, double region_size, me_region_row **rows, int64_t
   *rows = r;
   *n_regions = n;
   return ME_OK;
+}
+
+int me_surface_finalize(const me_nn_params *p, const double *host_block, int64_t n_est, int64_t n_gt, me_surface_result *out) {
+  if (!p || !host_block || !out) return ME_ERR_INVALID;
+  std::memset(out, 0, sizeof(*out));
+  me_nn_accum a, b;
+  std::memset(&a, 0, sizeof(a));
+  std::memset(&b, 0, sizeof(b));
+  decode_block(host_block, &a, &b, nullptr, nullptr);      // the NN-laid-out part: the five-level table of e
+  ME_TRY(me_nn_finalize(p, &a, &b, n_est, n_gt, &out->plane));
+  const double *x = host_block + 2 * kBlkNN, *mx = host_block + ME_SURFACE_BLOCK_SUM;
+  for (int q = 0; q < 2; ++q) {
+    me_surface_dir &D = q == 0 ? out->est_to_gt : out->gt_to_est;
+    D.n_no_normal = (int64_t)std::llround(x[4 * q]);
+    D.n_no_normal_nn = (int64_t)std::llround(x[4 * q + 1]);
+    D.n_nc = (int64_t)std::llround(x[4 * q + 2]);
+    D.normal_consistency = D.n_nc ? x[4 * q + 3] / x[4 * q + 2] : NAN;
+    D.max_e = mx[2 * q];
+    D.max_e_nn = mx[2 * q + 1];
+  }
+  out->normal_consistency = (out->est_to_gt.normal_consistency + out->gt_to_est.normal_consistency) / 2.0;
+  return ME_OK;
+}
+
+int me_nn_surface_begin(me_ctx *ctx, int32_t knn) {
+  ME_ENTER(ctx);
+  if (knn < 0 || knn > 64) return fail(ctx, ME_ERR_INVALID, "me_nn_surface*: knn must be 0 (the clouds' own normals) or in 1..64");
+  return nn_surface_begin(ctx, knn);
+}
+
+int me_nn_surface_normals_slice(me_ctx *ctx, int which, double **device_normals, int64_t *slice_points, int32_t *pending) {
+  ME_ENTER(ctx);
+  if (!cloud_id(which)) return fail(ctx, ME_ERR_INVALID, "bad cloud id");
+  if (!device_normals || !slice_points || !pending) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return nn_surface_normals_slice(ctx, which, device_normals, slice_points, pending);
+}
+
+int me_nn_surface_block(me_ctx *ctx, double **device_block, int32_t *n_sum, int32_t *n_max) {
+  ME_ENTER(ctx);
+  if (!device_block || !n_sum || !n_max) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return nn_surface_block(ctx, device_block, n_sum, n_max);
+}
+
+int me_nn_surface_end(me_ctx *ctx, me_surface_result *out) {
+  ME_ENTER(ctx);
+  if (!out) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return nn_surface_end(ctx, out);
+}
+
+int me_nn_surface(me_ctx *ctx, int32_t knn, me_surface_result *out) {
+  ME_ENTER(ctx);
+  if (!out) return fail(ctx, ME_ERR_INVALID, "null argument");
+  if (ctx->world != 1)
+    return fail(ctx, ME_ERR_INVALID, "me_nn_surface needs world == 1; use me_nn_surface_begin / _normals_slice / _block + all-reduce / _end");
+  ME_TRY(me_nn_surface_begin(ctx, knn));
+  double *d = nullptr;
+  int64_t s = 0;
+  int32_t pending = 0, n_sum = 0, n_max = 0;
+  ME_TRY(me_nn_surface_normals_slice(ctx, ME_CLOUD_EST, &d, &s, &pending));
+  ME_TRY(me_nn_surface_normals_slice(ctx, ME_CLOUD_GT, &d, &s, &pending));
+  ME_TRY(me_nn_surface_block(ctx, &d, &n_sum, &n_max));
+  return me_nn_surface_end(ctx, out);
 }
 
 int me_drift_begin(me_ctx *ctx, double region_size, double max_correspondence_distance, int32_t max_iteration,

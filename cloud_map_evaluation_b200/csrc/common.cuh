@@ -248,6 +248,19 @@ struct DriftRun {
   std::vector<double> h_blk;
 };
 
+// point-to-plane metrics (me_nn_surface_begin .. me_nn_surface_end, surface.cu): one fold of the NN records, the same calls
+// on every rank
+struct SurfaceRun {
+  bool open = false, done = false;     // done: the block holds this rank's fold
+  unsigned long long gen = 0;          // cloud_gen at me_nn_surface_begin
+  int knn = 0;
+  bool had_normals[2] = {false, false};       // the clouds' own normals
+  bool pending[2] = {false, false};           // working k-NN normals not estimated yet (me_nn_surface_normals_slice)
+  double *d_blk = nullptr;             // ME_SURFACE_BLOCK_SUM SUM values, then ME_SURFACE_BLOCK_MAX MAX values
+  double *d_part = nullptr;            // the fold's per-warp values
+  long long cap_part = 0;
+};
+
 // numpy's method="linear" position of probability p among n sorted values: h = (n - 1) p, k = floor(h), g = h - k
 inline void quantile_rank(long long n, double p, long long *k, double *g) {
   const double h = (double)(n - 1) * p;
@@ -332,6 +345,7 @@ struct me_ctx {
   me::QuantRun quant;                  // distance quantiles (me_nn_quantile*), from the same records
   me::RegionRun region;                // the per-region table (me_nn_region*), from the same records
   me::DriftRun drift;                  // the per-region drift loop (me_drift*)
+  me::SurfaceRun surface;              // point-to-plane metrics (me_nn_surface*), from the NN records
   std::string err;
 };
 
@@ -454,6 +468,12 @@ int drift_block(me_ctx *ctx, double **device_block, int32_t *n_sum);
 int drift_step(me_ctx *ctx, int32_t *done);
 int drift_end(me_ctx *ctx, me_drift_row *rows, int64_t capacity);
 void drift_close(me_ctx *ctx, bool restore);
+// point-to-plane metrics of the last me_eval_nn*'s records (knn checked by the caller) — me_nn_surface_* (surface.cu)
+int nn_surface_begin(me_ctx *ctx, int knn);
+int nn_surface_normals_slice(me_ctx *ctx, int which, double **d_normals, int64_t *slice_points, int32_t *pending);
+int nn_surface_block(me_ctx *ctx, double **device_block, int32_t *n_sum, int32_t *n_max);
+int nn_surface_end(me_ctx *ctx, me_surface_result *out);
+void nn_surface_free(me_ctx *ctx);
 // the accumulators go to the cloud's MME section of d_block
 int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors);
 

@@ -66,6 +66,33 @@ def regions_distributed(ctx, region_size, device, group=None):
     return ctx.region_end(n)
 
 
+def surface_distributed(ctx, device, knn=0, group=None):
+    """Point-to-plane metrics and normal consistency over every rank of the job (MapEvalB200.surface_metrics for world > 1):
+    every rank estimates its caller-index slice of a cloud's missing working normals, ONE in-place all-gather per such cloud,
+    then every rank folds its own records, ONE in-place SUM all-reduce of the block's sums (counts ride as fp64, exact) and
+    ONE MAX all-reduce of its maxima.  Every rank returns the same result."""
+    import torch
+    import torch.distributed as dist
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    rank = dist.get_rank(group) if dist.is_initialized() else 0
+    ctx.surface_begin(knn)
+    for which in (A.ME_CLOUD_EST, A.ME_CLOUD_GT):
+        ptr, s, pending = ctx.surface_normals_slice(which)
+        if pending:
+            ctx.synchronize()
+            buf = torch.as_tensor(_DeviceBlock(ptr, world * s * 3), device=device)
+            dist.all_gather_into_tensor(buf, buf[rank * s * 3:(rank + 1) * s * 3], group=group)
+            torch.cuda.current_stream(device).synchronize()
+    ptr, n_sum, n_max = ctx.surface_block()
+    if world > 1:
+        ctx.synchronize()
+        t = torch.as_tensor(_DeviceBlock(ptr, n_sum + n_max), device=device)
+        dist.all_reduce(t[:n_sum], group=group)
+        dist.all_reduce(t[n_sum:], op=dist.ReduceOp.MAX, group=group)
+        torch.cuda.current_stream(device).synchronize()
+    return ctx.surface_end()
+
+
 def quantiles_distributed(ctx, device, p, population=A.ME_DIST_KEPT, group=None):
     """Exact distance quantiles of the last NN evaluation over every rank of the job (MapEvalB200.distance_quantiles for
     world > 1): the selection loop with ONE in-place SUM all-reduce of the pass's integer counts (as fp64, exact) per pass.

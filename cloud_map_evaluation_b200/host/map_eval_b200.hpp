@@ -100,6 +100,10 @@ struct Param {   // map_eval.h:60-116
   // drift per region: every region floor(x / drift_region_size) of the estimate aligned to the ground truth on its own
   // (me_drift*: point-to-point ICP per region, R = icp_max_distance, ICP's criteria), written to region_drift.txt; absent or 0 = off
   double drift_region_size_ = 0.0;
+  // point-to-plane AC / COM / CD / F1 / IoU and normal consistency, written to surface_metrics.txt (me_nn_surface*: no new
+  // sweep); the clouds' normals where the files carry them, else working k-NN normals with surface_normals_knn neighbours
+  bool surface_metrics_ = false;
+  int surface_normals_knn_ = 20;
 };
 
 // map_eval_main.cpp:120-208
@@ -176,6 +180,12 @@ inline Param loadParametersFromYAML(const std::string &yaml_file_path) {
         throw std::runtime_error("drift_region_size must be finite and >= 0 (0 = off), not " +
                                  config["drift_region_size"].as<std::string>());
     }
+    if (config["surface_metrics"]) param.surface_metrics_ = config["surface_metrics"].as<bool>();
+    if (config["surface_normals_knn"]) {
+      param.surface_normals_knn_ = config["surface_normals_knn"].as<int>();
+      if (param.surface_normals_knn_ < 1 || param.surface_normals_knn_ > 64)
+        throw std::runtime_error("surface_normals_knn must be in 1..64, not " + config["surface_normals_knn"].as<std::string>());
+    }
     return param;
   } catch (const std::exception &e) {
     std::cerr << "Error loading parameters: " << e.what() << std::endl;
@@ -206,7 +216,8 @@ inline void dumpParam(const Param &p, std::ostream &os) {
      << "\naccuracy_curve_steps=" << p.accuracy_curve_steps_ << "\naccuracy_curve_max=" << p.accuracy_curve_max_
      << "\ndistance_quantiles=";
   for (size_t i = 0; i < p.distance_quantiles_.size(); ++i) os << (i ? "," : "") << p.distance_quantiles_[i];
-  os << "\nregion_size=" << p.region_size_ << "\ndrift_region_size=" << p.drift_region_size_ << "\n";
+  os << "\nregion_size=" << p.region_size_ << "\ndrift_region_size=" << p.drift_region_size_ << "\nsurface_metrics=" << p.surface_metrics_
+     << "\nsurface_normals_knn=" << p.surface_normals_knn_ << "\n";
 }
 
 // Eigen's default IOFormat for `vec.transpose()`: coefficients right-aligned to a common width, one space apart
@@ -349,6 +360,7 @@ class MapEvalB200 {
   int accuracyCurve(const me_nn_params &p, const me_nn_accum &e2g, const me_nn_accum &g2e);
   int distanceQuantiles();
   int regionErrors();
+  int surfaceMetrics();
   int regionDrift();
   GpuGroup gpus_;            // one context per GPU; rank r evaluates the r-th shard of every sweep's query range
   me_ctx *ctx_ = nullptr;    // = gpus_.ctx(0): the voxel stage and the single-GPU calls
@@ -369,8 +381,10 @@ inline int MapEvalB200::process() {
     return -1;
   }
   // point-to-plane ICP needs normals on the target cloud, which can only come from the ground-truth file; generalized ICP
-  // uses the normals of either file when it carries them (InitializePointCloudForGeneralizedICP)
-  const bool load_normals = !param_.evaluate_using_initial_ && (param_.evaluation_method_ == 1 || param_.evaluation_method_ == 2);
+  // uses the normals of either file when it carries them (InitializePointCloudForGeneralizedICP); the surface metrics use them
+  // on either path
+  const bool load_normals =
+      (!param_.evaluate_using_initial_ && (param_.evaluation_method_ == 1 || param_.evaluation_method_ == 2)) || param_.surface_metrics_;
   std::string file_extension = param_.map_gt_path_.substr(param_.map_gt_path_.find_last_of(".") + 1);
   bool gt_ok = false;
   if (file_extension == "pcd") gt_ok = cloud_io::read_pcd(param_.map_gt_path_, gt_3d_, &err, load_normals ? &gt_normals_ : nullptr);
@@ -633,6 +647,7 @@ inline int MapEvalB200::calculateMetricsWithInitialMatrix() {
   if (param_.accuracy_curve_steps_ > 0 && accuracyCurve(p, e2g, g2e) != 0) return -1;
   if (!param_.distance_quantiles_.empty() && distanceQuantiles() != 0) return -1;
   if (param_.region_size_ > 0.0 && regionErrors() != 0) return -1;
+  if (param_.surface_metrics_ && surfaceMetrics() != 0) return -1;
   if (nn_.gt_to_est.n_ub > 0)
     std::cerr << "WARNING: " << nn_.gt_to_est.n_ub << " gt->est pairs index past the end of a cloud (the reference reads out of "
                  "bounds there, map_eval.cpp:1233 vs :1093-1094: undefined behaviour); they are left out of the gt->est statistics, "
@@ -785,6 +800,81 @@ inline int MapEvalB200::regionErrors() {
     f << "\n";
   }
   std::cout << "INFO: errors of " << n[0] << " regions of edge " << s << " saved to " << path << std::endl;
+  return 0;
+}
+
+// point-to-plane metrics: the pass's NN records against the tangent plane of each neighbour (the me_nn_surface_* loop on every
+// GPU: one grouped NCCL all-gather per cloud that needs working k-NN normals, then one grouped SUM all-reduce of the block's
+// sums and one MAX all-reduce of its maxima) -> surface_metrics.txt next to map_results.txt
+inline int MapEvalB200::surfaceMetrics() {
+  const int G = gpus_.size(), knn = param_.surface_normals_knn_;
+  bool own[2];          // the cloud holds normals (from its file, averaged by VoxelDownSample); else working k-NN normals
+  {
+    std::vector<double> tmp((size_t)std::max(n_est_, n_gt_) * 3);
+    for (int w = 0; w < 2; ++w) own[w] = me_get_normals(ctx_, w, tmp.data()) == ME_OK;
+  }
+  if (gpus_.for_each([&](int, me_ctx *c) { return me_nn_surface_begin(c, knn); }) != ME_OK) return fail("me_nn_surface_begin");
+  for (int w : {ME_CLOUD_EST, ME_CLOUD_GT}) {
+    std::vector<double *> nrm(G, nullptr);
+    std::vector<int64_t> s(G, 0);
+    std::vector<int32_t> pend(G, 0);
+    if (gpus_.for_each([&](int r, me_ctx *c) {
+          const int rc = me_nn_surface_normals_slice(c, w, &nrm[r], &s[r], &pend[r]);
+          return rc != ME_OK ? rc : me_synchronize(c);
+        }) != ME_OK)
+      return fail("me_nn_surface_normals_slice");
+    if (pend[0] && !gpus_.allgather_device(nrm, (size_t)s[0] * 3)) return fail("all-gather of the working normals");
+  }
+  std::vector<double *> ptr(G, nullptr), ptr_max(G, nullptr);
+  std::vector<int32_t> n_sum(G, 0), n_max(G, 0);
+  if (gpus_.for_each([&](int r, me_ctx *c) {
+        const int rc = me_nn_surface_block(c, &ptr[r], &n_sum[r], &n_max[r]);
+        ptr_max[r] = ptr[r] + n_sum[r];
+        return rc != ME_OK ? rc : me_synchronize(c);
+      }) != ME_OK)
+    return fail("me_nn_surface_block");
+  if (!gpus_.allreduce_device(ptr, (size_t)n_sum[0], ncclSum) || !gpus_.allreduce_device(ptr_max, (size_t)n_max[0], ncclMax))
+    return fail("all-reduce of the surface block");
+  me_surface_result res;
+  if (gpus_.for_each([&](int r, me_ctx *c) {
+        me_surface_result mine;
+        const int rc = me_nn_surface_end(c, &mine);
+        if (r == 0) res = mine;
+        return rc;
+      }) != ME_OK)
+    return fail("me_nn_surface_end");
+  const std::string path = results_subfolder + "surface_metrics.txt";
+  std::ofstream f(path);
+  if (!f.is_open()) {
+    std::cerr << "ERROR: cannot write " << path << std::endl;
+    return -1;
+  }
+  auto source = [&](int w) { return own[w] ? std::string("file") : "k-NN (k = " + std::to_string(knn) + ")"; };
+  f << "# e = |(p - t) . n| / |n|: the distance of the query point p to the tangent plane of its geometric nearest neighbour t "
+       "(normal n); normal consistency = min(1, |m . n| / (|m| |n|)) with the query's normal m; mean_nn = sum of e over every "
+       "query / query count; est normals: " << source(ME_CLOUD_EST) << "; gt normals: " << source(ME_CLOUD_GT) << "\n";
+  f << "direction n_corr n_no_normal";
+  for (const char *field : {"n_inlier", "mean", "rmse", "fitness", "sigma"})
+    for (int k = 1; k <= 5; ++k) f << " " << field << "_" << k;
+  f << " mean_nn max_e max_e_nn n_nc normal_consistency\n" << std::fixed << std::setprecision(15);
+  for (int q = 0; q < 2; ++q) {
+    const me_dir_result &d = q == 0 ? res.plane.est_to_gt : res.plane.gt_to_est;
+    const me_surface_dir &x = q == 0 ? res.est_to_gt : res.gt_to_est;
+    f << (q == 0 ? "est_to_gt" : "gt_to_est") << " " << d.n_corr << " " << x.n_no_normal;
+    for (int k = 0; k < 5; ++k) f << " " << d.n_inlier[k];
+    for (const double *v : {d.mean, d.rmse, d.fitness, d.sigma})
+      for (int k = 0; k < 5; ++k) f << " " << v[k];
+    f << " " << d.sum_nn_dist / (double)d.n_source << " " << x.max_e << " " << x.max_e_nn << " " << x.n_nc << " "
+      << x.normal_consistency << "\n";
+  }
+  for (const char *field : {"cd", "f1", "iou"})
+    for (int k = 1; k <= 5; ++k) f << field << "_" << k << " ";
+  f << "full_cd normal_consistency\n";
+  for (const double *v : {res.plane.cd, res.plane.f1, res.plane.iou})
+    for (int k = 0; k < 5; ++k) f << v[k] << " ";
+  f << res.plane.full_cd << " " << res.normal_consistency << "\n";
+  std::cout << "INFO: point-to-plane CD at level 1: " << res.plane.cd[0] << ", normal consistency: " << res.normal_consistency
+            << "; surface metrics saved to " << path << std::endl;
   return 0;
 }
 
@@ -951,6 +1041,7 @@ inline int MapEvalB200::performRegistration() {
   if (param_.accuracy_curve_steps_ > 0 && accuracyCurve(p, e2g, g2e) != 0) return -1;
   if (!param_.distance_quantiles_.empty() && distanceQuantiles() != 0) return -1;
   if (param_.region_size_ > 0.0 && regionErrors() != 0) return -1;
+  if (param_.surface_metrics_ && surfaceMetrics() != 0) return -1;
   if (param_.save_immediate_result_ && renderDistances(true) != 0) return -1;
   if (param_.drift_region_size_ > 0.0 && regionDrift() != 0) return -1;
   full_chamfer_dist = nn_.full_cd;

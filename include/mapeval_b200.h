@@ -504,6 +504,60 @@ ME_API int  me_nn_regions(me_ctx *ctx, double region_size, me_region_row **rows,
 ME_API int  me_region_finalize(int64_t n_regions, double region_size, const int64_t *index, const int64_t *n_est,
                                const int64_t *n_gt, const double *host_block, me_region_row *rows);   /* host only */
 
+/* ---- point-to-plane metrics and normal consistency ---------------------------------------------------------------------
+ * From the per-query records of the LAST me_eval_nn* call (stale as for me_nn_curve*), with that call's tau, cut-off mode and
+ * want_full_cd: the five-level statistics with the point-to-point distance d replaced by the distance of the query point to
+ * the tangent plane of its nearest neighbour, and the agreement of the two normals of every pair.  No reference counterpart.
+ * Direction q (query cloud q, reference cloud 1 - q) walks its records with GEOMETRIC pairing always: under
+ * ME_PAIRING_AS_WRITTEN the gt->est pair is a pair of swapped indices, whose tangent plane means nothing, so n_corr of the
+ * gt->est table equals me_eval_nn's only under geometric pairing.  For a record with neighbour j >= 0: p = query point,
+ * t = reference point j (caller order), n = reference normal j, m = the query's own normal.  A normal is usable iff its
+ * squared norm (x*x + (y*y + z*z)) is finite and > 0.  With d = p - t, every operation rounded on its own (no FMA):
+ *   e = |(dx nx + dy ny) + dz nz| / sqrt(|n|^2),   c = min(1, |(mx nx + my ny) + mz nz| / (sqrt(|m|^2) sqrt(|n|^2))).
+ * (the min is fmin: a NaN ratio counts as 1).
+ * A kept pair (the five-level pass's cut-off on the record's d2) with usable n counts in n_corr and its e goes where the
+ * five-level pass puts d (n_inlier / sum_d / sum_d2 per level with e <= tau_k, the rank's moment slot); with unusable n it
+ * counts in n_no_normal and nowhere else.  A kept pair with usable n and m adds 1 to n_nc and c to sum_c.  After
+ * want_full_cd = 1 every query with j >= 0 and usable n adds e to sum_nn_dist and to max_e_nn (unusable n: n_no_normal_nn).
+ * max_e is the largest kept e; n_query is the five-level pass's; n_ub and n_far are 0.
+ * Device block: ME_SURFACE_BLOCK_SUM SUM-reducible values — the two directions laid out as the NN section of the accumulator
+ * block (ME_NN_ACCUM_I64 + ME_NN_ACCUM_F64 each, me_nn_accum's fields as fp64), then per direction n_no_normal,
+ * n_no_normal_nn, n_nc, sum_c — and ME_SURFACE_BLOCK_MAX MAX-reducible values, per direction max_e, max_e_nn.  No
+ * floating-point atomics: two calls on one device, world and layout give the same bits; counts and maxima are the same for
+ * any world and layout.
+ * Normals (knn): 0 — both clouds must hold normals (me_set_normals / me_estimate_normals, a file's, averaged by
+ * me_voxel_downsample); 1..64 — a cloud without normals gets exact k-NN normals (me_estimate_normals' rule) as a working
+ * copy: the cloud still has no normals afterwards, after a failure too.  A working estimate needs the replicated layout.
+ * The loop: me_nn_surface_begin checks; me_nn_surface_normals_slice per cloud estimates this rank's caller-index slice of a
+ * working normal set into the buffer it returns (*pending = 1: all-gather slice_points * 3 fp64 per rank in place after
+ * me_synchronize; 0: nothing to do); me_nn_surface_block folds the records into the block on its first call (SUM-reduce the
+ * first n_sum values and MAX-reduce the next n_max in place); me_nn_surface_end reads the reduced block.  The records are
+ * only read.  Refused: knn outside 0..64, stale records, missing normals with knn = 0, a working estimate on ME_LAYOUT_SLAB,
+ * begin while a registration or drift loop is open, calls out of order, and a cloud changed between begin and end.
+ * me_nn_surface: the whole loop at world 1.  me_surface_finalize (host only): the result from a reduced host block;
+ * plane is me_nn_finalize of the NN-laid-out part. */
+#define ME_SURFACE_BLOCK_SUM (2 * (ME_NN_ACCUM_I64 + ME_NN_ACCUM_F64) + 8)
+#define ME_SURFACE_BLOCK_MAX 4
+typedef struct {
+  int64_t n_no_normal;                          /* kept pairs without a usable reference normal */
+  int64_t n_no_normal_nn;                       /* full-CD queries without a usable reference normal */
+  int64_t n_nc;                                 /* kept pairs with both normals usable */
+  double  normal_consistency;                   /* sum_c / n_nc; NaN when n_nc = 0 */
+  double  max_e, max_e_nn;                      /* largest kept e, largest full-CD e; 0 for an empty set */
+} me_surface_dir;
+typedef struct {
+  me_nn_result   plane;                         /* the five-level table of e; full_cd from the e of every query */
+  me_surface_dir est_to_gt, gt_to_est;
+  double         normal_consistency;            /* mean of the two directions'; NaN if either is NaN */
+} me_surface_result;
+ME_API int  me_nn_surface_begin(me_ctx *ctx, int32_t knn);
+ME_API int  me_nn_surface_normals_slice(me_ctx *ctx, int which, double **device_normals, int64_t *slice_points, int32_t *pending);
+ME_API int  me_nn_surface_block(me_ctx *ctx, double **device_block, int32_t *n_sum, int32_t *n_max);
+ME_API int  me_nn_surface_end(me_ctx *ctx, me_surface_result *out);
+ME_API int  me_nn_surface(me_ctx *ctx, int32_t knn, me_surface_result *out);
+ME_API int  me_surface_finalize(const me_nn_params *p, const double *host_block, int64_t n_est, int64_t n_gt,
+                                me_surface_result *out);   /* host only */
+
 /* ---- drift per region: every region of the estimated cloud aligned to the ground truth on its own --------------------------
  * Separates a region that is shifted or turned as a whole (drift) from one that is noisy or smeared (damage): a rigid
  * point-to-point ICP per region, all of them in one pass over the cloud per iteration.
