@@ -204,6 +204,28 @@ class me_drift_row(C.Structure):
                 ("iterations", C.c_int32), ("status", C.c_int32)]
 
 
+# local map consistency: mean plane variance beside MME, whole map and per region (me_consistency*)
+ME_CONSISTENCY_SUM_FIELDS = 6   # per region: n_query n_valid n_pv sum_entropy sum_pv sum_sqrt_pv
+ME_CONSISTENCY_MAX_FIELDS = 1   # per region: max_pv
+ME_CONSISTENCY_WALK = 0         # me_consistency_kernel
+CONSISTENCY_KERNEL_NAMES = {ME_CONSISTENCY_WALK: "WALK"}
+
+
+class me_consistency_row(C.Structure):
+    _fields_ = [("index", C.c_int64 * 3), ("min", C.c_double * 3), ("max", C.c_double * 3), ("n_points", C.c_int64),
+                ("n_query", C.c_int64), ("n_valid", C.c_int64), ("n_pv", C.c_int64), ("sum_entropy", C.c_double),
+                ("sum_pv", C.c_double), ("sum_sqrt_pv", C.c_double), ("mme", C.c_double), ("mpv", C.c_double),
+                ("mean_plane_std", C.c_double), ("max_pv", C.c_double)]
+
+
+class me_consistency_result(C.Structure):
+    _fields_ = [("radius", C.c_double), ("region_size", C.c_double), ("min_neighbors", C.c_int32), ("kernel", C.c_int32),
+                ("rings", C.c_int32), ("solo", C.c_int32), ("n_regions", C.c_int64), ("n_points", C.c_int64),
+                ("n_query", C.c_int64), ("n_valid", C.c_int64), ("n_pv", C.c_int64), ("sum_entropy", C.c_double),
+                ("sum_pv", C.c_double), ("sum_sqrt_pv", C.c_double), ("mme", C.c_double), ("mpv", C.c_double),
+                ("mean_plane_std", C.c_double), ("max_pv", C.c_double)]
+
+
 class me_mme_accum(C.Structure):
     _fields_ = [("n_query", C.c_int64), ("n_valid", C.c_int64), ("sum_entropy", C.c_double),
                 ("min_entropy", C.c_double), ("max_entropy", C.c_double)]

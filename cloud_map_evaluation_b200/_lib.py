@@ -31,6 +31,8 @@ SYMBOLS = (
     "me_drift_begin", "me_drift_block", "me_drift_step", "me_drift_end", "me_drift",
     "me_nn_surface_begin", "me_nn_surface_normals_slice", "me_nn_surface_block", "me_nn_surface_end", "me_nn_surface",
     "me_surface_finalize",
+    "me_consistency_begin", "me_consistency_block", "me_consistency_end", "me_consistency", "me_consistency_finalize",
+    "me_get_consistency_points",
 )
 
 _lib = None
@@ -145,6 +147,14 @@ def load():
     L.me_nn_surface_end.argtypes = [ctx, C.POINTER(A.me_surface_result)]
     L.me_nn_surface.argtypes = [ctx, C.c_int32, C.POINTER(A.me_surface_result)]
     L.me_surface_finalize.argtypes = [C.POINTER(A.me_nn_params), dp, C.c_int64, C.c_int64, C.POINTER(A.me_surface_result)]
+    L.me_consistency_begin.argtypes = [ctx, C.c_int, C.c_double, C.c_int32, C.c_double, i64p]
+    L.me_consistency_block.argtypes = [ctx, C.POINTER(dp), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    L.me_consistency_end.argtypes = [ctx, C.c_void_p, C.c_int64, C.POINTER(A.me_consistency_result)]
+    L.me_consistency.argtypes = [ctx, C.c_int, C.c_double, C.c_int32, C.c_double, C.POINTER(C.c_void_p), i64p,
+                                 C.POINTER(A.me_consistency_result)]
+    L.me_consistency_finalize.argtypes = [C.c_int64, C.c_double, i64p, i64p, C.c_int64, dp, C.c_void_p,
+                                          C.POINTER(A.me_consistency_result)]
+    L.me_get_consistency_points.argtypes = [ctx, C.c_int, C.c_void_p, C.c_void_p]
     L.me_kernel_trace.argtypes = [ctx, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.c_int32]
     if L.me_abi_version() != A.ME_ABI_VERSION:
         raise RuntimeError("libmapeval_b200.so ABI version mismatch")

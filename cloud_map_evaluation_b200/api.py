@@ -194,6 +194,46 @@ def drift_dict(a):
     return out
 
 
+# me_consistency_row as a numpy record (8-byte fields only, so no padding)
+_CONS_ROW_DT = np.dtype([("index", "<i8", 3), ("min", "<f8", 3), ("max", "<f8", 3), ("n_points", "<i8"), ("n_query", "<i8"),
+                         ("n_valid", "<i8"), ("n_pv", "<i8"), ("sum_entropy", "<f8"), ("sum_pv", "<f8"), ("sum_sqrt_pv", "<f8"),
+                         ("mme", "<f8"), ("mpv", "<f8"), ("mean_plane_std", "<f8"), ("max_pv", "<f8")])
+assert _CONS_ROW_DT.itemsize == C.sizeof(A.me_consistency_row) and \
+    _CONS_ROW_DT.names == tuple(f[0] for f in A.me_consistency_row._fields_)
+
+
+def consistency_dict(rows, whole):
+    """me_consistency_row records (numpy, _CONS_ROW_DT) and the me_consistency_result -> {'whole': {field: value}, 'kernel'
+    (ME_CONSISTENCY_* name), then one array per row field: 'index' / 'min' / 'max' (n, 3), 'n_points', ..., 'max_pv'}"""
+    out = {name: np.array(rows[name]) for name in _CONS_ROW_DT.names}
+    out["whole"] = {f[0]: getattr(whole, f[0]) for f in A.me_consistency_result._fields_}
+    out["kernel"] = A.CONSISTENCY_KERNEL_NAMES.get(whole.kernel, str(whole.kernel))
+    return out
+
+
+def consistency_finalize(region_size, index, n_points, n_total, block):
+    """me_consistency_finalize (host only): the rows of n regions and the whole-map result from a reduced host block
+    (ME_CONSISTENCY_SUM_FIELDS SUM values per region, then ME_CONSISTENCY_MAX_FIELDS MAX values; one region, the whole map,
+    at region_size 0 with no index), the region indices (n, 3), the per-region point counts and the cloud size; as
+    consistency_dict (radius, min_neighbors, kernel, rings and solo are 0)"""
+    L = _lib.load()
+    idx = np.ascontiguousarray(index, dtype=np.int64).reshape(-1, 3)
+    n = idx.shape[0]
+    npts = np.ascontiguousarray(n_points, dtype=np.int64).reshape(-1)
+    blk = np.ascontiguousarray(block, dtype=np.float64).reshape(-1)
+    if npts.size != n or blk.size != (A.ME_CONSISTENCY_SUM_FIELDS + A.ME_CONSISTENCY_MAX_FIELDS) * max(n, 1):
+        raise ValueError("one index triple and one point count per region, and ME_CONSISTENCY_SUM_FIELDS + "
+                         "ME_CONSISTENCY_MAX_FIELDS values per region (one region at region_size 0)")
+    rows = np.zeros(max(n, 1), _CONS_ROW_DT)
+    whole = A.me_consistency_result()
+    i64 = C.POINTER(C.c_int64)
+    rc = L.me_consistency_finalize(n, float(region_size), idx.ctypes.data_as(i64), npts.ctypes.data_as(i64), int(n_total),
+                                   blk.ctypes.data_as(C.POINTER(C.c_double)), rows.ctypes.data_as(C.c_void_p), C.byref(whole))
+    if rc != A.ME_OK:
+        raise MapEvalError(rc, "me_consistency_finalize: n >= 0, region_size finite and >= 0, n = 0 exactly at region_size 0")
+    return consistency_dict(rows[:n], whole)
+
+
 class MapEvalB200:
     """One context = one GPU.  rank/world select this context's contiguous query range (multi-GPU sharding)."""
 
@@ -614,6 +654,59 @@ class MapEvalB200:
         rows = np.zeros(max(int(n_regions), 1), _DRIFT_ROW_DT)
         self._check(self._L.me_drift_end(self._ctx, rows.ctypes.data_as(C.POINTER(A.me_drift_row)), int(n_regions)))
         return drift_dict(rows[:int(n_regions)])
+
+    def local_consistency(self, which, radius, min_neighbors=10, region_size=0.0):
+        """Local map consistency of cloud `which` without a ground truth (me_consistency, world 1): per point MME's radius
+        neighbourhood, its entropy and its plane variance (the smallest eigenvalue of the neighbourhood covariance, m^2).
+        Returns consistency_dict's dict: 'whole' (mme, mpv, mean_plane_std, max_pv, the counts, and which sweep ran: kernel,
+        rings, solo) and one row per occupied region floor(x / region_size) when region_size > 0.  The sweep may lay the cloud
+        out again (its NN records are then stale).  Multi-GPU: dist.consistency_distributed."""
+        rows = C.c_void_p()
+        n = C.c_int64(0)
+        whole = A.me_consistency_result()
+        self._check(self._L.me_consistency(self._ctx, int(which), float(radius), int(min_neighbors), float(region_size),
+                                           C.byref(rows), C.byref(n), C.byref(whole)))
+        try:
+            nb = n.value * _CONS_ROW_DT.itemsize
+            a = np.frombuffer((C.c_char * nb).from_address(rows.value), _CONS_ROW_DT).copy() if nb else \
+                np.zeros(0, _CONS_ROW_DT)
+            return consistency_dict(a, whole)
+        finally:
+            if rows.value:
+                self._L.me_free(rows)
+
+    def consistency_begin(self, which, radius, min_neighbors=10, region_size=0.0):
+        """me_consistency_begin: sweeps this rank's query range and folds it by region; returns the row count (0 at
+        region_size 0)"""
+        n = C.c_int64(0)
+        self._check(self._L.me_consistency_begin(self._ctx, int(which), float(radius), int(min_neighbors), float(region_size),
+                                                 C.byref(n)))
+        return n.value
+
+    def consistency_block(self):
+        """(device pointer, n_sum, n_max) of the block: SUM-reduce its first n_sum values and MAX-reduce the next n_max in
+        place (after synchronize())"""
+        ptr = C.POINTER(C.c_double)()
+        n_sum, n_max = C.c_int32(0), C.c_int32(0)
+        self._check(self._L.me_consistency_block(self._ctx, C.byref(ptr), C.byref(n_sum), C.byref(n_max)))
+        return C.cast(ptr, C.c_void_p).value, n_sum.value, n_max.value
+
+    def consistency_end(self, n_regions):
+        """the rows and the whole-map result from the reduced block, as local_consistency"""
+        rows = np.zeros(max(int(n_regions), 1), _CONS_ROW_DT)
+        whole = A.me_consistency_result()
+        self._check(self._L.me_consistency_end(self._ctx, rows.ctypes.data_as(C.c_void_p), int(n_regions), C.byref(whole)))
+        return consistency_dict(rows[:int(n_regions)], whole)
+
+    def get_consistency_points(self, which):
+        """(entropy, plane_variance) per point of the last consistency call on cloud `which`, caller order: 0 / NaN where
+        invalid (k < min_neighbors) and at points another rank evaluated"""
+        n = self.n[which]
+        e = np.zeros(n, np.float64)
+        v = np.zeros(n, np.float64)
+        self._check(self._L.me_get_consistency_points(self._ctx, int(which), e.ctypes.data_as(C.c_void_p),
+                                                      v.ctypes.data_as(C.c_void_p)))
+        return e, v
 
     def get_nn(self, which_query):
         n = self.n[which_query]

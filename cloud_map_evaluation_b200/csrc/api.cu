@@ -233,6 +233,7 @@ void me_destroy(me_ctx *ctx) {
   nn_quantile_free(ctx);
   nn_region_free(ctx);
   nn_surface_free(ctx);
+  consistency_free(ctx);
   drift_close(ctx, false);
   if (ctx->copy_stream) { cudaStreamSynchronize(ctx->copy_stream); cudaStreamDestroy(ctx->copy_stream); }
   if (ctx->compute_mark) cudaEventDestroy(ctx->compute_mark);
@@ -1077,6 +1078,111 @@ int me_nn_surface(me_ctx *ctx, int32_t knn, me_surface_result *out) {
   ME_TRY(me_nn_surface_normals_slice(ctx, ME_CLOUD_GT, &d, &s, &pending));
   ME_TRY(me_nn_surface_block(ctx, &d, &n_sum, &n_max));
   return me_nn_surface_end(ctx, out);
+}
+
+// the means of one region (or of the whole map) from its counts and sums: me_consistency_finalize
+static void consistency_means(int64_t n_valid, int64_t n_pv, double sum_e, double sum_v, double sum_sv, double max_v, double *mme,
+                              double *mpv, double *mean_std, double *max_pv) {
+  *mme = n_valid > 0 ? sum_e / (double)n_valid : 0.0;      // as me_mme_finalize
+  *mpv = n_pv > 0 ? sum_v / (double)n_pv : NAN;
+  *mean_std = n_pv > 0 ? sum_sv / (double)n_pv : NAN;
+  *max_pv = n_pv > 0 ? max_v : NAN;
+}
+
+int me_consistency_finalize(int64_t n_regions, double region_size, const int64_t *index, const int64_t *n_points, int64_t n_total,
+                            const double *host_block, me_consistency_row *rows, me_consistency_result *whole) {
+  if (!host_block || !whole || n_regions < 0 || n_total < 0 || !(std::isfinite(region_size) && region_size >= 0.0)) return ME_ERR_INVALID;
+  if ((region_size == 0.0) != (n_regions == 0)) return ME_ERR_INVALID;
+  if (n_regions > 0 && (!index || !n_points || !rows)) return ME_ERR_INVALID;
+  const int S = ME_CONSISTENCY_SUM_FIELDS;
+  const int64_t B = std::max<int64_t>(n_regions, 1);      // s = 0: the block holds one region, the whole map
+  const double *mx = host_block + (size_t)S * B;
+  me_consistency_result &W = *whole;
+  std::memset(&W, 0, sizeof(W));
+  W.region_size = region_size;
+  W.n_regions = n_regions;
+  W.n_points = n_total;
+  double max_v = 0.0;
+  for (int64_t r = 0; r < B; ++r) {      // the whole map: the regions' sums in list order
+    const double *v = host_block + (size_t)r * S;
+    const int64_t nq = (int64_t)v[0], nv = (int64_t)v[1], np = (int64_t)v[2];
+    W.n_query += nq; W.n_valid += nv; W.n_pv += np;
+    W.sum_entropy += v[3]; W.sum_pv += v[4]; W.sum_sqrt_pv += v[5];
+    max_v = std::fmax(max_v, mx[r * ME_CONSISTENCY_MAX_FIELDS]);
+    if (n_regions == 0) continue;
+    me_consistency_row &R = rows[r];
+    std::memset(&R, 0, sizeof(R));
+    for (int a = 0; a < 3; ++a) {
+      R.index[a] = index[3 * r + a];
+      R.min[a] = (double)R.index[a] * region_size;
+      R.max[a] = (double)(R.index[a] + 1) * region_size;
+    }
+    R.n_points = n_points[r];
+    R.n_query = nq; R.n_valid = nv; R.n_pv = np;
+    R.sum_entropy = v[3]; R.sum_pv = v[4]; R.sum_sqrt_pv = v[5];
+    consistency_means(nv, np, v[3], v[4], v[5], mx[r * ME_CONSISTENCY_MAX_FIELDS], &R.mme, &R.mpv, &R.mean_plane_std, &R.max_pv);
+  }
+  consistency_means(W.n_valid, W.n_pv, W.sum_entropy, W.sum_pv, W.sum_sqrt_pv, max_v, &W.mme, &W.mpv, &W.mean_plane_std, &W.max_pv);
+  return ME_OK;
+}
+
+int me_consistency_begin(me_ctx *ctx, int which, double radius, int32_t min_neighbors, double region_size, int64_t *n_regions) {
+  ME_ENTER(ctx);
+  if (!n_regions) return fail(ctx, ME_ERR_INVALID, "null argument");
+  *n_regions = 0;
+  ctx->consistency.open = false;
+  if (!cloud_id(which)) return fail(ctx, ME_ERR_INVALID, "me_consistency_begin: which must be ME_CLOUD_EST or ME_CLOUD_GT");
+  if (!(std::isfinite(radius) && radius > 0.0)) return fail(ctx, ME_ERR_INVALID, "me_consistency_begin: radius must be finite and > 0");
+  if (min_neighbors < 3) return fail(ctx, ME_ERR_INVALID, "me_consistency_begin: min_neighbors must be >= 3");
+  if (!(std::isfinite(region_size) && region_size >= 0.0))
+    return fail(ctx, ME_ERR_INVALID, "me_consistency_begin: region_size must be finite and >= 0 (0: the whole map only)");
+  return consistency_begin(ctx, which, radius, min_neighbors, region_size, n_regions);
+}
+
+int me_consistency_block(me_ctx *ctx, double **device_block, int32_t *n_sum, int32_t *n_max) {
+  ME_ENTER(ctx);
+  if (!device_block || !n_sum || !n_max) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return consistency_block(ctx, device_block, n_sum, n_max);
+}
+
+int me_consistency_end(me_ctx *ctx, me_consistency_row *rows, int64_t capacity, me_consistency_result *whole) {
+  ME_ENTER(ctx);
+  if (!whole) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return consistency_end(ctx, rows, capacity, whole);
+}
+
+int me_consistency(me_ctx *ctx, int which, double radius, int32_t min_neighbors, double region_size, me_consistency_row **rows,
+                   int64_t *n_regions, me_consistency_result *whole) {
+  ME_ENTER(ctx);
+  if (!rows || !n_regions || !whole) return fail(ctx, ME_ERR_INVALID, "null argument");
+  *rows = nullptr;
+  *n_regions = 0;
+  if (ctx->world != 1)
+    return fail(ctx, ME_ERR_INVALID, "me_consistency needs world == 1; use me_consistency_begin / _block + all-reduce / _end");
+  int64_t n = 0;
+  ME_TRY(me_consistency_begin(ctx, which, radius, min_neighbors, region_size, &n));
+  me_consistency_row *r = nullptr;
+  if (n > 0) {
+    r = (me_consistency_row *)std::malloc((size_t)n * sizeof(me_consistency_row));
+    if (!r) {
+      ctx->consistency.open = false;
+      return fail(ctx, ME_ERR_NOMEM, "me_consistency: host allocation of the rows failed");
+    }
+  }
+  const int rc = me_consistency_end(ctx, r, n, whole);
+  if (rc != ME_OK) {
+    std::free(r);
+    return rc;
+  }
+  *rows = r;
+  *n_regions = n;
+  return ME_OK;
+}
+
+int me_get_consistency_points(me_ctx *ctx, int which, double *entropy, double *plane_variance) {
+  ME_ENTER(ctx);
+  if (!cloud_id(which)) return fail(ctx, ME_ERR_INVALID, "bad cloud id");
+  return consistency_points(ctx, which, entropy, plane_variance);
 }
 
 int me_drift_begin(me_ctx *ctx, double region_size, double max_correspondence_distance, int32_t max_iteration,

@@ -261,6 +261,27 @@ struct SurfaceRun {
   long long cap_part = 0;
 };
 
+// local map consistency (me_consistency_begin .. me_consistency_end, consistency.cu): the per-point values of the last call
+// per cloud, and the block of the open call, the same length on every rank
+struct ConsistencyRun {
+  bool open = false;
+  unsigned long long gen = 0;          // cloud_gen at me_consistency_begin
+  int which = 0, min_neighbors = 0, kernel = 0, rings = 0, solo = 0;
+  double radius = 0.0, s = 0.0;
+  long long R = 0;                     // listed regions (0 at s = 0: the block holds one, the whole map)
+  std::vector<int64_t> index, n_points;   // 3 per region; per region
+  double *d_blk = nullptr;             // ME_CONSISTENCY_SUM_FIELDS per region, then ME_CONSISTENCY_MAX_FIELDS per region
+  long long cap_blk = 0;
+  double *d_part = nullptr;            // the fold's per-chunk values
+  long long cap_part = 0;
+  // per cloud, caller order: entropy, plane variance and flags (1 evaluated here, 2 entropy valid, 4 plane variance valid)
+  double *d_e[2] = {nullptr, nullptr}, *d_v[2] = {nullptr, nullptr};
+  uint8_t *d_flag[2] = {nullptr, nullptr};
+  long long cap_e[2] = {0, 0}, cap_v[2] = {0, 0}, cap_flag[2] = {0, 0};
+  bool pts_valid[2] = {false, false};
+  unsigned long long pts_gen[2] = {0, 0};   // cloud_gen when they were computed
+};
+
 // numpy's method="linear" position of probability p among n sorted values: h = (n - 1) p, k = floor(h), g = h - k
 inline void quantile_rank(long long n, double p, long long *k, double *g) {
   const double h = (double)(n - 1) * p;
@@ -346,6 +367,7 @@ struct me_ctx {
   me::RegionRun region;                // the per-region table (me_nn_region*), from the same records
   me::DriftRun drift;                  // the per-region drift loop (me_drift*)
   me::SurfaceRun surface;              // point-to-plane metrics (me_nn_surface*), from the NN records
+  me::ConsistencyRun consistency;      // local map consistency (me_consistency*): MPV and MME per region
   std::string err;
 };
 
@@ -476,6 +498,16 @@ int nn_surface_end(me_ctx *ctx, me_surface_result *out);
 void nn_surface_free(me_ctx *ctx);
 // the accumulators go to the cloud's MME section of d_block
 int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors);
+// dst[caller index] = src[sorted position] over the n points of a cell-sorted cloud (mme.cu)
+__global__ void unsort_f64_kernel(const P4 *__restrict__ S, long long n, const double *__restrict__ src, double *__restrict__ dst);
+// the lattice of the radius sweeps (MME and local consistency; mme.cu)
+int radius_lattice(me_ctx *ctx, int which, double radius, bool *solo);
+// local map consistency (me_consistency_*, consistency.cu; arguments checked by the caller)
+int consistency_begin(me_ctx *ctx, int which, double radius, int min_neighbors, double s, int64_t *n_regions);
+int consistency_block(me_ctx *ctx, double **device_block, int32_t *n_sum, int32_t *n_max);
+int consistency_end(me_ctx *ctx, me_consistency_row *rows, int64_t capacity, me_consistency_result *whole);
+int consistency_points(me_ctx *ctx, int which, double *entropy, double *plane_variance);
+void consistency_free(me_ctx *ctx);
 
 // layout of me_ctx::d_block (fp64): the SUM-reducible part first, then the MAX-reducible part.  Counts ride as fp64 (exact
 // below 2^53, so their sums are exact and order-independent).

@@ -24,6 +24,7 @@
 // Test hooks (environment): ME_MME_WALK forces mme_kernel, ME_MME_SHARED_LATTICE keeps the shared lattice.
 #include "common.cuh"
 #include "flat.cuh"
+#include "mme_walk.cuh"
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -49,18 +50,6 @@ __global__ void mme_init_kernel(MmeAcc *a) {
   a->n_valid = 0; a->n_query = 0; a->sum = 0.0; a->n_fp64 = 0;
   a->min_enc = enc_ordered(INFINITY); a->max_enc = enc_ordered(-INFINITY);
 }
-
-struct Moments {
-  double s1x, s1y, s1z, sxx, sxy, sxz, syy, syz, szz;
-  unsigned int cnt;
-  __device__ __forceinline__ void init() { s1x = s1y = s1z = sxx = sxy = sxz = syy = syz = szz = 0.0; cnt = 0; }
-  __device__ __forceinline__ void add(double dx, double dy, double dz) {
-    cnt++;
-    s1x += dx; s1y += dy; s1z += dz;
-    sxx += dx * dx; sxy += dx * dy; sxz += dx * dz;
-    syy += dy * dy; syz += dy * dz; szz += dz * dz;
-  }
-};
 
 struct ThreadStats {
   double sum, mn, mx;
@@ -138,45 +127,6 @@ __device__ void flush_stats(ThreadStats &t, MmeAcc *acc) {
   }
 }
 
-// the radius walk of one query over the cell-sorted cloud
-__device__ __forceinline__ void walk_global(const P4 &q, const P4 *__restrict__ S, const CellIndex &I,
-                                            const Lattice &L, double r2, float rc2, int rings, Moments &m) {
-  // the query's own cell comes with its record (high half of the tag; the x index of a sparse lattice from the coordinate)
-  int cix, ciy, ciz;
-  long long xs = I.sparse ? cell_coord(q.x, L, 0) : 0;
-  xs = xs < 0 ? 0 : (xs >= L.dims[0] ? L.dims[0] - 1 : xs);
-  cell_from_tag(I, q.idx, (int)xs, cix, ciy, ciz);
-  const long long ix = cix, iy = ciy, iz = ciz;
-  const float ux = (float)(cell_coord_cont(q.x, L, 0) - (double)ix), uy = (float)(cell_coord_cont(q.y, L, 1) - (double)iy),
-              uz = (float)(cell_coord_cont(q.z, L, 2) - (double)iz);   // position inside the own cell, [0,1)
-  for (int dz = -rings; dz <= rings; ++dz) {
-    const long long z = iz + dz;
-    if (z < 0 || z >= L.dims[2]) continue;
-    const float mz = dz == 0 ? 0.f : (dz > 0 ? (float)dz - uz : uz - (float)(dz + 1));
-    const float remz = rc2 - (mz > 0.f ? mz * mz : 0.f);
-    if (remz < 0.f) continue;
-    for (int dy = -rings; dy <= rings; ++dy) {
-      const long long y = iy + dy;
-      if (y < 0 || y >= L.dims[1]) continue;
-      const float my = dy == 0 ? 0.f : (dy > 0 ? (float)dy - uy : uy - (float)(dy + 1));
-      const float rem = remz - (my > 0.f ? my * my : 0.f);
-      if (rem < 0.f) continue;
-      const float xw = sqrtf(rem) + 1e-4f;
-      const int da = max((int)floorf(ux - xw), -rings), db = min((int)floorf(ux + xw), rings);
-      const long long xa = max(ix + da, 0ll), xb = min(ix + db, (long long)L.dims[0] - 1);
-      if (xa > xb) continue;
-      uint32_t s, e;
-      cell_range(I, (int)z, (int)y, (int)xa, (int)xb, s, e);
-      for (uint32_t j = s; j < e; ++j) {
-        const P4 p = load_p4(S + j);
-        const double dx = __dsub_rn(q.x, p.x), dy2 = __dsub_rn(q.y, p.y), dz2 = __dsub_rn(q.z, p.z);
-        const double d2 = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy2, dy2)), __dmul_rn(dz2, dz2));
-        if (d2 < r2) m.add(dx, dy2, dz2);                     // nanoflann RadiusResultSet: strict <
-      }
-    }
-  }
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // one thread per query, queries in cell-sorted order: the 32 queries of a warp are neighbours along x in one lattice
 // row, so they walk the same (2k+1)^2 rows and their candidate loads hit the same L1 lines (measured: handing the
@@ -244,12 +194,6 @@ mme_fp64_finish_kernel(const P4 *__restrict__ S, const uint32_t *__restrict__ li
 // raw records with the reference's operation order (nanoflann: d2 < r2, strict), so the neighbour COUNT — and with it
 // the k >= min_neighbors validity test — is bit-exact.  Accepted offsets are accumulated in fp64.
 // ---------------------------------------------------------------------------------------------------------------
-
-// squared gap (in cells) between a point at u in [0,1) of its cell and the cell d steps away on the same axis
-__device__ __forceinline__ float gap2(int d, float u) {
-  const float g = d == 0 ? 0.f : (d > 0 ? (float)d - u : u - (float)(d + 1));
-  return g > 0.f ? g * g : 0.f;
-}
 
 template <int R, bool E16, int U2, int SP>      // U2: 0 plain walk, 1 two candidates (two loads in flight) per iteration; SP: sparse cell table
 // 8 CTAs/SM at R <= 2 (64 registers, a few spilled words) beat the unbounded register count on C3 (chosen on B200, not
@@ -637,6 +581,24 @@ __global__ void unsort_f64_kernel(const P4 *__restrict__ S, long long n, const d
   }
 }
 
+// The lattice of a radius sweep (MME, local consistency) of cloud `which`: *solo = lay the cloud out on a lattice of its own
+// with h = r/2, else on the shared lattice.  The caller lays it out: build_grid(ctx, which, *solo ? 0.5 * radius : 0.0).
+int radius_lattice(me_ctx *ctx, int which, double radius, bool *solo) {
+  Cloud &c = ctx->cloud[which];
+  ME_TRY(wait_upload(ctx, which));
+  ME_TRY(compute_bbox(ctx, which));
+  *solo = false;
+  if (!getenv("ME_MME_SHARED_LATTICE")) {
+    const double h_now = (c.grid_valid && !c.grid_solo) ? c.lat.h : (ctx->nn_cell_size > 0 ? ctx->nn_cell_size : density_edge(c));
+    *solo = radius / h_now > 3.0 + 1e-9;
+    if (!*solo && !(c.grid_valid && !c.grid_solo)) {      // the estimate may be refined downwards by the build
+      ME_TRY(build_grid(ctx, which));
+      *solo = radius / c.lat.h > 3.0 + 1e-9;
+    }
+  }
+  return ME_OK;
+}
+
 int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors) {
   Cloud &c = ctx->cloud[which];
   if (c.n <= 0) return fail(ctx, ME_ERR_EMPTY, "cloud is empty");
@@ -645,17 +607,8 @@ int run_mme(me_ctx *ctx, int which, double radius, int min_neighbors) {
   // radius spans more than 3 of its cells (dense surfaces: 1 cm spacing, r = 0.1 m -> 7 cells; or r = 1.0 m), most of
   // the (2R+1)^2 rows of a neighbourhood are empty and enumerating them dominates.  The cloud is then laid out on a
   // lattice of its own with h = r/2 (rings = 2) for this sweep; the next NN / voxel stage lays it out again.
-  ME_TRY(wait_upload(ctx, which));
-  ME_TRY(compute_bbox(ctx, which));
   bool solo = false;
-  if (!getenv("ME_MME_SHARED_LATTICE")) {
-    const double h_now = (c.grid_valid && !c.grid_solo) ? c.lat.h : (ctx->nn_cell_size > 0 ? ctx->nn_cell_size : density_edge(c));
-    solo = radius / h_now > 3.0 + 1e-9;
-    if (!solo && !(c.grid_valid && !c.grid_solo)) {      // the estimate may be refined downwards by the build
-      ME_TRY(build_grid(ctx, which));
-      solo = radius / c.lat.h > 3.0 + 1e-9;
-    }
-  }
+  ME_TRY(radius_lattice(ctx, which, radius, &solo));
   ME_TRY(build_grid(ctx, which, solo ? 0.5 * radius : 0.0));
   if (c.grid_solo) trace_kernel(ctx, ME_KBIT_MME_SOLO);
   StageTimer timer(ctx, which == ME_CLOUD_EST ? 4 : 5);

@@ -93,6 +93,23 @@ def surface_distributed(ctx, device, knn=0, group=None):
     return ctx.surface_end()
 
 
+def consistency_distributed(ctx, device, which, radius, min_neighbors=10, region_size=0.0, group=None):
+    """Local map consistency over every rank of the job (MapEvalB200.local_consistency for world > 1): every rank sweeps its
+    query range of the replicated cloud and folds it by region, then ONE in-place SUM all-reduce of the block's sums (counts
+    ride as fp64, exact) and ONE MAX all-reduce of its maxima.  Every rank returns the same result."""
+    import torch
+    import torch.distributed as dist
+    n = ctx.consistency_begin(which, radius, min_neighbors, region_size)
+    if dist.is_initialized() and dist.get_world_size(group) > 1:
+        ptr, n_sum, n_max = ctx.consistency_block()
+        ctx.synchronize()
+        t = torch.as_tensor(_DeviceBlock(ptr, n_sum + n_max), device=device)
+        dist.all_reduce(t[:n_sum], group=group)
+        dist.all_reduce(t[n_sum:], op=dist.ReduceOp.MAX, group=group)
+        torch.cuda.current_stream(device).synchronize()
+    return ctx.consistency_end(n)
+
+
 def quantiles_distributed(ctx, device, p, population=A.ME_DIST_KEPT, group=None):
     """Exact distance quantiles of the last NN evaluation over every rank of the job (MapEvalB200.distance_quantiles for
     world > 1): the selection loop with ONE in-place SUM all-reduce of the pass's integer counts (as fp64, exact) per pass.

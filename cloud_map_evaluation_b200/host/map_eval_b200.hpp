@@ -104,6 +104,11 @@ struct Param {   // map_eval.h:60-116
   // sweep); the clouds' normals where the files carry them, else working k-NN normals with surface_normals_knn neighbours
   bool surface_metrics_ = false;
   int surface_normals_knn_ = 20;
+  // local consistency without a ground truth: MME and the mean plane variance of MME's neighbourhoods (r = nn_radius; the
+  // est cloud with min_neighbors 10, the gt cloud with 5 when evaluate_gt_mme), whole map and per region
+  // floor(x / consistency_region_size) (0 = whole map only), written to map_consistency.txt (me_consistency*)
+  bool evaluate_consistency_ = false;
+  double consistency_region_size_ = 0.0;
 };
 
 // map_eval_main.cpp:120-208
@@ -186,6 +191,13 @@ inline Param loadParametersFromYAML(const std::string &yaml_file_path) {
       if (param.surface_normals_knn_ < 1 || param.surface_normals_knn_ > 64)
         throw std::runtime_error("surface_normals_knn must be in 1..64, not " + config["surface_normals_knn"].as<std::string>());
     }
+    if (config["evaluate_consistency"]) param.evaluate_consistency_ = config["evaluate_consistency"].as<bool>();
+    if (config["consistency_region_size"]) {
+      param.consistency_region_size_ = config["consistency_region_size"].as<double>();
+      if (!(std::isfinite(param.consistency_region_size_) && param.consistency_region_size_ >= 0.0))
+        throw std::runtime_error("consistency_region_size must be finite and >= 0 (0 = the whole map only), not " +
+                                 config["consistency_region_size"].as<std::string>());
+    }
     return param;
   } catch (const std::exception &e) {
     std::cerr << "Error loading parameters: " << e.what() << std::endl;
@@ -217,7 +229,8 @@ inline void dumpParam(const Param &p, std::ostream &os) {
      << "\ndistance_quantiles=";
   for (size_t i = 0; i < p.distance_quantiles_.size(); ++i) os << (i ? "," : "") << p.distance_quantiles_[i];
   os << "\nregion_size=" << p.region_size_ << "\ndrift_region_size=" << p.drift_region_size_ << "\nsurface_metrics=" << p.surface_metrics_
-     << "\nsurface_normals_knn=" << p.surface_normals_knn_ << "\n";
+     << "\nsurface_normals_knn=" << p.surface_normals_knn_ << "\nevaluate_consistency=" << p.evaluate_consistency_
+     << "\nconsistency_region_size=" << p.consistency_region_size_ << "\n";
 }
 
 // Eigen's default IOFormat for `vec.transpose()`: coefficients right-aligned to a common width, one space apart
@@ -361,6 +374,7 @@ class MapEvalB200 {
   int distanceQuantiles();
   int regionErrors();
   int surfaceMetrics();
+  int localConsistency();
   int regionDrift();
   GpuGroup gpus_;            // one context per GPU; rank r evaluates the r-th shard of every sweep's query range
   me_ctx *ctx_ = nullptr;    // = gpus_.ctx(0): the voxel stage and the single-GPU calls
@@ -468,6 +482,8 @@ inline int MapEvalB200::process() {
   }
   if (calculateVMD() != 0) return -1;
   if (param_.enable_debug) std::cout << "INFO: VMD calculation completed." << std::endl;
+  // after every consumer of the pass's NN records (the sweep may lay a cloud out again), with the estimate in its final frame
+  if (param_.evaluate_consistency_ && localConsistency() != 0) return -1;
   if (param_.save_immediate_result_) {
     if (param_.enable_debug) std::cout << "INFO: Saving registration results..." << std::endl;
     saveRegistrationResults();
@@ -800,6 +816,71 @@ inline int MapEvalB200::regionErrors() {
     f << "\n";
   }
   std::cout << "INFO: errors of " << n[0] << " regions of edge " << s << " saved to " << path << std::endl;
+  return 0;
+}
+
+// local consistency without a ground truth: the me_consistency_* loop on every GPU for the est cloud (and the gt cloud with
+// evaluate_gt_mme), one grouped NCCL SUM all-reduce of the block's sums and one MAX all-reduce of its maxima per cloud ->
+// map_consistency.txt next to map_results.txt
+inline int MapEvalB200::localConsistency() {
+  const double s = param_.consistency_region_size_, r = param_.nn_radius_;
+  struct Run {
+    int which, m;
+    const char *name;
+    me_consistency_result whole;
+    std::vector<me_consistency_row> rows;
+  };
+  std::vector<Run> runs;
+  runs.push_back(Run{ME_CLOUD_EST, 10, "est", me_consistency_result{}, {}});
+  if (param_.evaluate_gt_mme_) runs.push_back(Run{ME_CLOUD_GT, 5, "gt", me_consistency_result{}, {}});
+  for (Run &run : runs) {
+    std::vector<int64_t> n(gpus_.size(), 0);
+    std::vector<double *> ptr(gpus_.size(), nullptr), ptr_max(gpus_.size(), nullptr);
+    std::vector<int32_t> n_sum(gpus_.size(), 0), n_max(gpus_.size(), 0);
+    if (gpus_.for_each([&](int g, me_ctx *c) {
+          int rc = me_consistency_begin(c, run.which, r, run.m, s, &n[g]);
+          if (rc == ME_OK) rc = me_consistency_block(c, &ptr[g], &n_sum[g], &n_max[g]);
+          ptr_max[g] = ptr[g] + n_sum[g];
+          return rc != ME_OK ? rc : me_synchronize(c);
+        }) != ME_OK)
+      return fail("me_consistency_begin");
+    if (!gpus_.allreduce_device(ptr, (size_t)n_sum[0], ncclSum) || !gpus_.allreduce_device(ptr_max, (size_t)n_max[0], ncclMax))
+      return fail("all-reduce of the consistency block");
+    run.rows.resize((size_t)n[0]);
+    if (me_consistency_end(ctx_, run.rows.data(), n[0], &run.whole) != ME_OK) return fail("me_consistency_end");
+  }
+  const std::string path = results_subfolder + "map_consistency.txt";
+  std::ofstream f(path);
+  if (!f.is_open()) {
+    std::cerr << "ERROR: cannot write " << path << std::endl;
+    return -1;
+  }
+  f << std::setprecision(17) << "# local consistency without a ground truth: per point MME's neighbourhood (d2 < r^2), its entropy "
+       "and its plane variance (smallest eigenvalue of the covariance, m^2); r = " << r << ", min_neighbors est 10";
+  if (runs.size() > 1) f << ", gt 5";
+  f << ", region_size " << s << (s > 0.0 ? "" : " (whole map only)") << "; est in the ground truth's frame\n";
+  const char *stats = "n_query n_valid n_pv mme mpv mean_plane_std max_pv";
+  f << "cloud n_points " << stats << "\n" << std::fixed << std::setprecision(15);
+  auto put = [&](int64_t n_points, int64_t nq, int64_t nv, int64_t np, double mme, double mpv, double sd, double mx) {
+    f << " " << n_points << " " << nq << " " << nv << " " << np << " " << mme << " " << mpv << " " << sd << " " << mx << "\n";
+  };
+  for (const Run &run : runs) {
+    const me_consistency_result &w = run.whole;
+    f << run.name;
+    put(w.n_points, w.n_query, w.n_valid, w.n_pv, w.mme, w.mpv, w.mean_plane_std, w.max_pv);
+  }
+  if (s > 0.0) {
+    f << "cloud min_x min_y min_z max_x max_y max_z n_points " << stats << "\n";
+    for (const Run &run : runs)
+      for (const me_consistency_row &x : run.rows) {
+        f << run.name << " " << x.min[0] << " " << x.min[1] << " " << x.min[2] << " " << x.max[0] << " " << x.max[1] << " " << x.max[2];
+        put(x.n_points, x.n_query, x.n_valid, x.n_pv, x.mme, x.mpv, x.mean_plane_std, x.max_pv);
+      }
+  }
+  std::cout << "INFO: local consistency:";
+  for (size_t i = 0; i < runs.size(); ++i)
+    std::cout << (i ? "," : "") << " " << runs[i].name << " MPV " << runs[i].whole.mpv << " m^2, MME " << runs[i].whole.mme;
+  std::cout << "; saved to " << path << std::endl;
   return 0;
 }
 

@@ -609,6 +609,71 @@ ME_API int  me_drift_end(me_ctx *ctx, me_drift_row *rows, int64_t capacity);
 ME_API int  me_drift(me_ctx *ctx, double region_size, double max_correspondence_distance, int32_t max_iteration,
                      double relative_fitness, double relative_rmse, me_drift_row **rows, int64_t *n_regions);
 
+/* ---- local map consistency without a ground truth: mean plane variance beside MME ----------------------------------------
+ * For cloud `which` as it is now, radius r (finite, > 0) and min_neighbors m (>= 3), per point q: MME's neighbourhood (the
+ * points p of the same cloud with d2 < r^2, nanoflann's d2 and strict test, q included; k = accepted - 1) and MME's moments,
+ * taken about q from the fp64 offsets q - p of the raw coordinates in the order of MME's fp64 walk (rows by dz, then dy,
+ * ascending; x-runs ascending in the cell-sorted order).  C = (S2 - S1 S1^T / k) / (k - 1) as MME forms it.
+ *   entropy e = 0.5 ln(2 pi e det C) as MME: valid when k >= m and e is finite (n_valid, sum_entropy); invalid points store 0.
+ *   plane variance v = max(0, smallest eigenvalue of C) (cyclic Jacobi, fp64): valid when k >= m and v is finite (n_pv,
+ *   sum_pv, sum_sqrt_pv, max_pv); a point with k < m stores NaN.  A perfect plane has v = 0 (valid) and no entropy.
+ * Whole map: mme = sum_entropy / n_valid (0 when n_valid = 0, as me_mme_finalize), mpv = sum_pv / n_pv and mean_plane_std =
+ * sum_sqrt_pv / n_pv (NaN when n_pv = 0), max_pv (NaN when n_pv = 0).
+ * Regions, for region_size s > 0: a point's region is floor(x / s) per axis, the occupied list of me_nn_region_begin over est ++
+ * gt (est alone while the gt cloud is empty), with its limits and messages; one row per listed region, n_points = the region's
+ * points of this cloud.  s = 0: no rows.  The whole-map result is the rows' sums added in list order (s > 0).
+ * Device block: ME_CONSISTENCY_SUM_FIELDS SUM-reducible values per region [n_query n_valid n_pv sum_entropy sum_pv sum_sqrt_pv]
+ * (counts as fp64), then ME_CONSISTENCY_MAX_FIELDS MAX-reducible values per region [max_pv] (0 for an empty set); at s = 0 the
+ * block holds one region, the whole map.  The same length on every rank.  Folded in caller order per region (chunks of 1024
+ * points, a fixed shuffle tree, chunks added in order); no floating-point atomics, so two calls on one device, world and
+ * lattice give the same bits while the cloud is not laid out again in between (a new layout may order the points of a cell
+ * differently), and counts are the same for any world.
+ * The sweep lays the cloud out as me_eval_mme does (the shared lattice, or a lattice of its own with h = r / 2 when r spans
+ * more than 3 shared cells), which can make that cloud's NN records stale; it leaves MME's results (me_get_entropies) and
+ * the kernel trace alone.  *kernel / rings / solo of the result say which sweep ran (me_consistency_kernel).
+ * The loop (every rank the same calls): me_consistency_begin checks, sweeps this rank's query range and folds it; *n_regions =
+ * the rows me_consistency_end will fill (0 at s = 0).  me_consistency_block hands out the block (SUM-reduce the first n_sum
+ * values and MAX-reduce the next n_max in place, after me_synchronize); me_consistency_end reads the reduced block and fills
+ * rows[0 .. n_regions - 1] (capacity >= n_regions; rows may be NULL when n_regions = 0) and *whole.  Refused: r not finite
+ * and > 0, m < 3, s negative or not finite, an empty cloud, an open registration or drift loop, world > 1 with ME_LAYOUT_SLAB
+ * requested, the region list's limits, calls out of order, and a cloud changed between begin and end.
+ * me_consistency: the whole loop at world 1, rows allocated by the library (me_free; NULL at s = 0).
+ * me_consistency_finalize (host only): rows and the whole-map result from a reduced host block, the region indices (3 per
+ * region), the per-region point counts and the cloud size (radius, min_neighbors, kernel, rings and solo are left 0).
+ * me_get_consistency_points: the last call's e and v of cloud `which`, caller order (either pointer may be NULL); points
+ * another rank evaluated hold 0 and NaN.  Valid until the cloud changes. */
+#define ME_CONSISTENCY_SUM_FIELDS 6
+#define ME_CONSISTENCY_MAX_FIELDS 1
+enum me_consistency_kernel {
+  ME_CONSISTENCY_WALK = 0           /* consistency_walk_kernel: MME's fp64 generic walk (mme_kernel's order)   */
+};
+typedef struct {
+  int64_t index[3];                             /* (ix, iy, iz) */
+  double  min[3], max[3];                       /* index * s, (index + 1) * s */
+  int64_t n_points;                             /* points of the cloud in the region */
+  int64_t n_query, n_valid, n_pv;               /* evaluated points; valid entropies; valid plane variances */
+  double  sum_entropy, sum_pv, sum_sqrt_pv;
+  double  mme, mpv, mean_plane_std, max_pv;
+} me_consistency_row;
+typedef struct {
+  double  radius, region_size;
+  int32_t min_neighbors, kernel, rings, solo;   /* kernel: me_consistency_kernel; solo: the cloud's own lattice (h = r / 2) */
+  int64_t n_regions;
+  int64_t n_points, n_query, n_valid, n_pv;
+  double  sum_entropy, sum_pv, sum_sqrt_pv;
+  double  mme, mpv, mean_plane_std, max_pv;
+} me_consistency_result;
+ME_API int  me_consistency_begin(me_ctx *ctx, int which, double radius, int32_t min_neighbors, double region_size,
+                                 int64_t *n_regions);
+ME_API int  me_consistency_block(me_ctx *ctx, double **device_block, int32_t *n_sum, int32_t *n_max);
+ME_API int  me_consistency_end(me_ctx *ctx, me_consistency_row *rows, int64_t capacity, me_consistency_result *whole);
+ME_API int  me_consistency(me_ctx *ctx, int which, double radius, int32_t min_neighbors, double region_size,
+                           me_consistency_row **rows, int64_t *n_regions, me_consistency_result *whole);
+ME_API int  me_consistency_finalize(int64_t n_regions, double region_size, const int64_t *index, const int64_t *n_points,
+                                    int64_t n_total, const double *host_block, me_consistency_row *rows,
+                                    me_consistency_result *whole);   /* host only */
+ME_API int  me_get_consistency_points(me_ctx *ctx, int which, double *entropy, double *plane_variance);
+
 /* replaces: ComputeMeanMapEntropyUsingNormalTBB / ...UsingNormal (min_neighbors 10, map_eval.cpp:1608-1737, 1538-1606),
  * ComputeMeanMapEntropy (min_neighbors 5, :1438-1535), ComputeEntropy (:1433-1436) and the min/max side effect of
  * ColorPointCloudByMME (:697-701).  entropies_host (nullable) receives N fp64, zeros where invalid.
