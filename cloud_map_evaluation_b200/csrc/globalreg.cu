@@ -116,12 +116,13 @@ struct FeatGeom {
   const P4 *S; CellIndex I; Lattice L; CoarseGrid CG;
   const double *nrm;      // caller order
   int k; double slack, r2;
+  unsigned int *trace;    // me_kernel_trace's device word (ME_TEV_KNN_COARSE)
 };
 
 // the neighbourhood of sorted point s into this thread's slots; returns its size
 __device__ __forceinline__ int feature_neighbours(const FeatGeom &G, long long s, P4 &q, double *dk, uint32_t *ik) {
   q = load_p4(G.S + s);
-  return knn_walk<kFpfhThreads>(G.S, G.I, G.L, G.CG, q, G.k, G.slack, G.r2, true, dk, ik);
+  return knn_walk<kFpfhThreads>(G.S, G.I, G.L, G.CG, q, G.k, G.slack, G.r2, true, dk, ik, G.trace);
 }
 
 __global__ void __launch_bounds__(kFpfhThreads) fpfh_spfh_kernel(FeatGeom G, long long n, double *__restrict__ spfh) {
@@ -416,6 +417,7 @@ static int features_of(me_ctx *ctx, int which, const me_global_reg_params *p, Re
   FeatGeom G;
   G.S = c.d_sorted; G.I = index_of(c); G.L = c.lat; G.CG = coarse_of(c); G.nrm = c.d_normal;
   G.k = p->feature_max_nn; G.slack = slack_of(c); G.r2 = p->feature_radius * p->feature_radius;
+  G.trace = ctx->d_trace;
   ME_TRY(ensure_work(ctx, (size_t)c.n * kFeat * sizeof(double)));
   double *spfh = (double *)ctx->d_work;
   ME_TRY(ensure(ctx, (void **)&ctx->d_fpfh[which], &ctx->cap_fpfh[which], c.n * kFeat, sizeof(float)));

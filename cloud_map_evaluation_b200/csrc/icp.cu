@@ -208,13 +208,13 @@ static constexpr int kKnnThreads = 128;
 
 __global__ void __launch_bounds__(kKnnThreads)
 knn_normals_kernel(const P4 *__restrict__ S, long long n, const uint32_t *__restrict__ list, CellIndex I, Lattice L,
-                   CoarseGrid CG, int k, double slack, double *__restrict__ normals) {
+                   CoarseGrid CG, int k, double slack, double *__restrict__ normals, unsigned int *trace) {
   extern __shared__ __align__(16) unsigned char knn_smem[];
   double *dk = reinterpret_cast<double *>(knn_smem) + threadIdx.x;                                     // dk[t * kKnnThreads]
   uint32_t *ik = reinterpret_cast<uint32_t *>(knn_smem + (size_t)k * kKnnThreads * sizeof(double)) + threadIdx.x;
   for (long long i = blockIdx.x * (long long)kKnnThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kKnnThreads) {
     const P4 q = load_p4(S + (list ? (long long)__ldg(list + i) : i));
-    const int cnt = knn_walk<kKnnThreads>(S, I, L, CG, q, k, slack, INFINITY, false, dk, ik);
+    const int cnt = knn_walk<kKnnThreads>(S, I, L, CG, q, k, slack, INFINITY, false, dk, ik, trace);
     // utility::ComputeCovariance over the neighbours (cumulants about the query point instead of the origin: same
     // covariance, without the cancellation of raw coordinates); fewer than 3 neighbours -> identity
     double cov[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
@@ -298,7 +298,7 @@ int estimate_normals(me_ctx *ctx, int which, int knn, long long lo, long long hi
     const double slack = 1e-9 * c.lat.h + 4e-14 * maxabs;
     const int blocks = (int)std::min<long long>((nq + kKnnThreads - 1) / kKnnThreads, (long long)ctx->sm_count * 32);
     knn_normals_kernel<<<blocks, kKnnThreads, smem, ctx->stream>>>(c.d_sorted, nq, list, index_of(c), c.lat, coarse_of(c), k,
-                                                                   slack, c.d_normal);
+                                                                   slack, c.d_normal, ctx->d_trace);
     ME_LAUNCH_CHECK(ctx);
   }
   c.normal_valid = true;

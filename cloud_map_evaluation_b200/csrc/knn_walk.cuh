@@ -10,10 +10,14 @@ namespace me {
 // with d2 < r2 are candidates (r2 = INFINITY: none is excluded), and with skip_self the point with q's caller index is not
 // one.  The lattice is searched shell by shell (Chebyshev rings) until the k-th distance beats the distance to the border
 // of the searched block, or that border lies beyond the radius; points far from everything go on to blocks of f^3 cells
-// of the coarse occupancy grid, where empty blocks cost one load.
+// of the coarse occupancy grid, where empty blocks cost one load.  A query that goes on to those blocks sets
+// ME_TEV_KNN_COARSE in me_kernel_trace's device word *trace (nullable): one lane per warp of the queries that enter the phase
+// together, and none once the word carries the bit.  (A flag carried to the end of the kernel and voted there costs the
+// FPFH kernels registers: fpfh_kernel's spills grew from 280 to 516 bytes.)
 template <int STRIDE>
 __device__ __forceinline__ int knn_walk(const P4 *__restrict__ S, const CellIndex &I, const Lattice &L, const CoarseGrid &CG,
-                                        const P4 &q, int k, double slack, double r2, bool skip_self, double *dk, uint32_t *ik) {
+                                        const P4 &q, int k, double slack, double r2, bool skip_self, double *dk, uint32_t *ik,
+                                        unsigned int *trace) {
   int cix, ciy, ciz;
   long long xs = I.sparse ? cell_coord(q.x, L, 0) : 0;
   xs = xs < 0 ? 0 : (xs >= L.dims[0] ? L.dims[0] - 1 : xs);
@@ -72,6 +76,11 @@ __device__ __forceinline__ int knn_walk(const P4 *__restrict__ S, const CellInde
     if (ix - r <= 0 && ix + r >= L.dims[0] - 1 && iy - r <= 0 && iy + r >= L.dims[1] - 1 && iz - r <= 0 && iz + r >= L.dims[2] - 1) { resolved = true; break; }
   }
   if (!resolved) {
+    if (trace) {
+      const unsigned int m = __activemask();
+      if ((threadIdx.x & 31) == __ffs(m) - 1 && !((*(volatile unsigned int *)trace >> ME_TEV_KNN_COARSE) & 1u))
+        atomicOr(trace, 1u << ME_TEV_KNN_COARSE);
+    }
     // coarse phase, from scratch (the blocks cover the cells of the fine phase again): Chebyshev rings of blocks, empty
     // blocks cost one count load, blocks that cannot hold a candidate closer than the k-th best (or the radius) are skipped
     const int f = CG.f;
@@ -115,5 +124,7 @@ __device__ __forceinline__ int knn_walk(const P4 *__restrict__ S, const CellInde
   }
   return cnt;
 }
+
+static_assert((int)ME_KBIT_COUNT <= (int)ME_TEV_KNN_COARSE && (int)ME_TEV_KNN_COARSE < 32, "trace event bit");
 
 }  // namespace me

@@ -766,6 +766,7 @@ enum me_kernel_bit {
 /* Data events of the same mask, above the sweep bits.  They record what the data made a sweep do rather than which sweep
  * ran, so they are not part of enum me_kernel_bit; they are set on the device only when a query reaches the path. */
 enum me_trace_event {
+  ME_TEV_KNN_COARSE = 30,          /* a k-NN walk query left the fine rings for the coarse blocks (normals, FPFH)      */
   ME_TEV_MME_FP64_FINISH = 31      /* an fp32-offset MME sweep left queries to mme_fp64_finish_kernel (thin surfaces)  */
 };
 /* *mask (nullable) = the trace since creation or the last reset; *mme_rows_cfg (nullable) = (CAP << 8) | U of the last

@@ -17,6 +17,9 @@ the cross products of the rows of C - (lambda_0 + eps_s) I leave a component eps
   n^T C n - lambda_0 <= 2 E_F + C_EIG u lambda_2 + min(g, eps_s^2 / g) (E_F the Frobenius norm of E): no spectral gap is
   needed, so lines and isotropic blobs are covered;
   sin(n, v_0) <= (E_F + eps_s) / g (Davis-Kahan) where that is below SIN_DETERMINED.
+An exactly diagonal covariance takes FastEigen3x3's axis branch, which returns the axis of the strictly smallest diagonal
+entry and (0, 0, 1) otherwise, an eigenvector of the largest eigenvalue when a neighbourhood is collinear along z (k = 3
+on a lattice): that axis is accepted as well as any normal within the bounds below.
 The sign is FastEigen3x3's, a result rather than a convention (generalized ICP's Rx = I when n.x < -0.99): it must equal
 that of fast_eigen3x3 below applied to the exactly rounded covariance, except where a branch decision of that statement
 lies within TIE_REL of a tie.
@@ -239,7 +242,7 @@ def normals_exact(pts, queries=None, k=20, nbs=None):
     nbs = knn_exact(pts, queries, k) if nbs is None else nbs
     out = []
     for qi, nb in zip(queries, nbs):
-        row = dict(q=int(qi), nb=nb, cov=None)
+        row = dict(q=int(qi), nb=nb, cov=None, diagonal=False)       # diagonal: with a repeated smallest eigenvalue
         if len(nb) >= 3:
             cov = covariance_exact(pts, nb)
             lam, v0 = eig_exact(cov)
@@ -248,6 +251,8 @@ def normals_exact(pts, queries=None, k=20, nbs=None):
             if math.sqrt(_dot(stmt, stmt)) == 0.0:
                 stmt = [0.0, 0.0, 1.0]
             row.update(cov=cov, lam=lam, v0=v0, E=covariance_bound(pts, pts[qi], nb),
+                       diagonal=cov[0][1] == 0 and cov[0][2] == 0 and cov[1][2] == 0
+                       and sorted(cov[a][a] for a in range(3))[0] == sorted(cov[a][a] for a in range(3))[1],
                        E_raw=covariance_bound(pts, np.zeros(3), nb), stmt=np.array(stmt), tie=t.min_rel)
         out.append(row)
     return out
@@ -261,6 +266,9 @@ def check_normal(row, n, raw=False):
     if row["cov"] is None:
         ok = n.tolist() == [0.0, 0.0, 1.0]
         return dict(ok=ok, why="" if ok else "fewer than 3 neighbours: not (0, 0, 1)", sin_bound=0.0, sign_checked=ok)
+    if row["diagonal"] and n.tolist() == row["stmt"].tolist():
+        # FastEigen3x3's axis branch on an exactly diagonal covariance with a repeated smallest eigenvalue
+        return dict(ok=True, why="", sin_bound=0.0, sign_checked=False)
     lam, E = row["lam"], row["E_raw" if raw else "E"]
     l2 = max(abs(lam[2]), 0.0)
     EF = float(np.sqrt((E * E).sum()))

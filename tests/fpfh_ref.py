@@ -47,20 +47,24 @@ def d2_kd(a, b):
     return (d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1]) + d[..., 2] * d[..., 2]
 
 
-def hybrid_neighbours(xyz, radius, max_nn):
-    """per point (indices, d2): the <= max_nn nearest other points with d2 < radius^2, sorted by (d2, index)"""
+def hybrid_neighbours(xyz, radius, max_nn, queries=None, larger_index_on_tie=False, closed=False, skip_self=True):
+    """per point (or per index of queries) (indices, d2): the <= max_nn nearest other points with d2 < radius^2, sorted by
+    (d2, index).  larger_index_on_tie (ties to the larger index), closed (d2 <= radius^2) and skip_self=False (the point is
+    its own neighbour) are deliberately wrong variants for the tests' teeth."""
     xyz = np.asarray(xyz, np.float64)
     tree = cKDTree(xyz)
     r2 = radius * radius
-    cand = tree.query_ball_point(xyz, radius * (1 + 1e-9) + 1e-12, workers=-1)
+    queries = np.arange(len(xyz)) if queries is None else np.asarray(queries, np.int64)
+    cand = tree.query_ball_point(xyz[queries], radius * (1 + 1e-9) + 1e-12, workers=-1)
     out = []
-    for i, c in enumerate(cand):
+    for i, c in zip(queries, cand):
         c = np.asarray(c, np.int64)
-        c = c[c != i]
+        if skip_self:
+            c = c[c != i]
         d2 = d2_kd(xyz[i], xyz[c])
-        keep = d2 < r2
+        keep = d2 <= r2 if closed else d2 < r2
         c, d2 = c[keep], d2[keep]
-        o = np.lexsort((c, d2))[:max_nn]
+        o = np.lexsort((-c if larger_index_on_tie else c, d2))[:max(max_nn, 0)]
         out.append((c[o], d2[o]))
     return out
 
@@ -161,6 +165,29 @@ def fpfh(sp, nbrs, sp_flagged=None):
             if len(nbrs[i][0]) and sp_flagged[nbrs[i][0]].any():
                 flagged[i] = True
     return f64.astype(np.float32), f64, flagged
+
+
+def fpfh_sample(xyz, nrm, radius, max_nn, sample):
+    """(FPFH fp32, FPFH fp64, flagged) of the points `sample` alone, from the neighbourhoods of the sample and of its
+    neighbours: what features() gives at those rows, at a cost that does not grow with the cloud"""
+    xyz = np.asarray(xyz, np.float64)
+    sample = np.asarray(sample, np.int64)
+    n = len(xyz)
+    empty = (np.zeros(0, np.int64), np.zeros(0))
+    nb_s = hybrid_neighbours(xyz, radius, max_nn, sample)
+    ring = np.setdiff1d(np.unique(np.concatenate([ix for ix, _ in nb_s] + [np.zeros(0, np.int64)])), sample)
+    nb_r = hybrid_neighbours(xyz, radius, max_nn, ring)
+    nbrs = [empty] * n
+    for i, v in zip(sample, nb_s):
+        nbrs[i] = v
+    for i, v in zip(ring, nb_r):
+        nbrs[i] = v
+    sp, fl = spfh(xyz, nrm, nbrs)
+    only = [empty] * n
+    for i, v in zip(sample, nb_s):
+        only[i] = v
+    f32, f64, ffl = fpfh(sp, only, fl)
+    return f32[sample], f64[sample], ffl[sample]
 
 
 def features(xyz, nrm, radius, max_nn):
