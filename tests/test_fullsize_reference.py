@@ -4,6 +4,7 @@ planted fault in otherwise exact records."""
 import math
 import os
 import sys
+from fractions import Fraction
 
 import mpmath as mp
 import numpy as np
@@ -312,3 +313,206 @@ def test_scs_grid_equals_scs_exact():
     for t in range(0, len(keys) - 1, 37):
         assert abs(term[t] - float(F.scs_key_exact(table, tuple(keys[t]), 5))) <= 1e-13 * term[t]
     assert F.scs_key_exact(table, (40, 40, 40), 5) is None and math.isnan(term[-1])
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# segmented sums, the region table, point-to-plane pairs and local consistency
+# ---------------------------------------------------------------------------------------------------------------
+def test_segmented_sums_equal_exact_ref_per_segment():
+    rs = np.random.RandomState(21)
+    x = np.concatenate([rs.uniform(-1, 1, 6000) * 10.0 ** rs.randint(-20, 20, 6000), [0.0, 5e-200, -1e200, 1e200]])
+    seg = rs.randint(0, 37, len(x))
+    seg[-4:] = 36                                              # one segment whose sum cancels to 5e-200
+    hi, lo, ab, L, e0 = F.seg_sums(_t(x), _t(seg), 37)
+    for r in range(37):
+        ex = X.exact_sum(x[seg == r])
+        assert F.seg_fraction(L, e0, r) == ex
+        assert hi[r].item() == float(ex) or abs(Fraction(hi[r].item()) + Fraction(lo[r].item()) - ex) <= \
+            2.0 ** -100 * float(X.exact_sum(np.abs(x[seg == r])))
+    got = torch.tensor([float(X.exact_sum(x[seg == r])) for r in range(37)], dtype=torch.float64)
+    cnt = torch.bincount(_t(seg), minlength=37)
+    assert F.check_seg_sum("exact", got, (hi, lo, ab), cnt) <= 1.0
+    # a naive sum of each segment is within the order bound; one ulp beyond the bound is not
+    naive = torch.tensor([float(np.sum(x[seg == r])) for r in range(37)], dtype=torch.float64)
+    F.check_seg_sum("naive", naive, (hi, lo, ab), cnt)
+    bad = got.clone()
+    b = (cnt[5] - 1).item() * X.U * ab[5].item()
+    bad[5] = float(X.exact_sum(x[seg == 5])) + 2 * b + 1e-300
+    with pytest.raises(AssertionError):
+        F.check_seg_sum("planted", bad, (hi, lo, ab), cnt)
+
+
+def _region_scene(seed=22):
+    """two clouds with coordinates on the region faces of s = 0.1: fl(k s), where x (1 / s) and x / s can floor apart"""
+    rs = np.random.RandomState(seed)
+    est = rs.uniform(-1.0, 2.0, (3000, 3))
+    gt = rs.uniform(-1.0, 2.0, (2500, 3))
+    face = np.arange(-10, 20) * 0.1
+    est[:300, 0] = rs.choice(face, 300)
+    gt[:300, 1] = rs.choice(face, 300)
+    return est, gt, 0.1
+
+
+def test_region_table_restatement_equals_a_loop_over_regions():
+    """region_list_t and region_direction_t against per-region exact_ref.dir_stats, and check_region_row accepts rows built
+    from those exact values; the reciprocal key moves points on the face scene, and a pair filed under its reference
+    point's region changes n_corr"""
+    est, gt, s = _region_scene()
+    ie, de = brute(est, gt)
+    tau = [0.3, 0.2, 0.1, 0.05, 0.02]
+    Rc = 0.04
+    L = F.region_list_t(_t(est), _t(gt), s)
+    keys_e = X.voxel_keys(est, s)
+    keys_g = X.voxel_keys(gt, s)
+    occ = sorted(set(map(tuple, keys_e)) | set(map(tuple, keys_g)))
+    np.testing.assert_array_equal(L["index"].numpy(), np.array(occ))
+    n = len(occ)
+    qi, sq, d = F.region_pairs_t(_t(est), _t(gt), _t(ie), _t(de), Rc)
+    T = F.region_direction_t(L["seg_est"], n, _t(ie), _t(de), qi, sq, d, tau)
+    sq_x, d_x, _ = X.kept_pairs(est, gt, ie, de, Rc, 0)
+    kept = np.nonzero(de <= Rc)[0]
+    pos = {k: i for i, k in enumerate(occ)}
+    for r, key in enumerate(occ):
+        mine = np.array([pos[tuple(keys_e[q])] == r for q in kept], bool)
+        n_src = int((np.array([pos[tuple(k)] for k in keys_e]) == r).sum())
+        ex = X.dir_stats(sq_x[mine], d_x[mine], max(n_src, 1), tau)
+        assert int(T["n_corr"][r]) == ex["n_corr"]
+        assert [int(T["n_inlier"][k][r]) for k in range(5)] == ex["n_inlier"]
+        if n_src:
+            got = F._ex_dir(T, r, r, n_src, tau)
+            for f in ("mean", "rmse", "fitness"):
+                np.testing.assert_array_equal(got[f], ex[f])
+        for k in range(5):
+            assert F.seg_fraction(*T["sum_d"][k], r) == X.exact_sum(d_x[mine][d_x[mine] <= tau[k]])
+    W = F.region_list_t(_t(est), _t(gt), s, recip=True)
+    assert int((W["keys"][W["seg_est"]] != L["keys"][L["seg_est"]]).sum()) > 0
+    wrong = torch.bincount(L["seg_gt"][_t(ie)[qi]], minlength=n)
+    assert not torch.equal(wrong, T["n_corr"])
+
+
+def test_division_check_accepts_ieee_division():
+    est, _, s = _region_scene()
+    assert F.division_is_rounded(_t(est), s, 2000, 1) == 2002
+
+
+def test_surface_pairs_equal_surface_ref():
+    """e, c and the counts of surface_pairs_t equal surface_ref.fold bit for bit, with scaled, zero and NaN normals; e
+    divided by ||n||^2 differs on non-unit normals"""
+    import surface_ref as S
+    rs = np.random.RandomState(23)
+    est, gt = rs.uniform(0, 1, (2000, 3)), rs.uniform(0, 1, (1800, 3))
+    ne, ng = rs.normal(size=(2000, 3)) * rs.uniform(0.5, 3, (2000, 1)), rs.normal(size=(1800, 3))
+    ng[:20] = 0.0
+    ng[20:25] = np.nan
+    ne[:30] = 0.0
+    ie, de = brute(est, gt)
+    tau = [0.1, 0.05, 0.03, 0.02, 0.01]
+    Rc = 0.003
+    P = F.surface_pairs_t(_t(est), _t(gt), _t(ne), _t(ng), _t(ie), _t(de), Rc)
+    ref = S.fold(est, gt, ne, ng, ie, de, tau, Rc, 0, 1)          # cut-off mode 0: d2 <= R
+    ex = F.surface_direction_t(P, len(est), tau)
+    assert (ex["n_corr"], ex["n_no_normal"], ex["n_no_normal_nn"], ex["n_nc"]) == \
+        (ref["n_corr"], ref["n_no_normal"], ref["n_no_normal_nn"], ref["n_nc"])
+    assert list(ex["n_inlier"]) == list(ref["n_inlier"])
+    ek = P["e"][P["kept"] & P["ok_n"]].numpy()
+    np.testing.assert_array_equal(ek, ref["e_kept"])
+    assert ex["max_e"] == ref["max_e"] and ex["max_e_nn"] == ref["max_e_nn"]
+    assert X.exact_sum(P["c"][P["kept"] & P["ok_n"] & P["ok_m"]].numpy()) == ex["sum_c"]
+    Pw = F.surface_pairs_t(_t(est), _t(gt), _t(ne), _t(ng), _t(ie), _t(de), Rc, wrong_norm=True)
+    assert not torch.equal(Pw["e"][Pw["kept"] & Pw["ok_n"]], P["e"][P["kept"] & P["ok_n"]])
+    # against the definition: e within beta of mpmath
+    sel = np.nonzero((P["have"] & P["ok_n"]).numpy())[0][:200]
+    dd = est[sel] - gt[ie[sel]]
+    beta = F.plane_beta(dd, ng[ie[sel]])
+    for t, q in enumerate(sel):
+        e_ex, c_ex = F.exact_plane(est[q], gt[ie[q]], ng[ie[q]], ne[q] if bool(P["ok_m"][q]) else None)
+        assert abs(float(P["e"][q]) - e_ex) <= beta[t]
+        assert F.exact_inlier(est[q], gt[ie[q]], ng[ie[q]], e_ex * (1 + 1e-9))
+        assert not F.exact_inlier(est[q], gt[ie[q]], ng[ie[q]], e_ex * (1 - 1e-9))
+
+
+
+def test_consistency_sample_equals_consistency_ref():
+    """consistency_sample_exact's lambda3 and bound equal consistency_ref's on a sample of a tilted plane, and the
+    covariance divided by k and the largest eigenvalue lie beyond the bound of the exact lambda3"""
+    import consistency_ref as CR
+    pts = tilted_plane(1e-3, np.zeros(3), 3000, 5)
+    r = 0.12
+    qi = np.arange(0, 3000, 97)
+    qh, nbs = F.ball_neighbours(_t(pts), qi, r)
+    exs = F.mme_sample_exact(qh, nbs, 10)
+    got = F.consistency_sample_exact(qh, nbs, exs, 10)
+    ref = CR.exact_points(pts, r, 10, qi)
+    wk = F.consistency_sample_exact(qh, nbs, exs, 10, divisor_k=True)
+    wm = F.consistency_sample_exact(qh, nbs, exs, 10, largest=True)
+    bites = 0
+    for t in range(len(qi)):
+        if math.isnan(ref["lam"][t]):
+            assert math.isnan(got[t][0])
+            continue
+        assert got[t][0] == ref["lam"][t] and got[t][1] == ref["bound"][t]
+        bites += abs(wk[t][0] - got[t][0]) > got[t][1] and abs(wm[t][0] - got[t][0]) > got[t][1]
+    assert bites > 0.9 * len(qi)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# the exact k nearest neighbours and the normal check
+# ---------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("m0", [1 / 64, 1 / 4])
+def test_knn_windows_equal_brute_force(m0):
+    """exact_knn_sample against exact_reg.knn_exact (k = 20, query included) on a box and on a shuffled lattice whose
+    20th neighbour falls inside a tie group; a too small first window doubles, and a too small largest window takes the
+    brute force"""
+    import exact_reg as XR
+    rs = np.random.RandomState(24)
+    box = rs.uniform(0, 2.0, (6000, 3))
+    g = np.arange(-5, 6) * 0.125
+    lat = np.stack(np.meshgrid(g, g, g, indexing="ij"), -1).reshape(-1, 3)
+    lat = lat[rs.permutation(len(lat))]
+    for pts in (box, lat):
+        qi = np.sort(rs.choice(len(pts), 300, replace=False))
+        want = np.array(XR.knn_exact(pts, qi, 20))
+        got, n_brute = F.exact_knn_sample(_t(pts), qi, 20, m0, 1.0)
+        np.testing.assert_array_equal(got, want)
+        got, n_brute = F.exact_knn_sample(_t(pts), qi, 20, 1 / 256, 1 / 128)
+        np.testing.assert_array_equal(got, want)
+        assert n_brute == len(qi)
+    # a tie at the 20th place: the lattice's central queries have 6 + 12 + 8 neighbours within sqrt(3) spacings
+    d = np.sort(X.d2_kd(lat[want[0][0]], lat))
+    assert d[19] == d[20] or d[19] == d[18]
+
+
+def test_knn_window_needs_the_kth_neighbour_inside():
+    """the window (3 x 3 x 3 cells of edge 1, 1.5 from the query at its nearest face) holds a 21st neighbour at 1.598, but
+    the true 21st lies 1.55 away outside it: not proven, and the fallback finds it"""
+    import exact_reg as XR
+    m = 1.0
+    q = np.array([[0.5, 0.5, 0.5]])
+    near = q + np.random.RandomState(25).uniform(-0.05, 0.05, (19, 3))
+    inside = np.array([[0.5 + 1.13, 0.5 + 1.13, 0.5]])         # cell (1, 1, 0): in the window, d = 1.598
+    outside = np.array([[0.5 + 1.55, 0.5, 0.5]])               # cell (2, 0, 0): outside it, d = 1.55
+    ref = np.concatenate([q, near, inside, outside])
+    pts, idx = F.crop(_t(ref), _t(q), m)
+    assert list(idx) == list(range(21))
+    nb, dk, proven = F.window_knn(q, pts, idx, m, 21)
+    assert nb[0][-1] == 20 and not proven[0]
+    got, n_brute = F.exact_knn_sample(_t(ref), [0], 21, 1.0, 1.0)
+    assert n_brute == 1 and got[0][-1] == 21
+    np.testing.assert_array_equal(got[0], XR.knn_exact(ref, [0], 21)[0])
+
+
+def test_normal_check_accepts_fast_eigen_and_rejects_a_tilted_normal():
+    """check_normals_sample on a 1 mm-noise tilted plane: FastEigen3x3's normal of the rounded covariance passes, the same
+    normal tilted by 1e-3 rad does not"""
+    import exact_reg as XR
+    pts = tilted_plane(1e-3, np.zeros(3), 4000, 26)
+    qi = np.arange(0, 4000, 40)
+    nbs, _ = F.exact_knn_sample(_t(pts), qi, 20, 1 / 16, 1.0)
+    rows = XR.normals_exact(pts, qi, nbs=list(nbs))
+    good = np.array([r["stmt"] for r in rows])
+    checked, signed, worst = F.check_normals_sample(_t(pts), qi, nbs, good)
+    assert checked == len(qi) and signed > 0 and worst <= 1.0
+    c, s_ = math.cos(1e-3), math.sin(1e-3)
+    bad = good @ np.array([[c, -s_, 0], [s_, c, 0], [0, 0, 1]]).T
+    with pytest.raises(AssertionError):
+        F.check_normals_sample(_t(pts), qi, nbs, bad)

@@ -57,36 +57,6 @@ def api():
     return _api
 
 
-class Meter:
-    """device memory in use beyond the start (sampled after each stage) and wall time"""
-
-    def __init__(self, torch):
-        self.torch = torch
-        torch.cuda.synchronize()
-        free, total = torch.cuda.mem_get_info()
-        self.base, self.peak, self.t0 = total - free, 0, time.time()
-
-    def sample(self):
-        self.torch.cuda.synchronize()
-        free, total = self.torch.cuda.mem_get_info()
-        self.peak = max(self.peak, total - free - self.base)
-
-
-def _sweep_offsets(trace, r, maxabs):
-    """the fp32 offset error E of the MME sweep that ran (None: fp64 offsets; 'unknown': a shared lattice whose edge the
-    trace does not bound)"""
-    if "ME_KBIT_MME_GENERIC" in trace:
-        return None
-    if "ME_KBIT_MME_SOLO" in trace:
-        h, rings = 0.5 * r, 2
-    else:
-        rings = [k for k in (1, 2, 3) if any(f"MME_FLAT{k}_" in t or t.endswith(f"MME_ROWS{k}") for t in trace)]
-        if not rings or rings[0] < 2:
-            return "unknown"
-        h, rings = r / (rings[0] - 1), rings[0]
-    return X.mme_offset_error(h, rings, np.full((1, 3), maxabs))
-
-
 def _nn_direction(name, torch, query, ref, idx_h, d2_h, n_uniform, m_min, h_rows, seed, sparse):
     """checks 1 and 2 for one direction; returns what was covered"""
     dev = query.device
@@ -111,7 +81,7 @@ def test_full_size_against_exact(api, name):
     free = torch.cuda.mem_get_info()[0] / 2 ** 30
     if free < PEAK_GB[name]:
         pytest.skip(f"{name} needs {PEAK_GB[name]:.0f} GB of device memory; {free:.1f} GB free")
-    meter = Meter(torch)
+    meter = F.Meter()
     setup = SETUP[name]
     est, gt, cfg = synth_torch.make_pair(name, device=dev)
     n_est, n_gt = len(est), len(gt)
@@ -215,7 +185,7 @@ def test_full_size_against_exact(api, name):
     qh, nbs = F.ball_neighbours(est, mq, r)
     exs = F.mme_sample_exact(qh, nbs, 10)
     maxabs = float(est.abs().max())
-    E = _sweep_offsets(trace, r, maxabs)
+    E = F.sweep_offsets(trace, r, maxabs)
     if E == "unknown":          # a shared-lattice sweep whose cell edge the trace does not bound: B64 + 2 tau
         for ex in exs:
             ex["b64"] += 2 * X.TAU_FP64
