@@ -67,6 +67,8 @@ def kernel_bit_names(mask):
 
 
 # enum me_trace_event: data events in the trace mask, above the sweep bits
+ME_TEV_BOX_REMEMBERED = 28
+ME_TEV_BOX_MISSED = 29
 ME_TEV_KNN_COARSE = 30
 ME_TEV_MME_FP64_FINISH = 31
 TRACE_EVENTS = {k: v for k, v in dict(globals()).items() if k.startswith("ME_TEV_")}

@@ -47,11 +47,18 @@ int ensure_work(me_ctx *ctx, size_t bytes) {
   return ME_OK;
 }
 
-void invalidate_cloud(Cloud &c) {
+static void forget_results(Cloud &c) {
   c.grid_valid = false; c.bbox_valid = false; c.nn_valid = false; c.entropy_valid = false; c.entropy_caller_valid = false;
 }
-static void invalidate(Cloud &c) {      // a new cloud: its normals go as well
-  invalidate_cloud(c);
+// the library moved the points (transform, ICP, drift, degradation, copy): the box of the last build is no guess for them
+void invalidate_cloud(Cloud &c) {
+  forget_results(c);
+  c.last_box_valid = false;
+}
+// a cloud handed over (me_set_cloud*): its normals go as well; the box of the last build stays the guess of the next one,
+// which repeated passes over the same maps hand over every time
+static void invalidate(Cloud &c) {
+  forget_results(c);
   c.normal_valid = false;
 }
 

@@ -75,6 +75,13 @@ struct Cloud {
   double solo_h = 0.0;
   double bbox_min[3], bbox_max[3];
   bool bbox_valid = false;
+  // bbox_spec: bbox_min/max hold the box of the last shared dense build (last_box), not yet measured; the next build
+  // measures the box on the way (cell_count_kernel) and lays the cloud out again if it differs (bbox_missed).  last_box is
+  // kept across me_set_cloud* and dropped when the library moves the points (invalidate_cloud)
+  bool bbox_spec = false, bbox_missed = false;
+  bool last_box_valid = false;
+  long long last_box_n = 0;
+  double last_bmin[3], last_bmax[3];
   Lattice lat;
   P4 *d_sorted = nullptr;       // cell-sorted points
   long long cap_sorted = 0;
@@ -456,6 +463,7 @@ inline CellIndex index_of(const Cloud &c) {
 // stage entry points (implemented in grid.cu / nn.cu / mme.cu / voxel.cu)
 int wait_upload(me_ctx *ctx, int which);
 int compute_bbox(me_ctx *ctx, int which);
+int speculate_bbox(me_ctx *ctx, int which);
 int build_grid(me_ctx *ctx, int which, double solo_h = 0.0);
 double density_edge(const Cloud &c);
 int build_both(me_ctx *ctx);

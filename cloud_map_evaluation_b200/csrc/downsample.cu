@@ -144,7 +144,7 @@ int voxel_downsample(me_ctx *ctx, int which, double voxel_size, int64_t *n_out) 
     cudaFree(c.d_normal);
     c.d_normal = out_nrm; c.cap_normal = cap_nrm;
   }
-  c.grid_valid = false; c.bbox_valid = false; c.nn_valid = false; c.entropy_valid = false; c.entropy_caller_valid = false;
+  invalidate_cloud(c);
   if (n_out) *n_out = nv;
   return ME_OK;
 }

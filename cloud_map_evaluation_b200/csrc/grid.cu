@@ -110,7 +110,24 @@ int compute_bbox(me_ctx *ctx, int which) {
     return fail(ctx, ME_ERR_RANGE, "cloud holds non-finite coordinates (the reference drops them at load, map_eval.cpp:6)");
   for (int k = 0; k < 3; ++k) { c.bbox_min[k] = dec_ordered(h[k]); c.bbox_max[k] = dec_ordered(h[3 + k]); }
   c.bbox_valid = true;
+  c.bbox_spec = false;
   return ME_OK;
+}
+
+static bool slab_wanted(const me_ctx *ctx);
+
+// A cloud handed over again (repeated passes over the same maps) most likely has the box of its last shared dense build:
+// take that box, unmeasured, so that the build plans without a round trip to the host; the build's histogram measures
+// the box on the way and build_grid checks it at its one synchronise.  Not for slab layouts (their builds synchronise
+// more than once) or when the plan is not remembered.
+int speculate_bbox(me_ctx *ctx, int which) {
+  Cloud &c = ctx->cloud[which];
+  if (c.bbox_valid || !c.last_box_valid || c.last_box_n != c.n || slab_wanted(ctx) || getenv("ME_NO_PLAN_CACHE")) return 0;
+  c.bbox_missed = false;
+  for (int k = 0; k < 3; ++k) { c.bbox_min[k] = c.last_bmin[k]; c.bbox_max[k] = c.last_bmax[k]; }
+  c.bbox_valid = true;
+  c.bbox_spec = true;
+  return 1;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -145,20 +162,69 @@ __device__ __forceinline__ void point_cell(double x, double y, double z, const L
   iz = (int)(cz < 0 ? 0 : (cz >= L.dims[2] ? L.dims[2] - 1 : cz));
 }
 
-__global__ void __launch_bounds__(kThreads) cell_count_kernel(const double *__restrict__ xyz, long long n, Lattice L,
-                                                              uint32_t *__restrict__ count, uint32_t *__restrict__ rank) {
+// BOX: the lattice was planned on a remembered box (speculate_bbox); the histogram also reduces the box of the points it
+// stages into box[0..6] (bbox_kernel's layout and encoding: the same box, bit for bit).  Points outside the lattice are
+// clamped to its faces by point_cell, so a wrong guess costs a rebuild, never a write out of bounds.
+template <bool BOX>
+__device__ __forceinline__ void cell_count(const double *__restrict__ xyz, long long n, const Lattice &L,
+                                           uint32_t *__restrict__ count, uint32_t *__restrict__ rank,
+                                           unsigned long long *__restrict__ box) {
   __shared__ __align__(16) double s[3 * kThreads];
   const bool aligned16 = ((uintptr_t)xyz & 15) == 0;
+  double mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
+  unsigned long long bad = 0;
   for (long long p0 = (long long)blockIdx.x * kThreads; p0 < n; p0 += (long long)gridDim.x * kThreads) {
     __syncthreads();
     stage_tile(xyz, n, aligned16, p0, s);
     __syncthreads();
     if (p0 + threadIdx.x < n) {
+      const double x = s[3 * threadIdx.x], y = s[3 * threadIdx.x + 1], z = s[3 * threadIdx.x + 2];
+      if (BOX) {
+        const double v[3] = {x, y, z};
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          if (isfinite(v[k])) { mn[k] = fmin(mn[k], v[k]); mx[k] = fmax(mx[k], v[k]); } else bad++;
+        }
+      }
       int ix, iy, iz;
-      point_cell(s[3 * threadIdx.x], s[3 * threadIdx.x + 1], s[3 * threadIdx.x + 2], L, ix, iy, iz);
+      point_cell(x, y, z, L, ix, iy, iz);
       rank[p0 + threadIdx.x] = atomicAdd(count + ((long long)iz * L.dims[1] + iy) * (long long)L.dims[0] + ix, 1u);
     }
   }
+  if (BOX) {      // warps -> the block's box in shared memory -> one set of global atomics per block
+    __shared__ unsigned long long sbox[7];
+    if (threadIdx.x < 7) sbox[threadIdx.x] = threadIdx.x < 3 ? 0xffffffffffffffffull : 0ull;
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < 3; ++k) { mn[k] = warp_min(mn[k]); mx[k] = warp_max(mx[k]); }
+    bad = (unsigned long long)warp_sum_ll((long long)bad);
+    if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        if (mn[k] <= mx[k]) {
+          atomicMin(sbox + k, enc_ordered(mn[k]));
+          atomicMax(sbox + 3 + k, enc_ordered(mx[k]));
+        }
+      }
+      if (bad) atomicAdd(sbox + 6, bad);
+    }
+    __syncthreads();
+    if (threadIdx.x < 3) atomicMin(box + threadIdx.x, sbox[threadIdx.x]);
+    else if (threadIdx.x < 6) atomicMax(box + threadIdx.x, sbox[threadIdx.x]);
+    else if (threadIdx.x == 6 && sbox[6]) atomicAdd(box + 6, sbox[6]);
+  }
+}
+
+__global__ void __launch_bounds__(kThreads) cell_count_kernel(const double *__restrict__ xyz, long long n, Lattice L,
+                                                              uint32_t *__restrict__ count, uint32_t *__restrict__ rank) {
+  cell_count<false>(xyz, n, L, count, rank, nullptr);
+}
+
+// 5 blocks per SM, as cell_count_kernel gets (47 registers): the running box would otherwise take it to 63 and 4 blocks
+__global__ void __launch_bounds__(kThreads, 5) cell_count_box_kernel(const double *__restrict__ xyz, long long n, Lattice L,
+                                                                     uint32_t *__restrict__ count, uint32_t *__restrict__ rank,
+                                                                     unsigned long long *__restrict__ box) {
+  cell_count<true>(xyz, n, L, count, rank, box);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -442,19 +508,28 @@ static int histogram(me_ctx *ctx, Cloud &c, const Lattice &L) {
   ME_CUDA(ctx, cudaMemsetAsync(c.d_cell_off, 0, (size_t)(L.ncells + 1) * sizeof(uint32_t), ctx->stream));
   ME_TRY(ensure(ctx, (void **)&ctx->d_rank, &ctx->cap_rank, c.n, sizeof(uint32_t)));
   int blocks = (int)std::min<long long>((c.n + kThreads - 1) / kThreads, (long long)ctx->sm_count * 16);
-  cell_count_kernel<<<blocks, kThreads, 0, ctx->stream>>>(c.d_xyz, c.n, L, c.d_cell_off, ctx->d_rank);
+  if (c.bbox_spec) {      // the box is measured here (scratch [0..6]) and read back with the cell statistics
+    unsigned long long *box = (unsigned long long *)ctx->d_scratch;
+    bbox_init_kernel<<<1, 32, 0, ctx->stream>>>(box);
+    ME_LAUNCH_CHECK(ctx);
+    cell_count_box_kernel<<<blocks, kThreads, 0, ctx->stream>>>(c.d_xyz, c.n, L, c.d_cell_off, ctx->d_rank, box);
+  } else {
+    cell_count_kernel<<<blocks, kThreads, 0, ctx->stream>>>(c.d_xyz, c.n, L, c.d_cell_off, ctx->d_rank);
+  }
   ME_LAUNCH_CHECK(ctx);
   return ME_OK;
 }
 
 // exclusive scan of the cell counts, in place, with their statistics on the way: pinned slots [9] occupied cells, [10]
-// points in the fullest cell (bounds the run lengths of the sweeps), valid once the stream is synchronized
+// points in the fullest cell (bounds the run lengths of the sweeps), valid once the stream is synchronized.  On a remembered
+// box the measured box (slots [0..6], see histogram) comes back in the same copy.
 static int scan_cells(me_ctx *ctx, Cloud &c, const Lattice &L) {
   unsigned long long *d = (unsigned long long *)ctx->d_scratch + 9;
   ME_CUDA(ctx, cudaMemsetAsync(d, 0, 2 * sizeof(unsigned long long), ctx->stream));
   ME_TRY(exclusive_scan_inplace(ctx, c.d_cell_off, L.ncells + 1, d));
-  ME_CUDA(ctx, cudaMemcpyAsync((unsigned long long *)ctx->h_pinned + 9, d, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
-                               ctx->stream));
+  const int first = c.bbox_spec ? 0 : 9;
+  ME_CUDA(ctx, cudaMemcpyAsync((unsigned long long *)ctx->h_pinned + first, (unsigned long long *)ctx->d_scratch + first,
+                               (11 - first) * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
   return ME_OK;
 }
 
@@ -870,7 +945,34 @@ int build_grid(me_ctx *ctx, int which, double solo_h) {
   if (c.grid_valid && c.grid_solo == solo && (!solo || c.solo_h == solo_h)) return ME_OK;
   ME_TRY(wait_upload(ctx, which));
   StageTimer timer(ctx, which >= kFeatureSlot ? -1 : (which == ME_CLOUD_EST ? 0 : 1));
+  if (!solo) speculate_bbox(ctx, which);
+  else if (c.bbox_spec) c.bbox_valid = false;      // a solo lattice is planned on the measured box
   ME_TRY(compute_bbox(ctx, which));
+  // what a build on a remembered box changes before the box is checked: restored when it turns out wrong
+  struct {
+    bool o_grid, o_nn, o_entropy, slab_planned;
+    double spec_v; int spec_m;
+    PlanCache pc;
+  } const before = {o.grid_valid, o.nn_valid, o.entropy_valid, ctx->slab_planned, ctx->spec_v, ctx->spec_m,
+                    ctx->plan_cache[which]};
+  // the remembered box is wrong (bad_box) or the plan on it needs a sparse table (built on the measured box only): undo,
+  // take the measured box and build again
+  auto restart = [&](const unsigned long long *bad_box) -> int {
+    o.grid_valid = before.o_grid; o.nn_valid = before.o_nn; o.entropy_valid = before.o_entropy;
+    ctx->slab_planned = before.slab_planned; ctx->spec_v = before.spec_v; ctx->spec_m = before.spec_m;
+    ctx->plan_cache[which] = before.pc;
+    c.bbox_valid = false; c.bbox_spec = false;
+    if (!bad_box) ME_TRY(compute_bbox(ctx, which));
+    else {
+      if (bad_box[6] != 0)
+        return fail(ctx, ME_ERR_RANGE, "cloud holds non-finite coordinates (the reference drops them at load, map_eval.cpp:6)");
+      for (int k = 0; k < 3; ++k) { c.bbox_min[k] = dec_ordered(bad_box[k]); c.bbox_max[k] = dec_ordered(bad_box[3 + k]); }
+      c.bbox_valid = true;
+      c.bbox_missed = true;
+      trace_kernel(ctx, ME_TEV_BOX_MISSED);
+    }
+    return build_grid(ctx, which, solo_h);
+  };
   const long long budget = grid_budget(ctx);
   const double v_req = ctx->voxel_hint;
   const bool sp = sparse_allowed();
@@ -891,6 +993,7 @@ int build_grid(me_ctx *ctx, int which, double solo_h) {
     else ME_TRY(histogram(ctx, c, L));
   } else if (o.grid_valid && !o.grid_solo && ctx->spec_m > 0 && (v_req <= 0 || ctx->spec_v == v_req) &&
              make_lattice(c, ctx->spec_v, ctx->spec_m, budget, &L, sp)) {
+    if (L.sparse && c.bbox_spec) return restart(nullptr);
     if (L.sparse) { ME_TRY(build_sparse(ctx, c, L, &occupied)); built = true; }
     else ME_TRY(histogram(ctx, c, L));
   } else {
@@ -918,6 +1021,7 @@ int build_grid(me_ctx *ctx, int which, double solo_h) {
       const bool ok = choose_lattice(c, other, v_req, h_target, budget, sp, &v, &m, &cand);
       if (!ok) {
         if (have) break;      // the refined edge does not fit: keep the lattice of the previous iteration
+        if (c.bbox_spec) return restart(nullptr);
         return fail(ctx, ME_ERR_RANGE, v_req > 0 ? "voxel size too small for the lattice (dense budget and sparse limits exceeded)"
                                                  : "cannot fit the cloud into the lattice");
       }
@@ -925,6 +1029,7 @@ int build_grid(me_ctx *ctx, int which, double solo_h) {
       L = cand; have = true;
       h_used = h_target;
       ctx->spec_v = v; ctx->spec_m = m;
+      if (L.sparse && c.bbox_spec) return restart(nullptr);
       if (L.sparse) { ME_TRY(build_sparse(ctx, c, L, &occupied)); built = true; }
       else { built = false; scanned = false; ME_TRY(histogram(ctx, c, L)); }
       if (ctx->nn_cell_size > 0) break;   // caller fixed the cell size
@@ -1022,6 +1127,19 @@ int build_grid(me_ctx *ctx, int which, double solo_h) {
     }
     ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     c.max_cell_count = (long long)((unsigned long long *)ctx->h_pinned)[10];
+    if (c.bbox_spec) {      // the box the histogram measured (scan_cells brought it back with the statistics)
+      const unsigned long long *h = (const unsigned long long *)ctx->h_pinned;
+      bool same = h[6] == 0;
+      for (int k = 0; k < 3; ++k) same = same && h[k] == enc_ordered(c.bbox_min[k]) && h[3 + k] == enc_ordered(c.bbox_max[k]);
+      if (!same) return restart(h);
+      c.bbox_spec = false;
+      trace_kernel(ctx, ME_TEV_BOX_REMEMBERED);
+    }
+    if (!solo && !c.slab) {      // the box a later build of this cloud may start from
+      c.last_box_valid = true;
+      c.last_box_n = c.n;
+      for (int k = 0; k < 3; ++k) { c.last_bmin[k] = c.bbox_min[k]; c.last_bmax[k] = c.bbox_max[k]; }
+    }
   }
   ME_TRY(build_coarse(ctx, c));
   c.tiles_valid = false;

@@ -583,18 +583,29 @@ __global__ void unsort_f64_kernel(const P4 *__restrict__ S, long long n, const d
 
 // The lattice of a radius sweep (MME, local consistency) of cloud `which`: *solo = lay the cloud out on a lattice of its own
 // with h = r/2, else on the shared lattice.  The caller lays it out: build_grid(ctx, which, *solo ? 0.5 * radius : 0.0).
+// On a remembered plan the box is not measured ahead of the build: the decision is taken on the remembered box and the
+// build checks it; if the box was another, the decision is taken again on the measured one.
 int radius_lattice(me_ctx *ctx, int which, double radius, bool *solo) {
   Cloud &c = ctx->cloud[which];
   ME_TRY(wait_upload(ctx, which));
-  ME_TRY(compute_bbox(ctx, which));
+  const bool remembered = speculate_bbox(ctx, which);
+  if (!remembered) ME_TRY(compute_bbox(ctx, which));
   *solo = false;
   if (!getenv("ME_MME_SHARED_LATTICE")) {
     const double h_now = (c.grid_valid && !c.grid_solo) ? c.lat.h : (ctx->nn_cell_size > 0 ? ctx->nn_cell_size : density_edge(c));
     *solo = radius / h_now > 3.0 + 1e-9;
     if (!*solo && !(c.grid_valid && !c.grid_solo)) {      // the estimate may be refined downwards by the build
       ME_TRY(build_grid(ctx, which));
-      *solo = radius / c.lat.h > 3.0 + 1e-9;
+      // a wrong remembered box: the decision the measured box gives (the shared lattice it was laid out on is then
+      // replaced by the solo build, as after any MME sweep on a solo lattice)
+      if (remembered && c.bbox_missed && radius / (ctx->nn_cell_size > 0 ? ctx->nn_cell_size : density_edge(c)) > 3.0 + 1e-9) *solo = true;
+      else *solo = radius / c.lat.h > 3.0 + 1e-9;
     }
+  }
+  if (c.bbox_spec) {      // decided without a build that checks the box: measure it and decide again
+    c.bbox_valid = false;
+    ME_TRY(compute_bbox(ctx, which));
+    return radius_lattice(ctx, which, radius, solo);
   }
   return ME_OK;
 }

@@ -172,7 +172,9 @@ __device__ __forceinline__ void search_block_global(const P4 &q, long long ix, l
 
 // after the 3x3x3 block: is the best provably the global nearest neighbour?  If so record it (index, nanoflann-order d2 for
 // the cut-off, Eigen-order squared norm for the statistics; nn_stats_kernel folds them into the accumulators), otherwise
-// hand the query to the ring-expansion kernel.
+// hand the query to the ring-expansion kernel.  AW: ME_PAIRING_AS_WRITTEN gt->est (C.accumulate == 0), compiled apart so
+// that the other sweeps keep their code (and AW's drops the winner's offsets, which only the Eigen-order norm reads).
+template <bool AW>
 __device__ __forceinline__ void finish_query(const P4 &q, uint32_t i, long long ix, long long iy, long long iz,
                                              const Lattice &L, const NNConst &C, const Best &b,
                                              int32_t *__restrict__ nn_idx, double *__restrict__ nn_d2,
@@ -197,7 +199,11 @@ __device__ __forceinline__ void finish_query(const P4 &q, uint32_t i, long long 
   if (beyond || !(b.d2 < INFINITY)) { nn_idx[i] = -1; nn_d2[i] = INFINITY; return; }
   nn_idx[i] = b.idx;
   nn_d2[i] = b.d2;
-  nn_sq[i] = sqnorm_eigen(b.dx, b.dy, b.dz);
+  if (!AW) nn_sq[i] = sqnorm_eigen(b.dx, b.dy, b.dz);
+  // as-written: the swapped pair's squared norm (two random gathers, issued here inside the latency-bound sweep) for
+  // pair_as_written_kernel to fold; pairs past the cut-off are never read
+  else if (keep_pair(b.d2, C))
+    nn_sq[i] = as_written_sq(b.idx, orig_of(q.idx), C.aw_gt_xyz, C.aw_n_gt, C.aw_est_xyz, C.aw_n_est);
 }
 
 // clamp a (possibly far outside) lattice coordinate to one cell beyond the lattice
@@ -216,6 +222,7 @@ static constexpr int kRegRows = kRegW * kRegW;         // 36 rows
 static constexpr int kNNCap = 640;                     // staged candidates per tile (48 B each)
 static constexpr int kSegs = kTileEdge * kTileEdge;    // 16 query row segments per tile
 
+template <bool AW>
 __global__ void __launch_bounds__(kTileThreads)
 nn_tile_kernel(const P4 *__restrict__ Q, const uint32_t *__restrict__ q_off, Lattice Lq,
                const uint32_t *__restrict__ tiles, long long t_begin, long long t_end, const P4 *__restrict__ R,
@@ -380,7 +387,7 @@ nn_tile_kernel(const P4 *__restrict__ Q, const uint32_t *__restrict__ q_off, Lat
         search_block_global(q, r0x + lx, r0y + ly, r0z + lz, R, r_off, Lr, b);
       }
       // the searched block is centred on the query's own (unclamped) reference cell; the far kernel restarts from ring 0
-      finish_query(q, pos, r0x + lx, r0y + ly, r0z + lz, Lr, C, b, nn_idx, nn_d2, nn_sq, far_list, far_count,
+      finish_query<AW>(q, pos, r0x + lx, r0y + ly, r0z + lz, Lr, C, b, nn_idx, nn_d2, nn_sq, far_list, far_count,
                    cell_coord_cont(q.x, Lr, 0), cell_coord_cont(q.y, Lr, 1), cell_coord_cont(q.z, Lr, 2), 1e-9);
     }
     __syncthreads();   // shared tables and the staged region are re-used by the next tile
@@ -408,7 +415,7 @@ struct FlatGeom {
   double inv_h;
 };
 
-template <bool E16, int U2>      // U2: 0 plain walk, 1 two candidates (two loads in flight) per iteration
+template <bool E16, int U2, bool AW>      // U2: 0 plain walk, 1 two candidates (two loads in flight) per iteration
 // 8 CTAs/SM: faster on C3 than 10 or 12 (spills + less L1; chosen on B200, not re-measured on H100)
 __global__ void __launch_bounds__(kFlatThreads, 8)
 nn_flat_kernel(const P4 *__restrict__ Q, const float4 *__restrict__ qrel, long long q_begin, long long q_end,
@@ -497,7 +504,7 @@ nn_flat_kernel(const P4 *__restrict__ Q, const float4 *__restrict__ qrel, long l
       }
     }
     // position inside the own cell from the cell-relative copy (error ~1e-7 cells, covered by the face-test slack)
-    finish_query(q, (uint32_t)i, cx, cy, cz, Lr, C, b, nn_idx, nn_d2, nn_sq, far_list, far_count,
+    finish_query<AW>(q, (uint32_t)i, cx, cy, cz, Lr, C, b, nn_idx, nn_d2, nn_sq, far_list, far_count,
                  (double)cx + (double)qr.x * G.inv_h, (double)cy + (double)qr.y * G.inv_h,
                  (double)cz + (double)qr.z * G.inv_h, 2e-6);
   }
@@ -510,7 +517,8 @@ nn_flat_kernel(const P4 *__restrict__ Q, const float4 *__restrict__ qrel, long l
 // row of the reference cloud: a window of a few consecutive 128-byte lines instead of up to nine rows at once, no run
 // table in shared memory, no per-lane refill branches.  The near-tie pass re-walks the rows the same way.
 // ---------------------------------------------------------------------------------------------------------------
-template <int U, int SP>      // U candidates loaded per inner iteration (all issued before the first test); SP: sparse reference table
+// U candidates loaded per inner iteration (all issued before the first test); SP: sparse reference table; AW: finish_query
+template <int U, int SP, bool AW>
 __global__ void __launch_bounds__(kFlatThreads, (U <= 2 ? 8 : (U <= 4 ? 6 : 4)))
 nn_rows_kernel(const P4 *__restrict__ Q, const float4 *__restrict__ qrel, long long q_begin, long long q_end,
                const P4 *__restrict__ R, const float4 *__restrict__ rrel, CellIndex Ir,
@@ -598,7 +606,7 @@ nn_rows_kernel(const P4 *__restrict__ Q, const float4 *__restrict__ qrel, long l
         }
       }
     }
-    finish_query(q, (uint32_t)i, cx, cy, cz, Lr, C, b, nn_idx, nn_d2, nn_sq, far_list, far_count,
+    finish_query<AW>(q, (uint32_t)i, cx, cy, cz, Lr, C, b, nn_idx, nn_d2, nn_sq, far_list, far_count,
                  (double)cx + (double)qr.x * G.inv_h, (double)cy + (double)qr.y * G.inv_h,
                  (double)cz + (double)qr.z * G.inv_h, 2e-6);
   }
@@ -790,10 +798,11 @@ nn_brute_kernel(const P4 *__restrict__ Q, const double *__restrict__ ref_xyz, lo
   }
 }
 
-// far queries: Eigen-order squared norm of (query - winner); the winner's coordinates come from the caller-order array
+// far queries: Eigen-order squared norm of (query - winner); the winner's coordinates come from the caller-order array.
+// ME_PAIRING_AS_WRITTEN gt->est (C.accumulate == 0): the as-written pair's, as finish_query gives it to the swept queries
 __global__ void __launch_bounds__(kThreads)
 nn_far_sq_kernel(const P4 *__restrict__ Q, const double *__restrict__ ref_xyz, const int32_t *__restrict__ nn_idx,
-                 double *__restrict__ nn_sq, const uint32_t *__restrict__ far_list,
+                 const double *__restrict__ nn_d2, NNConst C, double *__restrict__ nn_sq, const uint32_t *__restrict__ far_list,
                  const unsigned int *__restrict__ far_count) {
   const unsigned int nfar = *far_count;
   for (long long w = blockIdx.x * (long long)blockDim.x + threadIdx.x; w < nfar; w += (long long)gridDim.x * blockDim.x) {
@@ -801,6 +810,10 @@ nn_far_sq_kernel(const P4 *__restrict__ Q, const double *__restrict__ ref_xyz, c
     const int32_t j = nn_idx[i];
     if (j < 0) continue;
     const P4 q = load_p4(Q + i);
+    if (!C.accumulate) {
+      if (keep_pair(nn_d2[i], C)) nn_sq[i] = as_written_sq(j, orig_of(q.idx), C.aw_gt_xyz, C.aw_n_gt, C.aw_est_xyz, C.aw_n_est);
+      continue;
+    }
     const double px = __ldg(ref_xyz + 3ll * j), py = __ldg(ref_xyz + 3ll * j + 1), pz = __ldg(ref_xyz + 3ll * j + 2);
     nn_sq[i] = sqnorm_eigen(__dsub_rn(q.x, px), __dsub_rn(q.y, py), __dsub_rn(q.z, pz));
   }
@@ -823,20 +836,19 @@ nn_stats_kernel(long long i_begin, long long i_end, const int32_t *__restrict__ 
   flush_acc(a, acc, mom);
 }
 
-// ME_PAIRING_AS_WRITTEN gt->est (as_written_pair, records.cuh).  Walks every gt point; points this rank did not evaluate
-// carry the marker -2.
+// ME_PAIRING_AS_WRITTEN gt->est (as_written_pair, records.cuh), a streaming fold of the records: the sweep and
+// nn_far_sq_kernel left the squared norm of every kept as-written pair in nn_sq (kAwOutOfRangeSq: out of range).  Walks
+// every gt point; points this rank did not evaluate carry the marker -2.
 __global__ void __launch_bounds__(kThreads, 4)      // as nn_stats_kernel
-pair_as_written_kernel(const P4 *__restrict__ Qgt, long long n, const int32_t *__restrict__ nn_idx,
-                       const double *__restrict__ nn_d2, const double *__restrict__ gt_xyz, long long n_gt,
-                       const double *__restrict__ est_xyz, long long n_est, NNConst C, AccBlock *__restrict__ acc,
-                       double *__restrict__ mom) {
+pair_as_written_kernel(long long n, const int32_t *__restrict__ nn_idx, const double *__restrict__ nn_d2,
+                       const double *__restrict__ nn_sq, NNConst C, AccBlock *__restrict__ acc, double *__restrict__ mom) {
   LocalAcc a;
   a.clear();
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    double sq;
-    const int r = as_written_pair(Qgt, i, nn_idx, nn_d2, gt_xyz, n_gt, est_xyz, n_est, C, sq);
-    if (r == kAwOutOfRange) a.ub();
-    else if (r == kAwPair) accum_sq(sq, C, a);
+    if (__ldg(nn_idx + i) < 0 || !keep_pair(__ldg(nn_d2 + i), C)) continue;
+    const double sq = __ldg(nn_sq + i);
+    if (sq < 0) a.ub();
+    else accum_sq(sq, C, a);
   }
   flush_acc(a, acc, mom);
 }
@@ -1112,6 +1124,8 @@ static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, int sta
   C.cov_dim = Rc.slab ? Rc.lat.dims[Rc.sl_axis] : 0;
   C.ref_maxabs = 0;
   for (int a = 0; a < 3; ++a) C.ref_maxabs = std::max(C.ref_maxabs, std::max(std::fabs(Rc.bbox_min[a]), std::fabs(Rc.bbox_max[a])));
+  C.aw_gt_xyz = Qc.d_xyz; C.aw_n_gt = Qc.n;      // read only when as_written (Qc is the gt cloud then)
+  C.aw_est_xyz = Rc.d_xyz; C.aw_n_est = Rc.n;
 
   // the flat kernel packs run lengths into 24 bits and x indices into an fp32 mantissa; otherwise the tile kernel runs
   const bool any_sparse = Qc.lat.sparse || Rc.lat.sparse;
@@ -1150,14 +1164,19 @@ static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, int sta
     fill_i32_kernel<<<fill_blocks, kThreads, 0, ctx->stream>>>(Qc.d_nn_idx, Qc.n, -2);
     ME_LAUNCH_CHECK(ctx);
   }
+  // the sweeps, compiled for the as-written pairing apart (finish_query)
+  auto *const tile_kernel = as_written ? nn_tile_kernel<true> : nn_tile_kernel<false>;
+  auto *const flat_kernel = as_written ? nn_flat_kernel<true, 0, true> : nn_flat_kernel<true, 0, false>;
+  auto *const rows_sparse = as_written ? nn_rows_kernel<4, 1, true> : nn_rows_kernel<4, 1, false>;
+  auto *const rows_dense = as_written ? nn_rows_kernel<4, 0, true> : nn_rows_kernel<4, 0, false>;
   const size_t dyn_smem = (size_t)kNNCap * (sizeof(P4) + sizeof(float4));
   if (use_tile)      // per launch: function attributes are per device
-    ME_CUDA(ctx, cudaFuncSetAttribute(nn_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_smem));
+    ME_CUDA(ctx, cudaFuncSetAttribute(tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_smem));
   if (use_tile ? te > tb : qe > qb) {
     if (use_tile) {
       // persistent CTAs: each walks tiles tb + blockIdx.x, + gridDim.x, ... and flushes its accumulators once
       const unsigned grid = (unsigned)std::min<long long>(te - tb, (long long)ctx->sm_count * 16);
-      nn_tile_kernel<<<grid, kTileThreads, dyn_smem, ctx->stream>>>(
+      tile_kernel<<<grid, kTileThreads, dyn_smem, ctx->stream>>>(
           Qc.d_sorted, Qc.d_cell_off, Qc.lat, Qc.d_tiles, tb, te, Rc.d_sorted, Rc.d_cell_off, Rc.lat, C, Qc.d_nn_idx,
           Qc.d_nn_d2, Qc.d_nn_sq, far_list, far_count);
       trace_kernel(ctx, ME_KBIT_NN_TILE);
@@ -1181,19 +1200,16 @@ static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, int sta
       // against 1.7 / 2.4 ms for the run-table walk, which stays behind ME_NN_KERNEL=flat)
       const char *kv = getenv("ME_NN_KERNEL");
       if (kv && !strcmp(kv, "flat")) {
-        nn_flat_kernel<true, 0><<<grid, kFlatThreads, 0, ctx->stream>>>(Qc.d_sorted, Qc.d_rel, qb, qe, Rc.d_sorted, Rc.d_rel,
-                                                                        index_of(Rc), Rc.lat, G, C, Qc.d_nn_idx, Qc.d_nn_d2,
-                                                                        Qc.d_nn_sq, far_list, far_count);
+        flat_kernel<<<grid, kFlatThreads, 0, ctx->stream>>>(Qc.d_sorted, Qc.d_rel, qb, qe, Rc.d_sorted, Rc.d_rel, index_of(Rc),
+                                                            Rc.lat, G, C, Qc.d_nn_idx, Qc.d_nn_d2, Qc.d_nn_sq, far_list, far_count);
         trace_kernel(ctx, ME_KBIT_NN_FLAT);
       } else if (Rc.lat.sparse) {
-        nn_rows_kernel<4, 1><<<grid, kFlatThreads, 0, ctx->stream>>>(Qc.d_sorted, Qc.d_rel, qb, qe, Rc.d_sorted, Rc.d_rel,
-                                                                     index_of(Rc), Rc.lat, G, C, Qc.d_nn_idx, Qc.d_nn_d2,
-                                                                     Qc.d_nn_sq, far_list, far_count);
+        rows_sparse<<<grid, kFlatThreads, 0, ctx->stream>>>(Qc.d_sorted, Qc.d_rel, qb, qe, Rc.d_sorted, Rc.d_rel, index_of(Rc),
+                                                            Rc.lat, G, C, Qc.d_nn_idx, Qc.d_nn_d2, Qc.d_nn_sq, far_list, far_count);
         trace_kernel(ctx, ME_KBIT_NN_ROWS_SPARSE);
       } else {
-        nn_rows_kernel<4, 0><<<grid, kFlatThreads, 0, ctx->stream>>>(Qc.d_sorted, Qc.d_rel, qb, qe, Rc.d_sorted, Rc.d_rel,
-                                                                     index_of(Rc), Rc.lat, G, C, Qc.d_nn_idx, Qc.d_nn_d2,
-                                                                     Qc.d_nn_sq, far_list, far_count);
+        rows_dense<<<grid, kFlatThreads, 0, ctx->stream>>>(Qc.d_sorted, Qc.d_rel, qb, qe, Rc.d_sorted, Rc.d_rel, index_of(Rc),
+                                                           Rc.lat, G, C, Qc.d_nn_idx, Qc.d_nn_d2, Qc.d_nn_sq, far_list, far_count);
         trace_kernel(ctx, ME_KBIT_NN_ROWS_DENSE);
       }
     }
@@ -1207,11 +1223,9 @@ static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, int sta
                                                                       unres_list, unres_count, ctx->d_trace);
       ME_LAUNCH_CHECK(ctx);
     }
-    if (C.accumulate) {
-      nn_far_sq_kernel<<<ctx->sm_count, kThreads, 0, ctx->stream>>>(Qc.d_sorted, Rc.d_xyz, Qc.d_nn_idx, Qc.d_nn_sq, far_list,
-                                                                    far_count);
-      ME_LAUNCH_CHECK(ctx);
-    }
+    nn_far_sq_kernel<<<ctx->sm_count, kThreads, 0, ctx->stream>>>(Qc.d_sorted, Rc.d_xyz, Qc.d_nn_idx, Qc.d_nn_d2, C, Qc.d_nn_sq,
+                                                                  far_list, far_count);
+    ME_LAUNCH_CHECK(ctx);
     int mom_slots = 0;     // blocks of the kernel that kept the pairs
     if (C.accumulate || C.want_full_cd) {
       const long long sb = use_tile ? 0 : qb, se = use_tile ? Qc.n : qe;
@@ -1222,8 +1236,7 @@ static int run_direction(me_ctx *ctx, int qwhich, const me_nn_params *p, int sta
       if (C.accumulate) mom_slots = sblocks;
     }
     if (as_written) {
-      pair_as_written_kernel<<<fill_blocks, kThreads, 0, ctx->stream>>>(Qc.d_sorted, Qc.ns, Qc.d_nn_idx, Qc.d_nn_d2,
-                                                                       Qc.d_xyz, Qc.n, Rc.d_xyz, Rc.n, C, acc, mom);
+      pair_as_written_kernel<<<fill_blocks, kThreads, 0, ctx->stream>>>(Qc.ns, Qc.d_nn_idx, Qc.d_nn_d2, Qc.d_nn_sq, C, acc, mom);
       ME_LAUNCH_CHECK(ctx);
       mom_slots = fill_blocks;
     }

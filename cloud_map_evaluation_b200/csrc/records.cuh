@@ -14,6 +14,9 @@ struct NNConst {
   int want_full_cd;
   double max_d2;        // nothing beyond this squared distance matters (inf when full CD is wanted)
   double ref_maxabs;    // max |coordinate| of the reference cloud (slack of the face test)
+  // ME_PAIRING_AS_WRITTEN gt->est (accumulate == 0): the caller-order clouds the sweep reads the as-written pair from
+  const double *aw_gt_xyz, *aw_est_xyz;
+  long long aw_n_gt, aw_n_est;
   // slab layout: only the planes [cov_lo, cov_hi) of the reference lattice along axis cov_axis (1: y, 2: z; 0: everything)
   // are laid out on this rank
   int cov_axis, cov_lo, cov_hi, cov_dim;
@@ -43,6 +46,20 @@ __device__ __forceinline__ void accum_sq(double sq, const NNConst &c, Acc &a) {
 // Walks every gt point; points this rank did not evaluate carry the marker -2.
 // ---------------------------------------------------------------------------------------------------------------
 enum { kAwNone = 0, kAwOutOfRange = 1, kAwPair = 2 };
+// the nn_sq record of an out-of-range pair (a squared norm is never negative)
+static constexpr double kAwOutOfRangeSq = -1.0;
+
+// Eigen's squaredNorm of gt[s] - est[t] for source index s = nn_est into gt and target index t = i_gt into est, or
+// kAwOutOfRangeSq when either index is past its cloud
+__device__ __forceinline__ double as_written_sq(long long s, long long t, const double *__restrict__ gt_xyz, long long n_gt,
+                                                const double *__restrict__ est_xyz, long long n_est) {
+  if (s >= n_gt || t >= n_est) return kAwOutOfRangeSq;
+  const double dx = __dsub_rn(__ldg(gt_xyz + 3 * s), __ldg(est_xyz + 3 * t));
+  const double dy = __dsub_rn(__ldg(gt_xyz + 3 * s + 1), __ldg(est_xyz + 3 * t + 1));
+  const double dz = __dsub_rn(__ldg(gt_xyz + 3 * s + 2), __ldg(est_xyz + 3 * t + 2));
+  return sqnorm_eigen(dx, dy, dz);
+}
+
 // gt query i (sorted order): kAwNone (no kept pair), kAwOutOfRange (counted in n_ub) or kAwPair with sq = Eigen's
 // squaredNorm of gt[nn_est] - est[i_gt]
 __device__ __forceinline__ int as_written_pair(const P4 *__restrict__ Qgt, long long i, const int32_t *__restrict__ nn_idx,
@@ -52,13 +69,8 @@ __device__ __forceinline__ int as_written_pair(const P4 *__restrict__ Qgt, long 
   if (nn_est < 0) return kAwNone;
   if (!keep_pair(nn_d2[i], C)) return kAwNone;
   const long long i_gt = orig_of(__double_as_longlong(__ldg(reinterpret_cast<const double *>(Qgt + i) + 3)));
-  const long long s = nn_est, t = i_gt;          // source index into gt, target index into est
-  if (s >= n_gt || t >= n_est) return kAwOutOfRange;
-  const double dx = __dsub_rn(__ldg(gt_xyz + 3 * s), __ldg(est_xyz + 3 * t));
-  const double dy = __dsub_rn(__ldg(gt_xyz + 3 * s + 1), __ldg(est_xyz + 3 * t + 1));
-  const double dz = __dsub_rn(__ldg(gt_xyz + 3 * s + 2), __ldg(est_xyz + 3 * t + 2));
-  sq = sqnorm_eigen(dx, dy, dz);
-  return kAwPair;
+  sq = as_written_sq(nn_est, i_gt, gt_xyz, n_gt, est_xyz, n_est);
+  return sq < 0 ? kAwOutOfRange : kAwPair;
 }
 
 struct CurveSrc {           // the per-query records of one direction

@@ -763,9 +763,12 @@ enum me_kernel_bit {
   ME_KBIT_SCS_RT_UNCACHED = 21,    /* scs_kernel, run-time radius too large for the per-lane cache         */
   ME_KBIT_COUNT = 22
 };
-/* Data events of the same mask, above the sweep bits.  They record what the data made a sweep do rather than which sweep
- * ran, so they are not part of enum me_kernel_bit; they are set on the device only when a query reaches the path. */
+/* Data events of the same mask, above the sweep bits.  They record what the data made a sweep or a lattice build do rather
+ * than which sweep ran, so they are not part of enum me_kernel_bit; a sweep's events are set on the device only when a
+ * query reaches the path. */
 enum me_trace_event {
+  ME_TEV_BOX_REMEMBERED = 28,      /* a lattice build planned on the remembered box of its cloud, and the box held     */
+  ME_TEV_BOX_MISSED = 29,          /* ... and the box it measured was another: the cloud was laid out again            */
   ME_TEV_KNN_COARSE = 30,          /* a k-NN walk query left the fine rings for the coarse blocks (normals, FPFH)      */
   ME_TEV_MME_FP64_FINISH = 31      /* an fp32-offset MME sweep left queries to mme_fp64_finish_kernel (thin surfaces)  */
 };
