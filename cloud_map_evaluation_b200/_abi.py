@@ -229,6 +229,27 @@ class me_consistency_result(C.Structure):
                 ("mean_plane_std", C.c_double), ("max_pv", C.c_double)]
 
 
+# the mutually orthogonal metric without a ground truth (me_mom*)
+ME_MOM_CELLS_PER_EDGE = 16
+ME_MOM_BINS = 6 * ME_MOM_CELLS_PER_EDGE * ME_MOM_CELLS_PER_EDGE
+ME_MOM_BLOCK = 6 + 3 * 4 * 256
+ME_MOM_OK, ME_MOM_NO_PLANAR, ME_MOM_NO_SECOND_AXIS, ME_MOM_SMALL_FAMILY = 0, 1, 2, 3
+MOM_STATUS_NAMES = {ME_MOM_OK: "OK", ME_MOM_NO_PLANAR: "NO_PLANAR", ME_MOM_NO_SECOND_AXIS: "NO_SECOND_AXIS",
+                    ME_MOM_SMALL_FAMILY: "SMALL_FAMILY"}
+
+
+class me_mom_params(C.Structure):
+    _fields_ = [("angle_deg", C.c_double), ("planarity", C.c_double), ("min_family", C.c_int64)]
+
+
+class me_mom_result(C.Structure):
+    _fields_ = [("radius", C.c_double), ("angle_deg", C.c_double), ("planarity", C.c_double), ("min_family", C.c_int64),
+                ("min_neighbors", C.c_int32), ("kernel", C.c_int32), ("rings", C.c_int32), ("solo", C.c_int32),
+                ("n_points", C.c_int64), ("n_query", C.c_int64), ("n_pv", C.c_int64), ("n_planar", C.c_int64),
+                ("axis", C.c_double * 9), ("n", C.c_int64 * 3), ("mean", C.c_double * 3), ("median", C.c_double * 3),
+                ("mom", C.c_double), ("status", C.c_int32), ("reserved", C.c_int32)]
+
+
 class me_mme_accum(C.Structure):
     _fields_ = [("n_query", C.c_int64), ("n_valid", C.c_int64), ("sum_entropy", C.c_double),
                 ("min_entropy", C.c_double), ("max_entropy", C.c_double)]

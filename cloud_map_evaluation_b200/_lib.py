@@ -33,6 +33,7 @@ SYMBOLS = (
     "me_surface_finalize",
     "me_consistency_begin", "me_consistency_block", "me_consistency_end", "me_consistency", "me_consistency_finalize",
     "me_get_consistency_points",
+    "me_mom_begin", "me_mom_block", "me_mom_step", "me_mom_end", "me_mom", "me_mom_axes", "me_get_mom_points",
 )
 
 _lib = None
@@ -155,6 +156,13 @@ def load():
     L.me_consistency_finalize.argtypes = [C.c_int64, C.c_double, i64p, i64p, C.c_int64, dp, C.c_void_p,
                                           C.POINTER(A.me_consistency_result)]
     L.me_get_consistency_points.argtypes = [ctx, C.c_int, C.c_void_p, C.c_void_p]
+    L.me_mom_begin.argtypes = [ctx, C.c_int, C.c_double, C.c_int32, C.POINTER(A.me_mom_params)]
+    L.me_mom_block.argtypes = [ctx, C.POINTER(dp), C.POINTER(C.c_int32)]
+    L.me_mom_step.argtypes = [ctx, C.POINTER(C.c_int32)]
+    L.me_mom_end.argtypes = [ctx, C.POINTER(A.me_mom_result)]
+    L.me_mom.argtypes = [ctx, C.c_int, C.c_double, C.c_int32, C.POINTER(A.me_mom_params), C.POINTER(A.me_mom_result)]
+    L.me_mom_axes.argtypes = [i64p, C.c_int32, C.c_double, dp, C.POINTER(C.c_int32)]
+    L.me_get_mom_points.argtypes = [ctx, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.me_kernel_trace.argtypes = [ctx, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.c_int32]
     if L.me_abi_version() != A.ME_ABI_VERSION:
         raise RuntimeError("libmapeval_b200.so ABI version mismatch")

@@ -211,6 +211,40 @@ def consistency_dict(rows, whole):
     return out
 
 
+def mom_dict(res):
+    """me_mom_result -> {field: value}; 'axis' (3, 3) rows a1 a2 a3, 'n' / 'mean' / 'median' (3,), 'status' its
+    ME_MOM_* name"""
+    out = {}
+    for f in A.me_mom_result._fields_:
+        if f[0] == "reserved":
+            continue
+        x = getattr(res, f[0])
+        out[f[0]] = np.array(x[:]) if isinstance(x, C.Array) else x
+    out["axis"] = out["axis"].reshape(3, 3)
+    out["status"] = A.MOM_STATUS_NAMES.get(res.status, str(res.status))
+    return out
+
+
+def mom_params(angle_deg=10.0, planarity=0.5, min_family=100):
+    return A.me_mom_params(float(angle_deg), float(planarity), int(min_family))
+
+
+def mom_axes(hist, angle_deg=10.0, cells_per_edge=A.ME_MOM_CELLS_PER_EDGE):
+    """me_mom_axes (host only): (axes (3, 3) rows a1 a2 a3, NaN where not found; status name) from an integer histogram
+    of 6 cells_per_edge^2 bins"""
+    L = _lib.load()
+    h = np.ascontiguousarray(hist, dtype=np.int64)
+    if h.shape != (6 * cells_per_edge * cells_per_edge,):
+        raise ValueError("the histogram needs 6 cells_per_edge^2 bins")
+    axes = np.zeros(9, np.float64)
+    st = C.c_int32(0)
+    rc = L.me_mom_axes(h.ctypes.data_as(C.POINTER(C.c_int64)), int(cells_per_edge), float(angle_deg),
+                       axes.ctypes.data_as(C.POINTER(C.c_double)), C.byref(st))
+    if rc != A.ME_OK:
+        raise MapEvalError(rc, "me_mom_axes: cells_per_edge in 1..1024, angle_deg in (0, 30], counts >= 0")
+    return axes.reshape(3, 3), A.MOM_STATUS_NAMES.get(st.value, str(st.value))
+
+
 def consistency_finalize(region_size, index, n_points, n_total, block):
     """me_consistency_finalize (host only): the rows of n regions and the whole-map result from a reduced host block
     (ME_CONSISTENCY_SUM_FIELDS SUM values per region, then ME_CONSISTENCY_MAX_FIELDS MAX values; one region, the whole map,
@@ -707,6 +741,51 @@ class MapEvalB200:
         self._check(self._L.me_get_consistency_points(self._ctx, int(which), e.ctypes.data_as(C.c_void_p),
                                                       v.ctypes.data_as(C.c_void_p)))
         return e, v
+
+    def mom(self, which, radius, min_neighbors=10, angle_deg=10.0, planarity=0.5, min_family=100):
+        """The mutually orthogonal metric of cloud `which` without a ground truth (me_mom, world 1): the plane thickness
+        (the median plane variance, m^2) of three mutually orthogonal plane families, summed.  Returns mom_dict's dict:
+        'mom' (NaN unless 'status' is 'OK'), 'axis' (3, 3), per family 'n' / 'mean' / 'median', the counts, and which sweep
+        ran.  The sweep may lay the cloud out again (its NN records are then stale).  Multi-GPU: dist.mom_distributed."""
+        out = A.me_mom_result()
+        p = mom_params(angle_deg, planarity, min_family)
+        self._check(self._L.me_mom(self._ctx, int(which), float(radius), int(min_neighbors), C.byref(p), C.byref(out)))
+        return mom_dict(out)
+
+    def mom_begin(self, which, radius, min_neighbors=10, angle_deg=10.0, planarity=0.5, min_family=100):
+        """me_mom_begin: sweeps this rank's query range and histograms its planar normals"""
+        p = mom_params(angle_deg, planarity, min_family)
+        self._check(self._L.me_mom_begin(self._ctx, int(which), float(radius), int(min_neighbors), C.byref(p)))
+
+    def mom_block(self):
+        """(device pointer, n) of the running pass's block: SUM-reduce it in place (after synchronize())"""
+        ptr = C.POINTER(C.c_double)()
+        n = C.c_int32(0)
+        self._check(self._L.me_mom_block(self._ctx, C.byref(ptr), C.byref(n)))
+        return C.cast(ptr, C.c_void_p).value, n.value
+
+    def mom_step(self):
+        """me_mom_step: reads the reduced block, runs the next pass; True after the last"""
+        done = C.c_int32(0)
+        self._check(self._L.me_mom_step(self._ctx, C.byref(done)))
+        return bool(done.value)
+
+    def mom_end(self):
+        out = A.me_mom_result()
+        self._check(self._L.me_mom_end(self._ctx, C.byref(out)))
+        return mom_dict(out)
+
+    def get_mom_points(self, which):
+        """(v, lambda2, normal (n, 3), family) per point of the last MOM call on cloud `which`, caller order: NaN / -1
+        where invalid and at points another rank evaluated; family 0..2 or -1"""
+        n = self.n[which]
+        v = np.zeros(n, np.float64)
+        l2 = np.zeros(n, np.float64)
+        nrm = np.zeros((n, 3), np.float64)
+        fam = np.zeros(n, np.int8)
+        self._check(self._L.me_get_mom_points(self._ctx, int(which), v.ctypes.data_as(C.c_void_p), l2.ctypes.data_as(C.c_void_p),
+                                              nrm.ctypes.data_as(C.c_void_p), fam.ctypes.data_as(C.c_void_p)))
+        return v, l2, nrm, fam
 
     def get_nn(self, which_query):
         n = self.n[which_query]

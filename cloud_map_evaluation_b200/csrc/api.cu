@@ -241,6 +241,7 @@ void me_destroy(me_ctx *ctx) {
   nn_region_free(ctx);
   nn_surface_free(ctx);
   consistency_free(ctx);
+  mom_free(ctx);
   drift_close(ctx, false);
   if (ctx->copy_stream) { cudaStreamSynchronize(ctx->copy_stream); cudaStreamDestroy(ctx->copy_stream); }
   if (ctx->compute_mark) cudaEventDestroy(ctx->compute_mark);
@@ -1190,6 +1191,58 @@ int me_get_consistency_points(me_ctx *ctx, int which, double *entropy, double *p
   ME_ENTER(ctx);
   if (!cloud_id(which)) return fail(ctx, ME_ERR_INVALID, "bad cloud id");
   return consistency_points(ctx, which, entropy, plane_variance);
+}
+
+static int mom_params_ok(me_ctx *ctx, const me_mom_params *p) {
+  if (!p) return fail(ctx, ME_ERR_INVALID, "null argument");
+  if (!(p->angle_deg > 0.0 && p->angle_deg <= 30.0)) return fail(ctx, ME_ERR_INVALID, "me_mom_begin: angle_deg must be in (0, 30]");
+  if (!(p->planarity > 0.0 && p->planarity <= 1.0)) return fail(ctx, ME_ERR_INVALID, "me_mom_begin: planarity must be in (0, 1]");
+  if (p->min_family < 1) return fail(ctx, ME_ERR_INVALID, "me_mom_begin: min_family must be >= 1");
+  return ME_OK;
+}
+
+int me_mom_begin(me_ctx *ctx, int which, double radius, int32_t min_neighbors, const me_mom_params *p) {
+  ME_ENTER(ctx);
+  ctx->mom.open = false;
+  if (!cloud_id(which)) return fail(ctx, ME_ERR_INVALID, "me_mom_begin: which must be ME_CLOUD_EST or ME_CLOUD_GT");
+  if (!(std::isfinite(radius) && radius > 0.0)) return fail(ctx, ME_ERR_INVALID, "me_mom_begin: radius must be finite and > 0");
+  if (min_neighbors < 3) return fail(ctx, ME_ERR_INVALID, "me_mom_begin: min_neighbors must be >= 3");
+  ME_TRY(mom_params_ok(ctx, p));
+  return mom_begin(ctx, which, radius, min_neighbors, p);
+}
+
+int me_mom_block(me_ctx *ctx, double **device_block, int32_t *n) {
+  ME_ENTER(ctx);
+  if (!device_block || !n) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return mom_block(ctx, device_block, n);
+}
+
+int me_mom_step(me_ctx *ctx, int32_t *done) {
+  ME_ENTER(ctx);
+  if (!done) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return mom_step(ctx, done);
+}
+
+int me_mom_end(me_ctx *ctx, me_mom_result *out) {
+  ME_ENTER(ctx);
+  if (!out) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return mom_end(ctx, out);
+}
+
+int me_mom(me_ctx *ctx, int which, double radius, int32_t min_neighbors, const me_mom_params *p, me_mom_result *out) {
+  ME_ENTER(ctx);
+  if (!out) return fail(ctx, ME_ERR_INVALID, "null argument");
+  if (ctx->world != 1) return fail(ctx, ME_ERR_INVALID, "me_mom needs world == 1; use me_mom_begin / _block + all-reduce / _step / _end");
+  ME_TRY(me_mom_begin(ctx, which, radius, min_neighbors, p));
+  int32_t done = 0;
+  while (!done) ME_TRY(me_mom_step(ctx, &done));
+  return me_mom_end(ctx, out);
+}
+
+int me_get_mom_points(me_ctx *ctx, int which, double *v, double *lambda2, double *normal, int8_t *family) {
+  ME_ENTER(ctx);
+  if (!cloud_id(which)) return fail(ctx, ME_ERR_INVALID, "bad cloud id");
+  return mom_points(ctx, which, v, lambda2, normal, family);
 }
 
 int me_drift_begin(me_ctx *ctx, double region_size, double max_correspondence_distance, int32_t max_iteration,

@@ -3,7 +3,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
+#include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <string>
 #include <vector>
 #include "../../include/mapeval_b200.h"
@@ -171,26 +173,115 @@ struct IcpRun {
   int it = 0, converged = 0;
 };
 
-// exact distance quantiles (me_nn_quantile_begin .. me_nn_quantile_end, nn.cu): radix selection over the NN records, the
-// same loop on every rank.  Slot s of a direction is one distinct prefix (the key bits the passes so far fixed) that some
-// target rank still lies under.
+// numpy's method="linear" position of probability p among n sorted values: h = (n - 1) p, k = floor(h), g = h - k
+inline void quantile_rank(long long n, double p, long long *k, double *g) {
+  const double h = (double)(n - 1) * p;
+  const double f = std::floor(h);
+  *k = (long long)f;
+  *g = h - f;
+}
+// numpy's _lerp in its operation order: lo + (hi - lo) g below g = 0.5, hi - (hi - lo) (1 - g) from there
+inline double quantile_lerp(double lo, double hi, double g) {
+  const double diff = hi - lo;
+  return g >= 0.5 ? hi - diff * (1.0 - g) : lo + diff * g;
+}
+
+// exact order statistics by radix selection over 64-bit keys (the bit patterns of finite doubles >= 0), the same loop on
+// every rank: pass j histograms digit j (8 bits, most significant first) of the keys under each slot's prefix; the host
+// reads the reduced counts and fixes digit j of every target rank.  Slot s of a population is one distinct prefix (the key
+// bits the passes so far fixed) that some target rank still lies under.  P populations are selected side by side: the two
+// directions of me_nn_quantile* (nn.cu), the three plane families of me_mom* (mom.cu).
 static constexpr int kQuantSlots = 2 * ME_QUANTILE_MAX_PROBS + 2;   // ranks k and k + 1 per probability, then 0 and n - 1
 static constexpr int kQuantBins = 256;                               // 8-bit digits
 static constexpr int kQuantPasses = 8;                               // 64-bit keys
 static constexpr int kQuantBlock = 2 * kQuantSlots * kQuantBins;     // fp64 counts per pass: [direction][slot][digit]
+template <int P, int Slots>
+struct RadixSel {
+  int pass = 0;                        // the digit the next reduced histogram holds
+  long long n[P] = {};                 // population sizes
+  int n_targets[P] = {};
+  long long rank[P][Slots];            // target ranks in the sorted population
+  long long resid[P][Slots];           // rank of the target among the keys under its prefix
+  unsigned long long key[P][Slots];    // the prefix of the target: the digits fixed so far, lower bits zero
+  int n_slots[P] = {};
+  unsigned long long slot_pfx[P][Slots];   // distinct prefixes of the running pass, ascending
+
+  // population q of nq keys (before pass 0): the target ranks k and k + 1 of numpy's linear quantile per probability p[0..K-1],
+  // then 0 and nq - 1; one slot, the empty prefix.  nq = 0: no targets, no slot
+  void set_targets(int q, long long nq, const double *p, int K) {
+    n[q] = nq;
+    n_targets[q] = 0;
+    n_slots[q] = 0;
+    if (nq <= 0) return;
+    int t = 0;
+    for (int k = 0; k < K; ++k) {
+      long long kk;
+      double g;
+      quantile_rank(nq, p[k], &kk, &g);
+      rank[q][t++] = kk;
+      rank[q][t++] = kk + 1 < nq - 1 ? kk + 1 : nq - 1;
+    }
+    rank[q][t++] = 0;
+    rank[q][t++] = nq - 1;
+    n_targets[q] = t;
+    for (int i = 0; i < t; ++i) { resid[q][i] = rank[q][i]; key[q][i] = 0; }
+    n_slots[q] = 1;
+    slot_pfx[q][0] = 0;
+  }
+  // digit `pass` of every target of population q from its reduced counts rows[slot * kQuantBins + digit]; false when a
+  // target's rank does not lie under the rows (a block not SUM-reduced over all ranks, or of another selection)
+  bool take_digits(int q, const double *rows) {
+    const int shift = 56 - 8 * pass;
+    for (int i = 0; i < n_targets[q]; ++i) {
+      const unsigned long long top = pass == 0 ? 0 : key[q][i] >> (shift + 8);
+      int s = 0;                       // first slot with prefix >= top
+      while (s < n_slots[q] && slot_pfx[q][s] < top) ++s;
+      if (s >= n_slots[q]) return false;
+      const double *row = rows + (size_t)s * kQuantBins;
+      long long below = 0;
+      int d = 0;
+      for (; d < kQuantBins; ++d) {
+        const long long c = (long long)row[d];
+        if (resid[q][i] < below + c) break;
+        below += c;
+      }
+      if (d == kQuantBins) return false;
+      resid[q][i] -= below;
+      key[q][i] |= (unsigned long long)d << shift;
+    }
+    return true;
+  }
+  // after the digits of every population: the distinct prefixes of the next pass, ascending
+  void next_pass() {
+    ++pass;
+    for (int q = 0; q < P; ++q) {
+      if (!n_slots[q]) continue;
+      unsigned long long *s = slot_pfx[q];
+      for (int i = 0; i < n_targets[q]; ++i) s[i] = key[q][i] >> (64 - 8 * pass);
+      std::sort(s, s + n_targets[q]);
+      n_slots[q] = (int)(std::unique(s, s + n_targets[q]) - s);
+    }
+  }
+  // the order statistic of rank r of population q once every pass ran, one of the targets (NaN otherwise)
+  double value(int q, long long r) const {
+    for (int i = 0; i < n_targets[q]; ++i)
+      if (rank[q][i] == r) {
+        double v;
+        std::memcpy(&v, &key[q][i], sizeof(v));
+        return v;
+      }
+    return (double)NAN;
+  }
+};
+
+// exact distance quantiles (me_nn_quantile_begin .. me_nn_quantile_end, nn.cu): radix selection over the NN records of
+// both directions
 struct QuantRun {
   bool open = false, done = false;
   unsigned long long gen = 0;          // cloud_gen at me_nn_quantile_begin
   int population = 0, K = 0, dirs = 0;
   double p[ME_QUANTILE_MAX_PROBS];
-  int pass = 0;                        // passes whose histogram the block holds / held (1 after begin)
-  long long n[2] = {0, 0};             // population sizes, from the reduced block of pass 0
-  int n_targets[2] = {0, 0};
-  long long rank[2][kQuantSlots];      // target ranks in the sorted population
-  long long resid[2][kQuantSlots];     // rank of the target among the keys under its prefix
-  unsigned long long key[2][kQuantSlots];   // the prefix of the target: the digits fixed so far, lower bits zero
-  int n_slots[2] = {0, 0};
-  unsigned long long slot_pfx[2][kQuantSlots];   // distinct prefixes of the running pass, ascending
+  RadixSel<2, kQuantSlots> sel;        // the targets of both directions; sel.pass: the digit the running pass histograms
   long long kb[2] = {0, 0}, ke[2] = {0, 0};      // the record range the keys cover
   unsigned long long *d_keys[2] = {nullptr, nullptr};
   long long cap_keys[2] = {0, 0};
@@ -198,6 +289,41 @@ struct QuantRun {
   double *d_blk = nullptr;                       // the same as fp64: the SUM-reducible block
   unsigned long long *d_pfx = nullptr;           // slot_pfx on the device
   std::vector<double> h_blk;
+};
+
+// the mutually orthogonal metric (me_mom_begin .. me_mom_end, mom.cu): the per-point values of the last call per cloud, the
+// loop state (the same on every rank) and the block, ME_MOM_BLOCK fp64 values in every pass
+static constexpr int kMomSlots = 4;     // ranks k and k + 1 of the median, then 0 and n - 1
+struct MomRun {
+  bool open = false, done = false;
+  unsigned long long gen = 0;          // cloud_gen at me_mom_begin
+  int which = 0, min_neighbors = 0, rings = 0, solo = 0;
+  double radius = 0.0, angle_deg = 0.0, planarity = 0.0, cos_a = 0.0;
+  long long min_family = 0;
+  int stage = 0;                       // what the block holds: 0 the direction histogram, 1 the fold and digit 0, 2.. digit stage - 1
+  long long n_query = 0, n_pv = 0, n_planar = 0;
+  int status = 0;
+  double axes[9];
+  long long n_fam[3] = {0, 0, 0};
+  double sum_v[3] = {0, 0, 0};
+  RadixSel<3, kMomSlots> sel;
+  long long keys_local[3] = {0, 0, 0};    // this rank's members per family: its keys, family by family, in d_keys
+  long long kb = 0, ke = 0;            // this rank's sorted query range
+  unsigned long long *d_hist = nullptr;   // ME_MOM_BLOCK integer counts, then the block as fp64, the slot prefixes, 3 counters
+  double *d_blk = nullptr;
+  unsigned long long *d_pfx = nullptr, *d_ctr = nullptr;
+  double *d_fold = nullptr;            // this rank's fold: n_j, sum_v_j
+  double *d_part = nullptr;            // the fold's per-chunk values
+  long long cap_part = 0;
+  unsigned long long *d_keys = nullptr;   // v of this rank's family members, family by family
+  long long cap_keys = 0;
+  std::vector<double> h_blk;
+  // per cloud, caller order: v, lambda2, the unit normal and a flag byte (1 evaluated, 2 v valid, 4 planar, family + 1 in bits 3..4)
+  double *d_v[2] = {nullptr, nullptr}, *d_l2[2] = {nullptr, nullptr}, *d_n[2] = {nullptr, nullptr};
+  uint8_t *d_flag[2] = {nullptr, nullptr};
+  long long cap_v[2] = {0, 0}, cap_l2[2] = {0, 0}, cap_n[2] = {0, 0}, cap_flag[2] = {0, 0};
+  bool pts_valid[2] = {false, false};
+  unsigned long long pts_gen[2] = {0, 0};
 };
 
 // the per-region table (me_nn_region_begin .. me_nn_region_end, region.cu): the occupied list and the block, the same
@@ -289,19 +415,6 @@ struct ConsistencyRun {
   unsigned long long pts_gen[2] = {0, 0};   // cloud_gen when they were computed
 };
 
-// numpy's method="linear" position of probability p among n sorted values: h = (n - 1) p, k = floor(h), g = h - k
-inline void quantile_rank(long long n, double p, long long *k, double *g) {
-  const double h = (double)(n - 1) * p;
-  const double f = std::floor(h);
-  *k = (long long)f;
-  *g = h - f;
-}
-// numpy's _lerp in its operation order: lo + (hi - lo) g below g = 0.5, hi - (hi - lo) (1 - g) from there
-inline double quantile_lerp(double lo, double hi, double g) {
-  const double diff = hi - lo;
-  return g >= 0.5 ? hi - diff * (1.0 - g) : lo + diff * g;
-}
-
 }  // namespace me
 
 struct me_ctx {
@@ -375,6 +488,7 @@ struct me_ctx {
   me::DriftRun drift;                  // the per-region drift loop (me_drift*)
   me::SurfaceRun surface;              // point-to-plane metrics (me_nn_surface*), from the NN records
   me::ConsistencyRun consistency;      // local map consistency (me_consistency*): MPV and MME per region
+  me::MomRun mom;                      // the mutually orthogonal metric (me_mom*)
   std::string err;
 };
 
@@ -516,6 +630,19 @@ int consistency_block(me_ctx *ctx, double **device_block, int32_t *n_sum, int32_
 int consistency_end(me_ctx *ctx, me_consistency_row *rows, int64_t capacity, me_consistency_result *whole);
 int consistency_points(me_ctx *ctx, int which, double *entropy, double *plane_variance);
 void consistency_free(me_ctx *ctx);
+struct RadiusSweep {
+  long long qb, qe;      // this rank's sorted query range
+  int rings;
+  float rc2;
+};
+int radius_sweep_layout(me_ctx *ctx, int which, double radius, const char *who, RadiusSweep *out);
+// the mutually orthogonal metric (me_mom_*, mom.cu; arguments checked by the caller)
+int mom_begin(me_ctx *ctx, int which, double radius, int min_neighbors, const me_mom_params *p);
+int mom_block(me_ctx *ctx, double **device_block, int32_t *n);
+int mom_step(me_ctx *ctx, int32_t *done);
+int mom_end(me_ctx *ctx, me_mom_result *out);
+int mom_points(me_ctx *ctx, int which, double *v, double *lambda2, double *normal, int8_t *family);
+void mom_free(me_ctx *ctx);
 
 // layout of me_ctx::d_block (fp64): the SUM-reducible part first, then the MAX-reducible part.  Counts ride as fp64 (exact
 // below 2^53, so their sums are exact and order-independent).

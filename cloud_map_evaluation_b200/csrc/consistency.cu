@@ -14,8 +14,7 @@
 // No floating-point atomics: two calls give the same bits as long as the cloud is not laid out again in between (a new
 // layout can order the points of a cell differently: grid.cu ranks them with atomics).
 #include "common.cuh"
-#include "eig3.cuh"
-#include "mme_walk.cuh"
+#include "plane.cuh"
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
@@ -34,36 +33,15 @@ struct PointOut {            // caller order
   uint8_t *flag;
 };
 
-// entropy and plane variance of one query from its moments.  The covariance and the entropy are finish_entropy's (mme.cu)
-// expressions, so e equals MME's bit for bit on the same moments.
+// entropy and plane variance of one query from its moments (plane_eig, shared with the mutually orthogonal metric's sweep)
 __device__ __forceinline__ void finish_point(const Moments &m, int min_neighbors, long long o, const PointOut &O) {
-  double e = 0.0, v = NAN;
+  PlaneEig P;
+  plane_eig(m, min_neighbors, P);
   uint8_t flag = kEvaluated;
-  const long long k = (long long)m.cnt - 1;                 // the query itself
-  if (m.cnt > 0 && k >= (long long)min_neighbors) {
-    const double kd = (double)k, inv = 1.0 / (double)(k - 1);
-    double c[9];
-    c[0] = (m.sxx - m.s1x * m.s1x / kd) * inv;
-    c[1] = (m.sxy - m.s1x * m.s1y / kd) * inv;
-    c[2] = (m.sxz - m.s1x * m.s1z / kd) * inv;
-    c[4] = (m.syy - m.s1y * m.s1y / kd) * inv;
-    c[5] = (m.syz - m.s1y * m.s1z / kd) * inv;
-    c[8] = (m.szz - m.s1z * m.s1z / kd) * inv;
-    c[3] = c[1]; c[6] = c[2]; c[7] = c[5];
-    const double det = det3(c);
-    const double ent = 0.5 * log(2 * M_PI * M_E * det);
-    if (!(isnan(ent) || isinf(ent))) { e = ent; flag |= kEntropyValid; }
-    double w[3], vec[9];
-    eig3_jacobi(c, w, vec);
-    double l = w[0];
-    if (w[1] < l) l = w[1];
-    if (w[2] < l) l = w[2];
-    if (isnan(w[0]) || isnan(w[1]) || isnan(w[2])) l = NAN;
-    v = l < 0.0 ? 0.0 : l;                                  // NaN stays NaN
-    if (isfinite(v)) flag |= kPvValid;
-  }
-  O.e[o] = e;
-  O.v[o] = v;
+  if (P.e_valid) flag |= kEntropyValid;
+  if (isfinite(P.v)) flag |= kPvValid;
+  O.e[o] = P.e;
+  O.v[o] = P.v;
   O.flag[o] = flag;
 }
 
@@ -198,11 +176,10 @@ void consistency_free(me_ctx *ctx) {
   K.open = false;
 }
 
-// the sweep of this rank's query range into the per-point arrays of cloud `which`
-static int consistency_sweep(me_ctx *ctx, int which, double radius, int min_neighbors) {
-  ConsistencyRun &K = ctx->consistency;
+// the lattice of a radius sweep of cloud `which` (MME's: the shared one, or the cloud's own with h = r / 2), this rank's
+// query range, and run_mme's ring count and row slack (the same rows and candidates as mme_kernel); shared with mom.cu
+int radius_sweep_layout(me_ctx *ctx, int which, double radius, const char *who, RadiusSweep *out) {
   Cloud &c = ctx->cloud[which];
-  K.pts_valid[which] = false;
   bool solo = false;
   ME_TRY(radius_lattice(ctx, which, radius, &solo));
   const double solo_h = solo ? 0.5 * radius : 0.0;
@@ -215,8 +192,25 @@ static int consistency_sweep(me_ctx *ctx, int which, double radius, int min_neig
     c.entropy_caller_valid = true;
   }
   ME_TRY(build_grid(ctx, which, solo_h));
-  long long qb, qe;
-  ME_TRY(query_shard(ctx, which, &qb, &qe));
+  ME_TRY(query_shard(ctx, which, &out->qb, &out->qe));
+  const double rings_f = std::max(1.0, std::ceil(radius / c.lat.h - 1e-9));
+  if (rings_f > 1.0e6) return fail(ctx, ME_ERR_RANGE, std::string(who) + ": radius spans too many lattice cells");
+  out->rings = (int)rings_f;
+  const double rc = radius / c.lat.h;
+  out->rc2 = (float)(rc * rc * (1.0 + 1e-5) + 1e-4);
+  return ME_OK;
+}
+
+// the sweep of this rank's query range into the per-point arrays of cloud `which`
+static int consistency_sweep(me_ctx *ctx, int which, double radius, int min_neighbors) {
+  ConsistencyRun &K = ctx->consistency;
+  Cloud &c = ctx->cloud[which];
+  K.pts_valid[which] = false;
+  RadiusSweep RS;
+  ME_TRY(radius_sweep_layout(ctx, which, radius, "me_consistency_begin", &RS));
+  const long long qb = RS.qb, qe = RS.qe;
+  const int rings = RS.rings;
+  const float rc2 = RS.rc2;
   ME_TRY(ensure(ctx, (void **)&K.d_e[which], &K.cap_e[which], c.n, sizeof(double)));
   ME_TRY(ensure(ctx, (void **)&K.d_v[which], &K.cap_v[which], c.n, sizeof(double)));
   ME_TRY(ensure(ctx, (void **)&K.d_flag[which], &K.cap_flag[which], c.n, sizeof(uint8_t)));
@@ -226,12 +220,6 @@ static int consistency_sweep(me_ctx *ctx, int which, double radius, int min_neig
     consistency_init_kernel<<<blocks, kThreads, 0, ctx->stream>>>(c.n, O.e, O.v, O.flag);
     ME_LAUNCH_CHECK(ctx);
   }
-  // run_mme's ring count and row slack (the same rows and candidates as mme_kernel)
-  const double rings_f = std::max(1.0, std::ceil(radius / c.lat.h - 1e-9));
-  if (rings_f > 1.0e6) return fail(ctx, ME_ERR_RANGE, "me_consistency_begin: radius spans too many lattice cells");
-  const int rings = (int)rings_f;
-  const double rc = radius / c.lat.h;
-  const float rc2 = (float)(rc * rc * (1.0 + 1e-5) + 1e-4);
   K.rings = rings;
   K.solo = c.grid_solo ? 1 : 0;
   K.kernel = ME_CONSISTENCY_WALK;

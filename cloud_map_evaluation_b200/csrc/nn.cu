@@ -21,6 +21,7 @@
 #include "records.cuh"
 #include "tile.cuh"
 #include "flat.cuh"
+#include "radix.cuh"
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -950,17 +951,10 @@ __global__ void nn_curve_merge_kernel(const double *__restrict__ part, int n_blo
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Exact distance quantiles (me_nn_quantile_*): radix selection over the records.  Pass 0 turns every record of a
-// direction into a 64-bit key — the bit pattern of its d, which for a finite d >= 0 sorts as an unsigned integer, or
-// kQuantOut outside the population — and histograms the top 8-bit digit.  Pass j histograms digit j of the keys under
-// each slot's prefix (the top 8j bits some target rank still lies under).  Prefixes of one length are disjoint, so a key
-// falls under at most one slot, found by binary search over the ascending prefixes.  Counts only: per block a shared
-// integer histogram (warp-aggregated), merged into the global one with integer atomics — the result does not depend on
-// the order of the additions.
+// Exact distance quantiles (me_nn_quantile_*): radix selection over the records (radix.cuh).  Pass 0 turns every record of
+// a direction into a 64-bit key — the bit pattern of its d, or kQuantOut outside the population — and histograms the top
+// 8-bit digit; the later passes are nn_quantile_hist_kernel's.
 // ---------------------------------------------------------------------------------------------------------------
-static constexpr int kQuantThreads = 512;
-static constexpr unsigned long long kQuantOut = ~0ull;     // not in the population (no finite d >= 0 has the sign bit)
-
 // d of record i of the population, false when the record is not in it
 __device__ __forceinline__ bool quant_record(const CurveSrc &S, const NNConst &C, int nn_pop, long long i, double &d) {
   if (nn_pop) {            // the terms of nn_stats_kernel's full-CD sum
@@ -973,19 +967,6 @@ __device__ __forceinline__ bool quant_record(const CurveSrc &S, const NNConst &C
   if (!kept_record(S, C, i, sq, ub)) return false;
   d = pair_dist(sq);
   return true;
-}
-
-// one count into s_hist[bin] (bin < 0: none), the lanes of a warp with the same bin added by one atomic; the whole warp calls
-__device__ __forceinline__ void quant_count(unsigned int *s_hist, int bin) {
-  const unsigned int peers = __match_any_sync(0xffffffffu, bin);
-  if (bin >= 0 && (threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(s_hist + bin, (unsigned int)__popc(peers));
-}
-
-// the block's histogram of nbins bins, added into hist
-__device__ __forceinline__ void quant_flush(const unsigned int *s_hist, int nbins, unsigned long long *__restrict__ hist) {
-  __syncthreads();
-  for (int t = threadIdx.x; t < nbins; t += blockDim.x)
-    if (s_hist[t]) atomicAdd(hist + t, (unsigned long long)s_hist[t]);
 }
 
 // pass 0: keys[i - S.b] for every record of [S.b, S.e), and the histogram of the top digit into hist[0 .. 255]
@@ -1002,7 +983,7 @@ nn_quantile_keys_kernel(CurveSrc S, NNConst C, int nn_pop, unsigned long long *_
       double d;
       unsigned long long key = kQuantOut;
       if (quant_record(S, C, nn_pop, i, d)) {
-        key = (unsigned long long)__double_as_longlong(d == 0.0 ? 0.0 : d);     // -0 sorts with +0
+        key = quant_key(d);
         bin = (int)(key >> 56);
       }
       keys[i - S.b] = key;
@@ -1010,37 +991,6 @@ nn_quantile_keys_kernel(CurveSrc S, NNConst C, int nn_pop, unsigned long long *_
     quant_count(s_hist, bin);
   }
   quant_flush(s_hist, kQuantBins, hist);
-}
-
-// pass j >= 1 (shift = 56 - 8j): per key under the prefix of slot s (pfx[s] = its top 8j bits, ascending), one count into
-// hist[s * 256 + digit j]
-__global__ void __launch_bounds__(kQuantThreads)
-nn_quantile_hist_kernel(const unsigned long long *__restrict__ keys, long long n, int shift, const unsigned long long *__restrict__ pfx,
-                        int n_slots, unsigned long long *__restrict__ hist) {
-  extern __shared__ unsigned int s_hist_dyn[];        // n_slots * 256
-  __shared__ unsigned long long s_pfx[kQuantSlots];
-  for (int t = threadIdx.x; t < n_slots * kQuantBins; t += kQuantThreads) s_hist_dyn[t] = 0;
-  for (int t = threadIdx.x; t < n_slots; t += kQuantThreads) s_pfx[t] = pfx[t];
-  __syncthreads();
-  const long long stride = (long long)gridDim.x * kQuantThreads;
-  for (long long base = (long long)blockIdx.x * kQuantThreads; base < n; base += stride) {
-    const long long i = base + threadIdx.x;
-    int bin = -1;
-    if (i < n) {
-      const unsigned long long key = __ldg(keys + i);
-      if (key != kQuantOut) {
-        const unsigned long long top = key >> (shift + 8);
-        int lo = 0, hi = n_slots;          // first slot with prefix >= top
-        while (lo < hi) {
-          const int mid = (lo + hi) >> 1;
-          if (s_pfx[mid] < top) lo = mid + 1; else hi = mid;
-        }
-        if (lo < n_slots && s_pfx[lo] == top) bin = lo * kQuantBins + (int)((key >> shift) & 0xffu);
-      }
-    }
-    quant_count(s_hist_dyn, bin);
-  }
-  quant_flush(s_hist_dyn, n_slots * kQuantBins, hist);
 }
 
 __global__ void quant_to_block_kernel(const unsigned long long *__restrict__ hist, int n, double *__restrict__ blk) {
@@ -1346,34 +1296,27 @@ void nn_quantile_free(me_ctx *ctx) {
   R.open = false;
 }
 
-// launch pass R.pass of every direction: pass 0 writes the keys, the later ones read them under the slots' prefixes
+// launch pass R.sel.pass of every direction: pass 0 writes the keys, the later ones read them under the slots' prefixes
 static int quant_launch(me_ctx *ctx) {
   QuantRun &R = ctx->quant;
   ME_CUDA(ctx, cudaMemsetAsync(R.d_hist, 0, (size_t)kQuantBlock * sizeof(unsigned long long), ctx->stream));
-  if (R.pass > 0)
-    ME_CUDA(ctx, cudaMemcpyAsync(R.d_pfx, R.slot_pfx, sizeof(R.slot_pfx), cudaMemcpyHostToDevice, ctx->stream));
+  if (R.sel.pass > 0)
+    ME_CUDA(ctx, cudaMemcpyAsync(R.d_pfx, R.sel.slot_pfx, sizeof(R.sel.slot_pfx), cudaMemcpyHostToDevice, ctx->stream));
   for (int q = 0; q < 2; ++q) {
     const long long n = R.ke[q] - R.kb[q];
-    if (n <= 0 || R.n_slots[q] == 0) continue;
+    if (n <= 0 || R.sel.n_slots[q] == 0) continue;
     unsigned long long *hist = R.d_hist + (size_t)q * kQuantSlots * kQuantBins;
-    if (R.pass == 0) {
+    if (R.sel.pass == 0) {
       NNConst C{};
       set_cutoff(C, &ctx->curve_p);
       CurveSrc S = record_src(ctx, q);
       S.b = R.kb[q]; S.e = R.ke[q];
       const int grid = (int)std::min<long long>((n + kQuantThreads - 1) / kQuantThreads, (long long)ctx->sm_count * 4);
       nn_quantile_keys_kernel<<<grid, kQuantThreads, 0, ctx->stream>>>(S, C, R.population == ME_DIST_NN, R.d_keys[q], hist);
+      ME_LAUNCH_CHECK(ctx);
     } else {
-      const size_t smem = (size_t)R.n_slots[q] * kQuantBins * sizeof(unsigned int);
-      ME_CUDA(ctx, cudaFuncSetAttribute(nn_quantile_hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)(kQuantSlots * kQuantBins * sizeof(unsigned int))));
-      int per_sm = 0;
-      ME_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nn_quantile_hist_kernel, kQuantThreads, smem));
-      const int grid = (int)std::min<long long>((n + kQuantThreads - 1) / kQuantThreads, (long long)ctx->sm_count * std::max(per_sm, 1));
-      nn_quantile_hist_kernel<<<grid, kQuantThreads, smem, ctx->stream>>>(R.d_keys[q], n, 56 - 8 * R.pass, R.d_pfx + q * kQuantSlots,
-                                                                         R.n_slots[q], hist);
+      ME_TRY(quant_hist_launch(ctx, R.d_keys[q], n, R.sel.pass, R.d_pfx + q * kQuantSlots, R.sel.n_slots[q], hist));
     }
-    ME_LAUNCH_CHECK(ctx);
   }
   quant_to_block_kernel<<<(kQuantBlock + 255) / 256, 256, 0, ctx->stream>>>(R.d_hist, kQuantBlock, R.d_blk);
   ME_LAUNCH_CHECK(ctx);
@@ -1393,26 +1336,24 @@ int nn_quantile_begin(me_ctx *ctx, int population, const double *p, int K) {
   R.dirs = ctx->curve_p.directions ? ctx->curve_p.directions : 3;
   R.gen = ctx->cloud_gen;
   R.done = false;
-  R.pass = 0;
+  R.sel.pass = 0;
   if (!R.d_hist) {      // the integer histogram, its fp64 block and the slot prefixes in one allocation
-    const size_t bytes = (size_t)kQuantBlock * (sizeof(unsigned long long) + sizeof(double)) + sizeof(R.slot_pfx);
+    const size_t bytes = (size_t)kQuantBlock * (sizeof(unsigned long long) + sizeof(double)) + sizeof(R.sel.slot_pfx);
     ME_CUDA(ctx, cudaMalloc((void **)&R.d_hist, bytes));
     R.d_blk = (double *)(R.d_hist + kQuantBlock);
     R.d_pfx = (unsigned long long *)(R.d_blk + kQuantBlock);
   }
   for (int q = 0; q < 2; ++q) {
-    R.n[q] = 0;
-    R.n_targets[q] = 0;
+    R.sel.set_targets(q, 0, R.p, R.K);
     R.kb[q] = R.ke[q] = 0;
-    R.n_slots[q] = 0;
     if (!(R.dirs & (1 << q))) continue;
     const CurveSrc S = record_src(ctx, q);
     const Cloud &Qc = ctx->cloud[q];
     R.kb[q] = population == ME_DIST_NN ? Qc.nn_b : S.b;      // ME_DIST_NN: the range of the full-CD sum
     R.ke[q] = std::max(R.kb[q], population == ME_DIST_NN ? Qc.nn_e : S.e);
     ME_TRY(ensure(ctx, (void **)&R.d_keys[q], &R.cap_keys[q], R.ke[q] - R.kb[q], sizeof(unsigned long long)));
-    R.n_slots[q] = 1;      // pass 0: the empty prefix
-    R.slot_pfx[q][0] = 0;
+    R.sel.n_slots[q] = 1;      // pass 0: the empty prefix
+    R.sel.slot_pfx[q][0] = 0;
   }
   ME_TRY(quant_launch(ctx));
   R.open = true;
@@ -1440,70 +1381,35 @@ int nn_quantile_block(me_ctx *ctx, double **device_block, int32_t *n) {
 int nn_quantile_step(me_ctx *ctx, int32_t *done) {
   ME_TRY(quant_ready(ctx, "me_nn_quantile_step"));
   QuantRun &R = ctx->quant;
+  auto &T = R.sel;
   if (R.done) { *done = 1; return ME_OK; }
-  // the reduced block of pass R.pass: only the rows of the slots in use are read
+  // the reduced block of pass T.pass: only the rows of the slots in use are read
   R.h_blk.resize(kQuantBlock);
   for (int q = 0; q < 2; ++q)
-    if (R.n_slots[q])
+    if (T.n_slots[q])
       ME_CUDA(ctx, cudaMemcpyAsync(R.h_blk.data() + (size_t)q * kQuantSlots * kQuantBins, R.d_blk + (size_t)q * kQuantSlots * kQuantBins,
-                                   (size_t)R.n_slots[q] * kQuantBins * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+                                   (size_t)T.n_slots[q] * kQuantBins * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  const int shift = 56 - 8 * R.pass;            // digit R.pass of a key
   for (int q = 0; q < 2; ++q) {
-    if (!R.n_slots[q]) continue;
+    if (!T.n_slots[q]) continue;
     const double *rows = R.h_blk.data() + (size_t)q * kQuantSlots * kQuantBins;
-    if (R.pass == 0) {      // the population size, then the target ranks: k and k + 1 per probability, 0 and n - 1
+    if (T.pass == 0) {      // the population size, then the target ranks: k and k + 1 per probability, 0 and n - 1
       double n = 0;
       for (int b = 0; b < kQuantBins; ++b) n += rows[b];
-      R.n[q] = (long long)n;
-      if (R.n[q] > 0) {
-        int t = 0;
-        for (int k = 0; k < R.K; ++k) {
-          long long kk;
-          double g;
-          quantile_rank(R.n[q], R.p[k], &kk, &g);
-          R.rank[q][t++] = kk;
-          R.rank[q][t++] = std::min(kk + 1, R.n[q] - 1);
-        }
-        R.rank[q][t++] = 0;
-        R.rank[q][t++] = R.n[q] - 1;
-        R.n_targets[q] = t;
-        for (int i = 0; i < t; ++i) { R.resid[q][i] = R.rank[q][i]; R.key[q][i] = 0; }
-      }
+      T.set_targets(q, (long long)n, R.p, R.K);
     }
-    for (int i = 0; i < R.n_targets[q]; ++i) {      // the digit of each target and its rank below that digit
-      const unsigned long long top = R.pass == 0 ? 0 : R.key[q][i] >> (shift + 8);
-      const int s = (int)(std::lower_bound(R.slot_pfx[q], R.slot_pfx[q] + R.n_slots[q], top) - R.slot_pfx[q]);
-      const double *row = rows + (size_t)s * kQuantBins;
-      long long below = 0;
-      int d = 0;
-      for (; d < kQuantBins; ++d) {
-        const long long c = (long long)row[d];
-        if (R.resid[q][i] < below + c) break;
-        below += c;
-      }
-      if (s >= R.n_slots[q] || d == kQuantBins) {
-        R.open = false;
-        return fail(ctx, ME_ERR_INVALID, "me_nn_quantile_step: the block does not hold a rank the selection needs (a block not "
-                                         "SUM-reduced over all ranks, or of another selection)");
-      }
-      R.resid[q][i] -= below;
-      R.key[q][i] |= (unsigned long long)d << shift;
+    if (!T.take_digits(q, rows)) {
+      R.open = false;
+      return fail(ctx, ME_ERR_INVALID, "me_nn_quantile_step: the block does not hold a rank the selection needs (a block not "
+                                       "SUM-reduced over all ranks, or of another selection)");
     }
   }
-  if (R.pass == kQuantPasses - 1) {
+  if (T.pass == kQuantPasses - 1) {
     R.done = true;
     *done = 1;
     return ME_OK;
   }
-  ++R.pass;
-  for (int q = 0; q < 2; ++q) {      // the distinct prefixes of the next pass, ascending
-    if (!R.n_slots[q]) continue;
-    unsigned long long *s = R.slot_pfx[q];
-    for (int i = 0; i < R.n_targets[q]; ++i) s[i] = R.key[q][i] >> (64 - 8 * R.pass);
-    std::sort(s, s + R.n_targets[q]);
-    R.n_slots[q] = (int)(std::unique(s, s + R.n_targets[q]) - s);
-  }
+  T.next_pass();
   ME_TRY(quant_launch(ctx));
   *done = 0;
   return ME_OK;
@@ -1520,16 +1426,8 @@ int nn_quantile_end(me_ctx *ctx, me_quantile_result *out) {
   for (int k = 0; k < R.K; ++k) out->p[k] = R.p[k];
   for (int q = 0; q < 2; ++q) {
     me_quantile_dir &D = q == 0 ? out->est_to_gt : out->gt_to_est;
-    D.n = R.n[q];
-    auto x = [&](long long r) {      // the order statistic of rank r, one of the targets
-      for (int i = 0; i < R.n_targets[q]; ++i)
-        if (R.rank[q][i] == r) {
-          double v;
-          std::memcpy(&v, &R.key[q][i], sizeof(v));
-          return v;
-        }
-      return (double)NAN;
-    };
+    D.n = R.sel.n[q];
+    auto x = [&](long long r) { return R.sel.value(q, r); };      // the order statistic of rank r, one of the targets
     D.min = D.n > 0 ? x(0) : NAN;
     D.max = D.n > 0 ? x(D.n - 1) : NAN;
     for (int k = 0; k < R.K; ++k) {

@@ -110,6 +110,26 @@ def consistency_distributed(ctx, device, which, radius, min_neighbors=10, region
     return ctx.consistency_end(n)
 
 
+def mom_distributed(ctx, device, which, radius, min_neighbors=10, angle_deg=10.0, planarity=0.5, min_family=100, group=None):
+    """The mutually orthogonal metric over every rank of the job (MapEvalB200.mom for world > 1): every rank sweeps its
+    query range of the replicated cloud, then ONE in-place SUM all-reduce per pass: the direction histogram, the family
+    fold with the medians' first digit, then the selection's later digits (counts ride as fp64, exact).  Every rank
+    returns the same result."""
+    import torch
+    import torch.distributed as dist
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    ctx.mom_begin(which, radius, min_neighbors, angle_deg, planarity, min_family)
+    done = False
+    while not done:
+        if world > 1:
+            ptr, n = ctx.mom_block()
+            ctx.synchronize()
+            dist.all_reduce(torch.as_tensor(_DeviceBlock(ptr, n), device=device), group=group)
+            torch.cuda.current_stream(device).synchronize()
+        done = ctx.mom_step()
+    return ctx.mom_end()
+
+
 def quantiles_distributed(ctx, device, p, population=A.ME_DIST_KEPT, group=None):
     """Exact distance quantiles of the last NN evaluation over every rank of the job (MapEvalB200.distance_quantiles for
     world > 1): the selection loop with ONE in-place SUM all-reduce of the pass's integer counts (as fp64, exact) per pass.

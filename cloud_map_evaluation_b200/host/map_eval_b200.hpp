@@ -109,6 +109,13 @@ struct Param {   // map_eval.h:60-116
   // floor(x / consistency_region_size) (0 = whole map only), written to map_consistency.txt (me_consistency*)
   bool evaluate_consistency_ = false;
   double consistency_region_size_ = 0.0;
+  // the mutually orthogonal metric without a ground truth (me_mom*, r = nn_radius; est with min_neighbors 10, gt with 5 when
+  // evaluate_gt_mme), written to map_mom.txt
+  bool evaluate_mom_ = false;
+  double mom_angle_deg_ = 10.0, mom_planarity_ = 0.5;
+  int64_t mom_min_family_ = 100;
+  // the estimate alone: gt_map_path is neither read nor required; MME, local consistency and MOM run on the est cloud
+  bool evaluate_without_gt_ = false;
 };
 
 // map_eval_main.cpp:120-208
@@ -134,7 +141,9 @@ inline Param loadParametersFromYAML(const std::string &yaml_file_path) {
     param.vmd_voxel_size_ = config["vmd_voxel_size"].as<double>();
     param.downsample_size = config["downsample_size"].as<double>();
     param.evaluation_map_pcd_path_ = config["estimate_map_path"].as<std::string>();
-    param.map_gt_path_ = config["gt_map_path"].as<std::string>();
+    if (config["evaluate_without_gt"]) param.evaluate_without_gt_ = config["evaluate_without_gt"].as<bool>();
+    if (!param.evaluate_without_gt_ || config["gt_map_path"]) param.map_gt_path_ = config["gt_map_path"].as<std::string>();
+    else param.map_gt_path_.clear();
     param.name_ = config["scene_name"].as<std::string>();
     if (!param.evaluation_map_pcd_path_.empty() && param.evaluation_map_pcd_path_.back() != '/')
       param.evaluation_map_pcd_path_ += '/';
@@ -198,6 +207,23 @@ inline Param loadParametersFromYAML(const std::string &yaml_file_path) {
         throw std::runtime_error("consistency_region_size must be finite and >= 0 (0 = the whole map only), not " +
                                  config["consistency_region_size"].as<std::string>());
     }
+    if (config["evaluate_mom"]) param.evaluate_mom_ = config["evaluate_mom"].as<bool>();
+    if (config["mom_angle_deg"]) {
+      param.mom_angle_deg_ = config["mom_angle_deg"].as<double>();
+      if (!(param.mom_angle_deg_ > 0.0 && param.mom_angle_deg_ <= 30.0))
+        throw std::runtime_error("mom_angle_deg must be in (0, 30], not " + config["mom_angle_deg"].as<std::string>());
+    }
+    if (config["mom_planarity"]) {
+      param.mom_planarity_ = config["mom_planarity"].as<double>();
+      if (!(param.mom_planarity_ > 0.0 && param.mom_planarity_ <= 1.0))
+        throw std::runtime_error("mom_planarity must be in (0, 1], not " + config["mom_planarity"].as<std::string>());
+    }
+    if (config["mom_min_family"]) {
+      const double mf = config["mom_min_family"].as<double>();
+      if (!(mf >= 1.0 && mf <= 9.0e18 && mf == std::floor(mf)))
+        throw std::runtime_error("mom_min_family must be an integer >= 1, not " + config["mom_min_family"].as<std::string>());
+      param.mom_min_family_ = (int64_t)mf;
+    }
     return param;
   } catch (const std::exception &e) {
     std::cerr << "Error loading parameters: " << e.what() << std::endl;
@@ -230,7 +256,9 @@ inline void dumpParam(const Param &p, std::ostream &os) {
   for (size_t i = 0; i < p.distance_quantiles_.size(); ++i) os << (i ? "," : "") << p.distance_quantiles_[i];
   os << "\nregion_size=" << p.region_size_ << "\ndrift_region_size=" << p.drift_region_size_ << "\nsurface_metrics=" << p.surface_metrics_
      << "\nsurface_normals_knn=" << p.surface_normals_knn_ << "\nevaluate_consistency=" << p.evaluate_consistency_
-     << "\nconsistency_region_size=" << p.consistency_region_size_ << "\n";
+     << "\nconsistency_region_size=" << p.consistency_region_size_ << "\nevaluate_mom=" << p.evaluate_mom_
+     << "\nmom_angle_deg=" << p.mom_angle_deg_ << "\nmom_planarity=" << p.mom_planarity_ << "\nmom_min_family=" << p.mom_min_family_
+     << "\nevaluate_without_gt=" << p.evaluate_without_gt_ << "\n";
 }
 
 // Eigen's default IOFormat for `vec.transpose()`: coefficients right-aligned to a common width, one space apart
@@ -303,6 +331,24 @@ class MapEvalB200 {
         *why = "distance_quantiles: every probability must be finite and in [0, 1]";
         return false;
       }
+    if (p.evaluate_without_gt_) {      // the keys that need a ground truth
+      const char *key = p.evaluate_noised_gt_ ? "evaluate_noised_gt"
+                        : p.global_registration_ ? "global_registration"
+                        : p.accuracy_curve_steps_ > 0 ? "accuracy_curve_steps"
+                        : !p.distance_quantiles_.empty() ? "distance_quantiles"
+                        : p.region_size_ > 0.0 ? "region_size"
+                        : p.drift_region_size_ > 0.0 ? "drift_region_size"
+                        : p.surface_metrics_ ? "surface_metrics" : nullptr;
+      if (key) {
+        *why = std::string(key) + " needs a ground truth; evaluate_without_gt evaluates the estimate alone";
+        return false;
+      }
+      if (!p.evaluate_mme_ && !p.evaluate_consistency_ && !p.evaluate_mom_) {
+        *why = "evaluate_without_gt: nothing to do (evaluate_mme, evaluate_consistency and evaluate_mom are all off)";
+        return false;
+      }
+      return true;
+    }
     if (p.evaluate_using_initial_) return true;
     if (p.evaluation_method_ < 0 || p.evaluation_method_ > 2) {
       *why = "Invalid registration type specified (registration_methods: " + std::to_string(p.evaluation_method_) +
@@ -375,6 +421,9 @@ class MapEvalB200 {
   int regionErrors();
   int surfaceMetrics();
   int localConsistency();
+  int mom();
+  int processWithoutGt();
+  bool gt_mme() const { return param_.evaluate_gt_mme_ && !param_.evaluate_without_gt_; }
   int regionDrift();
   GpuGroup gpus_;            // one context per GPU; rank r evaluates the r-th shard of every sweep's query range
   me_ctx *ctx_ = nullptr;    // = gpus_.ctx(0): the voxel stage and the single-GPU calls
@@ -394,6 +443,7 @@ inline int MapEvalB200::process() {
     std::cerr << "ERROR: " << err << std::endl;
     return -1;
   }
+  if (param_.evaluate_without_gt_) return processWithoutGt();
   // point-to-plane ICP needs normals on the target cloud, which can only come from the ground-truth file; generalized ICP
   // uses the normals of either file when it carries them (InitializePointCloudForGeneralizedICP); the surface metrics use them
   // on either path
@@ -484,6 +534,7 @@ inline int MapEvalB200::process() {
   if (param_.enable_debug) std::cout << "INFO: VMD calculation completed." << std::endl;
   // after every consumer of the pass's NN records (the sweep may lay a cloud out again), with the estimate in its final frame
   if (param_.evaluate_consistency_ && localConsistency() != 0) return -1;
+  if (param_.evaluate_mom_ && mom() != 0) return -1;
   if (param_.save_immediate_result_) {
     if (param_.enable_debug) std::cout << "INFO: Saving registration results..." << std::endl;
     saveRegistrationResults();
@@ -622,7 +673,7 @@ inline int MapEvalB200::computeMME() {
   if (mme_est_res_.n_valid * 100.0 / (double)mme_est_res_.n_total < 0.6)
     std::cerr << "valid points is too small, please check the input point cloud" << std::endl;   // :1732
   min_abs_entropy = mme_est_res_.min_abs_entropy; max_abs_entropy = mme_est_res_.max_abs_entropy;   // :179 -> :700-701
-  if (param_.evaluate_gt_mme_) {
+  if (gt_mme()) {
     if (eval_mme(ME_CLOUD_GT, 5, n_gt_, &mme_gt_res_) != 0) return fail("me_eval_mme(gt)");
     if (param_.save_immediate_result_ && renderEntropy(ME_CLOUD_GT, n_gt_, &gt_3d_entropy_) != 0) return -1;      // :181
     mme_gt = mme_gt_res_.mme;
@@ -832,7 +883,7 @@ inline int MapEvalB200::localConsistency() {
   };
   std::vector<Run> runs;
   runs.push_back(Run{ME_CLOUD_EST, 10, "est", me_consistency_result{}, {}});
-  if (param_.evaluate_gt_mme_) runs.push_back(Run{ME_CLOUD_GT, 5, "gt", me_consistency_result{}, {}});
+  if (gt_mme()) runs.push_back(Run{ME_CLOUD_GT, 5, "gt", me_consistency_result{}, {}});
   for (Run &run : runs) {
     std::vector<int64_t> n(gpus_.size(), 0);
     std::vector<double *> ptr(gpus_.size(), nullptr), ptr_max(gpus_.size(), nullptr);
@@ -858,7 +909,8 @@ inline int MapEvalB200::localConsistency() {
   f << std::setprecision(17) << "# local consistency without a ground truth: per point MME's neighbourhood (d2 < r^2), its entropy "
        "and its plane variance (smallest eigenvalue of the covariance, m^2); r = " << r << ", min_neighbors est 10";
   if (runs.size() > 1) f << ", gt 5";
-  f << ", region_size " << s << (s > 0.0 ? "" : " (whole map only)") << "; est in the ground truth's frame\n";
+  f << ", region_size " << s << (s > 0.0 ? "" : " (whole map only)")
+    << (param_.evaluate_without_gt_ ? "; est as loaded\n" : "; est in the ground truth's frame\n");
   const char *stats = "n_query n_valid n_pv mme mpv mean_plane_std max_pv";
   f << "cloud n_points " << stats << "\n" << std::fixed << std::setprecision(15);
   auto put = [&](int64_t n_points, int64_t nq, int64_t nv, int64_t np, double mme, double mpv, double sd, double mx) {
@@ -881,6 +933,106 @@ inline int MapEvalB200::localConsistency() {
   for (size_t i = 0; i < runs.size(); ++i)
     std::cout << (i ? "," : "") << " " << runs[i].name << " MPV " << runs[i].whole.mpv << " m^2, MME " << runs[i].whole.mme;
   std::cout << "; saved to " << path << std::endl;
+  return 0;
+}
+
+// the mutually orthogonal metric: the me_mom_* loop on every GPU for the est cloud (and the gt cloud with evaluate_gt_mme), one
+// grouped NCCL SUM all-reduce of the block per pass -> map_mom.txt next to map_results.txt
+inline int MapEvalB200::mom() {
+  const double r = param_.nn_radius_;
+  const me_mom_params p{param_.mom_angle_deg_, param_.mom_planarity_, param_.mom_min_family_};
+  struct Run {
+    int which, m;
+    const char *name;
+    me_mom_result res;
+  };
+  std::vector<Run> runs;
+  runs.push_back(Run{ME_CLOUD_EST, 10, "est", me_mom_result{}});
+  if (gt_mme()) runs.push_back(Run{ME_CLOUD_GT, 5, "gt", me_mom_result{}});
+  for (Run &run : runs) {
+    std::vector<double *> ptr(gpus_.size(), nullptr);
+    std::vector<int32_t> n(gpus_.size(), 0), done(gpus_.size(), 0);
+    if (gpus_.for_each([&](int, me_ctx *c) { return me_mom_begin(c, run.which, r, run.m, &p); }) != ME_OK) return fail("me_mom_begin");
+    while (!done[0]) {
+      if (gpus_.for_each([&](int g, me_ctx *c) {
+            const int rc = me_mom_block(c, &ptr[g], &n[g]);
+            return rc != ME_OK ? rc : me_synchronize(c);
+          }) != ME_OK)
+        return fail("me_mom_block");
+      if (!gpus_.allreduce_device(ptr, (size_t)n[0], ncclSum)) return fail("all-reduce of the MOM block");
+      if (gpus_.for_each([&](int g, me_ctx *c) { return me_mom_step(c, &done[g]); }) != ME_OK) return fail("me_mom_step");
+    }
+    if (me_mom_end(ctx_, &run.res) != ME_OK) return fail("me_mom_end");
+  }
+  const std::string path = results_subfolder + "map_mom.txt";
+  std::ofstream f(path);
+  if (!f.is_open()) {
+    std::cerr << "ERROR: cannot write " << path << std::endl;
+    return -1;
+  }
+  static const char *status[] = {"OK", "NO_PLANAR", "NO_SECOND_AXIS", "SMALL_FAMILY"};
+  f << std::setprecision(17) << "# mutually orthogonal metric without a ground truth (after Kornilova & Ferrer 2021, this project's "
+       "rule): planar points (v <= planarity lambda2) of MME's neighbourhoods, three orthogonal plane families |n . a_j| >= "
+       "cos(angle), mom = the sum of the families' median plane variance (m^2); r = " << r << ", min_neighbors est 10";
+  if (runs.size() > 1) f << ", gt 5";
+  f << ", angle_deg " << p.angle_deg << ", planarity " << p.planarity << ", min_family " << p.min_family
+    << (param_.evaluate_without_gt_ ? "; est as loaded\n" : "; est in the ground truth's frame\n");
+  f << "cloud n_points n_query n_pv n_planar a1_x a1_y a1_z a2_x a2_y a2_z a3_x a3_y a3_z n_1 mean_1 median_1 n_2 mean_2 median_2 "
+       "n_3 mean_3 median_3 mom status\n" << std::fixed << std::setprecision(15);
+  for (const Run &run : runs) {
+    const me_mom_result &x = run.res;
+    f << run.name << " " << x.n_points << " " << x.n_query << " " << x.n_pv << " " << x.n_planar;
+    for (int k = 0; k < 9; ++k) f << " " << x.axis[k];
+    for (int j = 0; j < 3; ++j) f << " " << x.n[j] << " " << x.mean[j] << " " << x.median[j];
+    f << " " << x.mom << " " << (x.status >= 0 && x.status < 4 ? status[x.status] : "?") << "\n";
+  }
+  std::cout << "INFO: mutually orthogonal metric:";
+  for (size_t i = 0; i < runs.size(); ++i)
+    std::cout << (i ? "," : "") << " " << runs[i].name << " MOM " << runs[i].res.mom << " m^2 ("
+              << status[std::min(3, std::max(0, (int)runs[i].res.status))] << ")";
+  std::cout << "; saved to " << path << std::endl;
+  return 0;
+}
+
+// evaluate_without_gt: the estimate alone, loaded and down-sampled as on the other paths, then MME, local consistency and MOM
+inline int MapEvalB200::processWithoutGt() {
+  TicToc tic_toc;
+  std::cout << "INFO: evaluate_without_gt: only the estimate is evaluated; gt_map_path, registration_methods, accuracy_level, "
+               "initial_matrix, evaluate_using_initial, evaluate_gt_mme and vmd_voxel_size are ignored" << std::endl;
+  std::string err;
+  const std::string est_path = param_.evaluation_map_pcd_path_ + param_.pcd_file_name_;
+  if (!cloud_io::read_pcd(est_path, map_3d_, &err, nullptr)) {
+    std::cerr << "ERROR: Failed to load point cloud from the specified path." << std::endl;
+    return -1;
+  }
+  if (map_3d_.empty()) {
+    std::cerr << "ERROR: the estimated map is empty!" << std::endl;
+    return -1;
+  }
+  if (!gpus_.create(std::max(1, param_.n_gpus_), param_.gpu_device_, 0.0)) return fail("cannot create the GPU context(s)");
+  ctx_ = gpus_.ctx(0);
+  if (gpus_.size() > 1) std::cout << "INFO: sharding the sweeps over " << gpus_.size() << " GPUs (NCCL all-reduce of the accumulators)" << std::endl;
+  std::vector<int64_t> ne(gpus_.size(), (int64_t)(map_3d_.size() / 3));
+  if (gpus_.for_each([&](int r, me_ctx *c) {
+        int rc = me_set_cloud(c, ME_CLOUD_EST, map_3d_.data(), (int64_t)(map_3d_.size() / 3));
+        if (rc == ME_OK && param_.downsample_size > 0) rc = me_voxel_downsample(c, ME_CLOUD_EST, param_.downsample_size, &ne[r]);
+        return rc;
+      }) != ME_OK)
+    return fail("uploading / down-sampling the estimated map");
+  if (!(param_.downsample_size > 0)) std::cout << "INFO: downsample_size <= 0: the map is evaluated as loaded." << std::endl;
+  n_est_ = ne[0];
+  n_gt_ = 0;
+  file_result << std::fixed << std::setprecision(15) << "Estimated-Ground Truth point count: " << n_est_ << " / " << 0 << std::endl;
+  t1 = tic_toc.toc();
+  if (param_.evaluate_mme_) {
+    if (computeMME() != 0) return -1;
+    t2 = tic_toc.toc();
+    if (param_.save_immediate_result_) saveMmeResults();
+    else file_result << std::fixed << std::setprecision(5) << "MME: " << mme_est << " " << mme_gt << " " << min_abs_entropy << " "
+                     << max_abs_entropy << std::endl;
+  }
+  if (param_.evaluate_consistency_ && localConsistency() != 0) return -1;
+  if (param_.evaluate_mom_ && mom() != 0) return -1;
   return 0;
 }
 
@@ -1189,7 +1341,7 @@ inline void MapEvalB200::saveMmeResults() {   // map_eval.cpp:392-421
   // map_eval.cpp:404-412
   if (!render::write_pcd(results_subfolder + "map_entropy.pcd", map_3d_entropy_)) std::cerr << "ERROR: cannot write map_entropy.pcd" << std::endl;
   else if (param_.enable_debug) std::cout << "INFO: Saved rendered entropy map to " << results_subfolder + "map_entropy.pcd" << std::endl;
-  if (param_.evaluate_gt_mme_) {
+  if (gt_mme()) {
     if (!render::write_pcd(results_subfolder + "gt_entropy.pcd", gt_3d_entropy_)) std::cerr << "ERROR: cannot write gt_entropy.pcd" << std::endl;
     else if (param_.enable_debug)
       std::cout << "INFO: Saved rendered entropy ground truth map to " << results_subfolder + "gt_entropy.pcd" << std::endl;

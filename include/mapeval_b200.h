@@ -674,6 +674,61 @@ ME_API int  me_consistency_finalize(int64_t n_regions, double region_size, const
                                     me_consistency_result *whole);   /* host only */
 ME_API int  me_get_consistency_points(me_ctx *ctx, int which, double *entropy, double *plane_variance);
 
+/* ---- the mutually orthogonal metric (MOM) without a ground truth: plane thickness on three orthogonal plane families ------
+ * After Kornilova & Ferrer (ECMR 2021), by this project's own rule (DESIGN §3.16).  For cloud `which` as it is now, radius r
+ * and min_neighbors m as me_consistency_begin, and the parameters p (angle_deg in (0, 30], planarity in (0, 1], min_family >=
+ * 1), per point: me_consistency's neighbourhood, covariance and v (the same bits), lambda2 = the middle eigenvalue, and the
+ * unit normal n = the eigenvector of v's eigenvalue, normalised in fp64, its largest component positive (the lowest axis on a
+ * tie).  Planar: k >= m, v finite, lambda2 > 0 and v <= planarity * lambda2.  Every planar point adds 1 to the cube-map bins
+ * of n and of -n (6 ME_MOM_CELLS_PER_EDGE^2 bins; DESIGN §3.16); me_mom_axes picks a1, a2, a3 from the reduced histogram.
+ * Family j: the planar points with |n . a_j| >= cos(angle) (the lowest j first).  Per family: n_j, mean_j = sum v / n_j and
+ * median_j = numpy's quantile(v, 0.5, method="linear"), exact.  mom = median_1 + median_2 + median_3, NaN unless status is
+ * ME_MOM_OK (any n_j < min_family: ME_MOM_SMALL_FAMILY; the per-family fields are still filled).  Without axes
+ * (ME_MOM_NO_PLANAR, ME_MOM_NO_SECOND_AXIS) no family is formed: n_j = 0, mean_j and median_j are NaN, every point's family
+ * is -1, and axis holds a1 (ME_MOM_NO_SECOND_AXIS) or NaN.
+ * The loop (every rank the same calls): me_mom_begin checks, sweeps this rank's query range and histograms it;
+ * me_mom_block hands out the running pass's block (*n = ME_MOM_BLOCK fp64 values, every rank and pass), which the caller
+ * SUM-reduces in place (after me_synchronize); me_mom_step reads the reduced block and runs the next pass (*done = 1 after
+ * the last); me_mom_end fills the result.  Refused as me_consistency_begin (r, m, an empty cloud, an open registration or
+ * drift loop, world > 1 with ME_LAYOUT_SLAB requested, calls out of order, a cloud changed between begin and end), and
+ * angle_deg, planarity or min_family out of range.  The sweep lays the cloud out as me_consistency_begin does.
+ * me_mom: the whole loop at world 1.  me_mom_axes (host only): the axes (9 values, a1 a2 a3, NaN when not found) and the
+ * status (ME_MOM_OK, ME_MOM_NO_PLANAR, ME_MOM_NO_SECOND_AXIS) from an integer histogram of 6 M^2 bins.
+ * me_get_mom_points: the last call's v, lambda2, normal (3 per point) and family (0..2, -1 none) of cloud `which`, caller
+ * order (any pointer may be NULL); points another rank evaluated hold NaN and -1.  Valid until the cloud changes. */
+#define ME_MOM_CELLS_PER_EDGE 16
+#define ME_MOM_BINS (6 * ME_MOM_CELLS_PER_EDGE * ME_MOM_CELLS_PER_EDGE)
+#define ME_MOM_BLOCK (6 + 3 * 4 * 256)
+enum me_mom_status {
+  ME_MOM_OK = 0,
+  ME_MOM_NO_PLANAR = 1,             /* no planar point                                  */
+  ME_MOM_NO_SECOND_AXIS = 2,        /* no populated bin within angle_deg of a1's plane   */
+  ME_MOM_SMALL_FAMILY = 3           /* a family has fewer than min_family points         */
+};
+typedef struct {
+  double  angle_deg;                            /* (0, 30]; 10 by default */
+  double  planarity;                            /* (0, 1];  0.5 by default */
+  int64_t min_family;                           /* >= 1;    100 by default */
+} me_mom_params;
+typedef struct {
+  double  radius, angle_deg, planarity;
+  int64_t min_family;
+  int32_t min_neighbors, kernel, rings, solo;   /* as me_consistency_result */
+  int64_t n_points, n_query, n_pv, n_planar;
+  double  axis[9];                              /* a1, a2, a3 */
+  int64_t n[3];
+  double  mean[3], median[3];
+  double  mom;
+  int32_t status, reserved;
+} me_mom_result;
+ME_API int  me_mom_begin(me_ctx *ctx, int which, double radius, int32_t min_neighbors, const me_mom_params *p);
+ME_API int  me_mom_block(me_ctx *ctx, double **device_block, int32_t *n);
+ME_API int  me_mom_step(me_ctx *ctx, int32_t *done);
+ME_API int  me_mom_end(me_ctx *ctx, me_mom_result *out);
+ME_API int  me_mom(me_ctx *ctx, int which, double radius, int32_t min_neighbors, const me_mom_params *p, me_mom_result *out);
+ME_API int  me_mom_axes(const int64_t *hist, int32_t cells_per_edge, double angle_deg, double *axes, int32_t *status);  /* host only */
+ME_API int  me_get_mom_points(me_ctx *ctx, int which, double *v, double *lambda2, double *normal, int8_t *family);
+
 /* replaces: ComputeMeanMapEntropyUsingNormalTBB / ...UsingNormal (min_neighbors 10, map_eval.cpp:1608-1737, 1538-1606),
  * ComputeMeanMapEntropy (min_neighbors 5, :1438-1535), ComputeEntropy (:1433-1436) and the min/max side effect of
  * ColorPointCloudByMME (:697-701).  entropies_host (nullable) receives N fp64, zeros where invalid.
