@@ -250,6 +250,12 @@ class me_mom_result(C.Structure):
                 ("mom", C.c_double), ("status", C.c_int32), ("reserved", C.c_int32)]
 
 
+class me_mom_region_row(C.Structure):
+    _fields_ = [("index", C.c_int64 * 3), ("n_points", C.c_int64), ("n_planar", C.c_int64), ("n", C.c_int64 * 3),
+                ("mean", C.c_double * 3), ("median", C.c_double * 3), ("mom", C.c_double), ("status", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
 class me_mme_accum(C.Structure):
     _fields_ = [("n_query", C.c_int64), ("n_valid", C.c_int64), ("sum_entropy", C.c_double),
                 ("min_entropy", C.c_double), ("max_entropy", C.c_double)]

@@ -34,6 +34,7 @@ SYMBOLS = (
     "me_consistency_begin", "me_consistency_block", "me_consistency_end", "me_consistency", "me_consistency_finalize",
     "me_get_consistency_points",
     "me_mom_begin", "me_mom_block", "me_mom_step", "me_mom_end", "me_mom", "me_mom_axes", "me_get_mom_points",
+    "me_mom_region_begin", "me_mom_region_block", "me_mom_region_end", "me_mom_regions",
 )
 
 _lib = None
@@ -163,6 +164,10 @@ def load():
     L.me_mom.argtypes = [ctx, C.c_int, C.c_double, C.c_int32, C.POINTER(A.me_mom_params), C.POINTER(A.me_mom_result)]
     L.me_mom_axes.argtypes = [i64p, C.c_int32, C.c_double, dp, C.POINTER(C.c_int32)]
     L.me_get_mom_points.argtypes = [ctx, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.me_mom_region_begin.argtypes = [ctx, C.c_double, C.c_int64, i64p]
+    L.me_mom_region_block.argtypes = [ctx, C.POINTER(dp), i64p]
+    L.me_mom_region_end.argtypes = [ctx, C.c_void_p, C.c_int64]
+    L.me_mom_regions.argtypes = [ctx, C.c_double, C.c_int64, C.POINTER(C.c_void_p), i64p]
     L.me_kernel_trace.argtypes = [ctx, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.c_int32]
     if L.me_abi_version() != A.ME_ABI_VERSION:
         raise RuntimeError("libmapeval_b200.so ABI version mismatch")

@@ -225,6 +225,32 @@ def mom_dict(res):
     return out
 
 
+# me_mom_region_row as a numpy record (8-byte fields, then two int32: no padding)
+_MOM_REGION_ROW_DT = np.dtype([("index", "<i8", 3), ("n_points", "<i8"), ("n_planar", "<i8"), ("n", "<i8", 3), ("mean", "<f8", 3),
+                               ("median", "<f8", 3), ("mom", "<f8"), ("status", "<i4"), ("reserved", "<i4")])
+assert _MOM_REGION_ROW_DT.itemsize == C.sizeof(A.me_mom_region_row) and \
+    _MOM_REGION_ROW_DT.names == tuple(f[0] for f in A.me_mom_region_row._fields_)
+
+
+def mom_region_dict(rows, region_size):
+    """me_mom_region_row records (numpy, _MOM_REGION_ROW_DT) at region size s -> {'index' / 'lo' / 'hi' (n, 3): the region
+    floor(x / s) and its bounds index * s, (index + 1) * s; 'n_points', 'n_planar' (n,); 'n' / 'mean' / 'median' (n, 3)
+    per family; 'mom' (n,); 'status' (n,) ME_MOM_* names, as mom_dict names them}"""
+    s = float(region_size)
+    out = {name: np.array(rows[name]) for name in ("index", "n_points", "n_planar", "n", "mean", "median", "mom")}
+    out["index"] = out["index"].reshape(-1, 3)
+    for name in ("n", "mean", "median"):
+        out[name] = out[name].reshape(-1, 3)
+    out["lo"] = out["index"].astype(np.float64) * s
+    out["hi"] = (out["index"] + 1).astype(np.float64) * s
+    codes = np.asarray(rows["status"]).reshape(-1)
+    names = np.array([A.MOM_STATUS_NAMES[k] for k in sorted(A.MOM_STATUS_NAMES)], dtype=object)
+    if len(codes) and not ((codes >= 0) & (codes < len(names))).all():
+        raise ValueError("mom_region_dict: a status outside me_mom_status")
+    out["status"] = names[codes]
+    return out
+
+
 def mom_params(angle_deg=10.0, planarity=0.5, min_family=100):
     return A.me_mom_params(float(angle_deg), float(planarity), int(min_family))
 
@@ -289,6 +315,8 @@ class MapEvalB200:
             raise MapEvalError(rc, msg.decode() if msg else "me_create failed")
         self.n = [0, 0]
         self._keep = [None, None]   # keeps host/device buffers alive while the library may read them
+        self._mom_min_family_last = None   # min_family of the last finished MOM call (mom_regions' default)
+        self._mom_region_size = None
         self.rank, self.world = int(rank), int(world)
 
     # -- lifecycle -------------------------------------------------------------------------------------------
@@ -750,6 +778,7 @@ class MapEvalB200:
         out = A.me_mom_result()
         p = mom_params(angle_deg, planarity, min_family)
         self._check(self._L.me_mom(self._ctx, int(which), float(radius), int(min_neighbors), C.byref(p), C.byref(out)))
+        self._mom_min_family_last = out.min_family
         return mom_dict(out)
 
     def mom_begin(self, which, radius, min_neighbors=10, angle_deg=10.0, planarity=0.5, min_family=100):
@@ -773,6 +802,7 @@ class MapEvalB200:
     def mom_end(self):
         out = A.me_mom_result()
         self._check(self._L.me_mom_end(self._ctx, C.byref(out)))
+        self._mom_min_family_last = out.min_family
         return mom_dict(out)
 
     def get_mom_points(self, which):
@@ -786,6 +816,51 @@ class MapEvalB200:
         self._check(self._L.me_get_mom_points(self._ctx, int(which), v.ctypes.data_as(C.c_void_p), l2.ctypes.data_as(C.c_void_p),
                                               nrm.ctypes.data_as(C.c_void_p), fam.ctypes.data_as(C.c_void_p)))
         return v, l2, nrm, fam
+
+    def mom_regions(self, region_size, min_family=None):
+        """The last finished MOM call broken down by region floor(x / region_size) (me_mom_regions, world 1), without a new
+        sweep: per region the cloud's points, its planar points and, per family of the whole map, the count, mean and exact
+        median of v; 'mom' the sum of the medians.  min_family None: the MOM call's.  Returns mom_region_dict's dict.
+        Multi-GPU: dist.mom_regions_distributed."""
+        rows = C.c_void_p()
+        n = C.c_int64(0)
+        self._check(self._L.me_mom_regions(self._ctx, float(region_size), self._mom_min_family(min_family), C.byref(rows),
+                                           C.byref(n)))
+        try:
+            nb = n.value * _MOM_REGION_ROW_DT.itemsize
+            a = np.frombuffer((C.c_char * nb).from_address(rows.value), _MOM_REGION_ROW_DT).copy() if nb else \
+                np.zeros(0, _MOM_REGION_ROW_DT)
+            return mom_region_dict(a, region_size)
+        finally:
+            if rows.value:
+                self._L.me_free(rows)
+
+    def _mom_min_family(self, min_family):
+        if min_family is not None:
+            return int(min_family)
+        if self._mom_min_family_last is None:
+            raise MapEvalError(A.ME_ERR_INVALID, "mom_regions: min_family=None needs a MOM call on this context first")
+        return self._mom_min_family_last
+
+    def mom_region_begin(self, region_size, min_family=None):
+        """me_mom_region_begin: writes this rank's points of the last finished MOM call into the block; returns the row count"""
+        n = C.c_int64(0)
+        self._check(self._L.me_mom_region_begin(self._ctx, float(region_size), self._mom_min_family(min_family), C.byref(n)))
+        self._mom_region_size = float(region_size)
+        return n.value
+
+    def mom_region_block(self):
+        """(device pointer, n) of the block [v | code], 2 n_points fp64 values: SUM-reduce it in place (after synchronize())"""
+        ptr = C.POINTER(C.c_double)()
+        n = C.c_int64(0)
+        self._check(self._L.me_mom_region_block(self._ctx, C.byref(ptr), C.byref(n)))
+        return C.cast(ptr, C.c_void_p).value, n.value
+
+    def mom_region_end(self, n_regions):
+        """the rows from the reduced block, as mom_regions"""
+        rows = np.zeros(max(int(n_regions), 1), _MOM_REGION_ROW_DT)
+        self._check(self._L.me_mom_region_end(self._ctx, rows.ctypes.data_as(C.c_void_p), int(n_regions)))
+        return mom_region_dict(rows[:int(n_regions)], self._mom_region_size)
 
     def get_nn(self, which_query):
         n = self.n[which_query]

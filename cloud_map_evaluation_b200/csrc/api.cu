@@ -242,6 +242,7 @@ void me_destroy(me_ctx *ctx) {
   nn_surface_free(ctx);
   consistency_free(ctx);
   mom_free(ctx);
+  mom_region_free(ctx);
   drift_close(ctx, false);
   if (ctx->copy_stream) { cudaStreamSynchronize(ctx->copy_stream); cudaStreamDestroy(ctx->copy_stream); }
   if (ctx->compute_mark) cudaEventDestroy(ctx->compute_mark);
@@ -1243,6 +1244,52 @@ int me_get_mom_points(me_ctx *ctx, int which, double *v, double *lambda2, double
   ME_ENTER(ctx);
   if (!cloud_id(which)) return fail(ctx, ME_ERR_INVALID, "bad cloud id");
   return mom_points(ctx, which, v, lambda2, normal, family);
+}
+
+int me_mom_region_begin(me_ctx *ctx, double region_size, int64_t min_family, int64_t *n_regions) {
+  ME_ENTER(ctx);
+  if (!n_regions) return fail(ctx, ME_ERR_INVALID, "null argument");
+  *n_regions = 0;
+  ctx->mom_region.open = false;
+  if (!(std::isfinite(region_size) && region_size > 0.0))
+    return fail(ctx, ME_ERR_INVALID, "me_mom_region_begin: region_size must be finite and > 0");
+  if (min_family < 1) return fail(ctx, ME_ERR_INVALID, "me_mom_region_begin: min_family must be >= 1");
+  return mom_region_begin(ctx, region_size, min_family, n_regions);
+}
+
+int me_mom_region_block(me_ctx *ctx, double **device_block, int64_t *n) {
+  ME_ENTER(ctx);
+  if (!device_block || !n) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return mom_region_block(ctx, device_block, n);
+}
+
+int me_mom_region_end(me_ctx *ctx, me_mom_region_row *rows, int64_t capacity) {
+  ME_ENTER(ctx);
+  return mom_region_end(ctx, rows, capacity);
+}
+
+int me_mom_regions(me_ctx *ctx, double region_size, int64_t min_family, me_mom_region_row **rows, int64_t *n_regions) {
+  ME_ENTER(ctx);
+  if (!rows || !n_regions) return fail(ctx, ME_ERR_INVALID, "null argument");
+  *rows = nullptr;
+  *n_regions = 0;
+  if (ctx->world != 1)
+    return fail(ctx, ME_ERR_INVALID, "me_mom_regions needs world == 1; use me_mom_region_begin / _block + all-reduce / _end");
+  int64_t n = 0;
+  ME_TRY(me_mom_region_begin(ctx, region_size, min_family, &n));
+  me_mom_region_row *r = (me_mom_region_row *)std::malloc((size_t)std::max<int64_t>(n, 1) * sizeof(me_mom_region_row));
+  if (!r) {
+    ctx->mom_region.open = false;
+    return fail(ctx, ME_ERR_NOMEM, "me_mom_regions: host allocation of the rows failed");
+  }
+  const int rc = me_mom_region_end(ctx, r, n);
+  if (rc != ME_OK) {
+    std::free(r);
+    return rc;
+  }
+  *rows = r;
+  *n_regions = n;
+  return ME_OK;
 }
 
 int me_drift_begin(me_ctx *ctx, double region_size, double max_correspondence_distance, int32_t max_iteration,

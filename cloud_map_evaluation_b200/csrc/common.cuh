@@ -173,15 +173,17 @@ struct IcpRun {
   int it = 0, converged = 0;
 };
 
-// numpy's method="linear" position of probability p among n sorted values: h = (n - 1) p, k = floor(h), g = h - k
-inline void quantile_rank(long long n, double p, long long *k, double *g) {
+// numpy's method="linear" position of probability p among n sorted values: h = (n - 1) p, k = floor(h), g = h - k.  Also
+// called on the device (mom_region.cu): a device caller is compiled with -fmad=false, so that it rounds every operation as the
+// host does.
+__host__ __device__ inline void quantile_rank(long long n, double p, long long *k, double *g) {
   const double h = (double)(n - 1) * p;
   const double f = std::floor(h);
   *k = (long long)f;
   *g = h - f;
 }
 // numpy's _lerp in its operation order: lo + (hi - lo) g below g = 0.5, hi - (hi - lo) (1 - g) from there
-inline double quantile_lerp(double lo, double hi, double g) {
+__host__ __device__ inline double quantile_lerp(double lo, double hi, double g) {
   const double diff = hi - lo;
   return g >= 0.5 ? hi - diff * (1.0 - g) : lo + diff * g;
 }
@@ -301,6 +303,7 @@ struct MomRun {
   double radius = 0.0, angle_deg = 0.0, planarity = 0.0, cos_a = 0.0;
   long long min_family = 0;
   int stage = 0;                       // what the block holds: 0 the direction histogram, 1 the fold and digit 0, 2.. digit stage - 1
+  bool ended = false;                  // me_mom_end filled the result of this call (the per-region breakdown reads it)
   long long n_query = 0, n_pv = 0, n_planar = 0;
   int status = 0;
   double axes[9];
@@ -324,6 +327,32 @@ struct MomRun {
   long long cap_v[2] = {0, 0}, cap_l2[2] = {0, 0}, cap_n[2] = {0, 0}, cap_flag[2] = {0, 0};
   bool pts_valid[2] = {false, false};
   unsigned long long pts_gen[2] = {0, 0};
+};
+
+// the per-region breakdown of the last finished MOM call (me_mom_region_begin .. me_mom_region_end, mom_region.cu): the
+// occupied list, the [v | code] block (2 n fp64, the same length on every rank) and the scratch of the segmented selection
+struct MomRegionRun {
+  bool open = false;
+  unsigned long long gen = 0;          // cloud_gen at me_mom_region_begin
+  int which = 0, status = 0;           // the MOM call's cloud and its whole-map status (before the family-size test)
+  long long min_family = 0;
+  double s = 0.0;
+  long long R = 0, n = 0;              // listed regions; points of the cloud
+  std::vector<int64_t> index, n_points;   // 3 per region; per region
+  double *d_blk = nullptr;             // v of every planar point, then its code (0, family + 1, 4 planar without a family)
+  long long cap_blk = 0;
+  uint32_t *d_rid = nullptr;           // caller index -> region
+  long long cap_rid = 0;
+  unsigned long long *d_keys = nullptr;   // 3 n: the two buffers of the sort by v, then one of the sort by segment
+  long long cap_keys = 0;
+  uint32_t *d_vals = nullptr;          // 2 n
+  long long cap_vals = 0;
+  uint32_t *d_cnt = nullptr;           // segment counts (3 R + 1), planar counts (R), chunk counts (3 R + 1), the member counter
+  long long cap_cnt = 0;
+  double *d_out = nullptr;             // per segment: the median, then the sum of v
+  long long cap_out = 0;
+  double *d_part = nullptr;            // the fold's per-chunk sums
+  long long cap_part = 0;
 };
 
 // the per-region table (me_nn_region_begin .. me_nn_region_end, region.cu): the occupied list and the block, the same
@@ -489,6 +518,7 @@ struct me_ctx {
   me::SurfaceRun surface;              // point-to-plane metrics (me_nn_surface*), from the NN records
   me::ConsistencyRun consistency;      // local map consistency (me_consistency*): MPV and MME per region
   me::MomRun mom;                      // the mutually orthogonal metric (me_mom*)
+  me::MomRegionRun mom_region;         // its per-region breakdown (me_mom_region*)
   std::string err;
 };
 
@@ -605,6 +635,8 @@ int nn_region_block(me_ctx *ctx, double **device_block, int32_t *n_sum, int32_t 
 int nn_region_end(me_ctx *ctx, me_region_row *rows, int64_t capacity);
 void nn_region_free(me_ctx *ctx);
 int list_regions(me_ctx *ctx, const char *who, double s, bool with_gt, RegionList *L);
+// rid[i] = the region of point i of cloud `which` in the list L (which must be listed)
+int region_ids(me_ctx *ctx, const RegionList &L, int which, uint32_t *rid);
 int record_positions(me_ctx *ctx, int which, uint32_t *pos_of);
 // one point-to-point ICP per region of the estimated cloud (arguments checked by the caller) — me_drift_* (drift.cu)
 int drift_begin(me_ctx *ctx, double s, double max_dist, int max_iter, double rel_fitness, double rel_rmse, int64_t *n_regions);
@@ -643,6 +675,11 @@ int mom_step(me_ctx *ctx, int32_t *done);
 int mom_end(me_ctx *ctx, me_mom_result *out);
 int mom_points(me_ctx *ctx, int which, double *v, double *lambda2, double *normal, int8_t *family);
 void mom_free(me_ctx *ctx);
+// its per-region breakdown (me_mom_region_*, mom_region.cu; arguments checked by the caller)
+int mom_region_begin(me_ctx *ctx, double s, long long min_family, int64_t *n_regions);
+int mom_region_block(me_ctx *ctx, double **device_block, int64_t *n);
+int mom_region_end(me_ctx *ctx, me_mom_region_row *rows, int64_t capacity);
+void mom_region_free(me_ctx *ctx);
 
 // layout of me_ctx::d_block (fp64): the SUM-reducible part first, then the MAX-reducible part.  Counts ride as fp64 (exact
 // below 2^53, so their sums are exact and order-independent).

@@ -4,7 +4,7 @@
 //
 // Begin:
 //   list_regions (region.cu, est only)  the occupied regions floor(x / s) in caller order
-//   drift_rid_kernel                    rid[i] = the region of caller index i
+//   region_ids (region.cu)             rid[i] = the region of caller index i
 //   drift_fold_kernel<true> + merge     per region count and sum (x - c_r) of the original points: the centroids
 // Per iteration:
 //   drift_transform_kernel              x_i := T_{rid[i]} x_i^orig, transform_kernel's rounding, from the original coordinates
@@ -26,12 +26,6 @@ namespace me {
 
 static constexpr int kThreads = 256;
 static constexpr int kB = ME_ICP_BLOCK_P2P;         // values per region
-
-__global__ void __launch_bounds__(kThreads) drift_rid_kernel(const uint32_t *__restrict__ val, const uint32_t *__restrict__ pos,
-                                                             long long n, uint32_t *__restrict__ rid) {
-  for (long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x; j < n; j += (long long)gridDim.x * blockDim.x)
-    rid[__ldg(val + j)] = __ldg(pos + j + 1) - 1;
-}
 
 // transform_kernel's operation order: o_r = (((T_r0 x + T_r1 y) + T_r2 z) + T_r3), x' = o_0 / o_3, ..., with T of the point's
 // region
@@ -225,10 +219,8 @@ int drift_begin(me_ctx *ctx, double s, double max_dist, int max_iter, double rel
   D.open = true;
   D.gen = ctx->cloud_gen;
   // the list lives in d_work, which the sweeps reuse: keep what the loop needs
-  const int blocks = (int)std::min<long long>((n + kThreads - 1) / kThreads, (long long)ctx->sm_count * 16);
-  drift_rid_kernel<<<blocks, kThreads, 0, ctx->stream>>>(RL.val, RL.pos, n, D.d_rid);
-  if (cudaGetLastError() != cudaSuccess) return drift_fail(ctx, fail(ctx, ME_ERR_CUDA, "drift_rid_kernel launch failed"));
-  ctx->launches++;
+  rc = region_ids(ctx, RL, ME_CLOUD_EST, D.d_rid);
+  if (rc != ME_OK) return drift_fail(ctx, rc);
   if (cudaMemcpyAsync(D.d_val, RL.val, (size_t)n * 4, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess ||
       cudaMemcpyAsync(D.d_seg, RL.seg, (size_t)(R + 1) * 4, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess ||
       cudaMemcpyAsync(D.d_chunk_off, RL.chunks, (size_t)(R + 1) * 4, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess ||

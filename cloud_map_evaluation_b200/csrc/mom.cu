@@ -305,6 +305,7 @@ static int mom_to_block(me_ctx *ctx, int n) {
 int mom_begin(me_ctx *ctx, int which, double radius, int min_neighbors, const me_mom_params *p) {
   MomRun &R = ctx->mom;
   R.open = false;
+  R.ended = false;
   Cloud &c = ctx->cloud[which];
   if (c.n <= 0) return fail(ctx, ME_ERR_EMPTY, "me_mom_begin: the cloud is empty");
   if (ctx->icp.open) return fail(ctx, ME_ERR_INVALID, "me_mom_begin while a registration is open (me_icp_end first)");
@@ -525,6 +526,7 @@ int mom_end(me_ctx *ctx, me_mom_result *out) {
       if (out->n[j] < R.min_family) status = ME_MOM_SMALL_FAMILY;
   out->status = status;
   out->mom = status == ME_MOM_OK ? (out->median[0] + out->median[1]) + out->median[2] : NAN;
+  R.ended = true;
   return ME_OK;
 }
 

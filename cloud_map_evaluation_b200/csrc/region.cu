@@ -9,6 +9,7 @@
 //   region_head_kernel   + exclusive_scan_inplace: the region of every sorted point and the region count
 //   region_list_kernel   first sorted position, est/gt split and key of every region
 //   region_count_kernel  n_est / n_gt per region, and the chunks of kRegionChunk query points per region and direction
+//   region_rid_kernel    (region_ids) the region of every caller index of one cloud: the drift loop, the MOM breakdown
 // Record fold, per evaluated direction, over this rank's records:
 //   record_pos_kernel    caller index -> position of its record in the cell-sorted cloud (~0u: not laid out here)
 //   region_fold_kernel   one warp per chunk: lane l walks the chunk's points l, l + 32, ..., keeps the pairs with
@@ -73,6 +74,16 @@ __global__ void __launch_bounds__(kThreads) region_list_kernel(const unsigned lo
     const bool last = i + 1 == n || pos[i + 2] != pos[i + 1];
     if (val[i] < n_est && (last || val[i + 1] >= n_est)) est_end[r] = (uint32_t)(i + 1);
     if (i == n - 1) seg[r + 1] = (uint32_t)n;
+  }
+}
+
+// rid[val[j] - id0] = the region of sorted point j, for the caller ids [id0, id0 + n_c) of one cloud (the other cloud's ids
+// wrap to >= n_c)
+__global__ void __launch_bounds__(kThreads) region_rid_kernel(const uint32_t *__restrict__ val, const uint32_t *__restrict__ pos,
+                                                              long long n, uint32_t id0, uint32_t n_c, uint32_t *__restrict__ rid) {
+  for (long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x; j < n; j += (long long)gridDim.x * blockDim.x) {
+    const uint32_t i = __ldg(val + j) - id0;
+    if (i < n_c) rid[i] = __ldg(pos + j + 1) - 1;
   }
 }
 
@@ -313,6 +324,14 @@ int list_regions(me_ctx *ctx, const char *who, double s, bool with_gt, RegionLis
     L->n_est[r] = hcnt[r];
     L->n_gt[r] = hcnt[R + r];
   }
+  return ME_OK;
+}
+
+int region_ids(me_ctx *ctx, const RegionList &L, int which, uint32_t *rid) {
+  const uint32_t id0 = which == ME_CLOUD_EST ? 0u : (uint32_t)ctx->cloud[ME_CLOUD_EST].n;
+  const int blocks = (int)std::min<long long>((L.n + kThreads - 1) / kThreads, (long long)ctx->sm_count * 16);
+  region_rid_kernel<<<std::max(blocks, 1), kThreads, 0, ctx->stream>>>(L.val, L.pos, L.n, id0, (uint32_t)ctx->cloud[which].n, rid);
+  ME_LAUNCH_CHECK(ctx);
   return ME_OK;
 }
 

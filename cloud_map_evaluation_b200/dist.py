@@ -130,6 +130,21 @@ def mom_distributed(ctx, device, which, radius, min_neighbors=10, angle_deg=10.0
     return ctx.mom_end()
 
 
+def mom_regions_distributed(ctx, device, region_size, min_family=None, group=None):
+    """The last finished MOM call per region over every rank of the job (MapEvalB200.mom_regions for world > 1): every rank
+    writes the points it swept into the block [v | code], ONE in-place SUM all-reduce gathers them exactly (x + 0 = x), and
+    every rank runs the same segmented selection on the same bits, so every rank returns the same rows."""
+    import torch
+    import torch.distributed as dist
+    n = ctx.mom_region_begin(region_size, min_family)
+    if dist.is_initialized() and dist.get_world_size(group) > 1:
+        ptr, m = ctx.mom_region_block()
+        ctx.synchronize()
+        dist.all_reduce(torch.as_tensor(_DeviceBlock(ptr, m), device=device), group=group)
+        torch.cuda.current_stream(device).synchronize()
+    return ctx.mom_region_end(n)
+
+
 def quantiles_distributed(ctx, device, p, population=A.ME_DIST_KEPT, group=None):
     """Exact distance quantiles of the last NN evaluation over every rank of the job (MapEvalB200.distance_quantiles for
     world > 1): the selection loop with ONE in-place SUM all-reduce of the pass's integer counts (as fp64, exact) per pass.

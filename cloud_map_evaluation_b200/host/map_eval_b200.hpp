@@ -114,6 +114,8 @@ struct Param {   // map_eval.h:60-116
   bool evaluate_mom_ = false;
   double mom_angle_deg_ = 10.0, mom_planarity_ = 0.5;
   int64_t mom_min_family_ = 100;
+  // the MOM call of each cloud per region floor(x / mom_region_size) (0 = off), written to map_mom_regions.txt (me_mom_region*)
+  double mom_region_size_ = 0.0;
   // the estimate alone: gt_map_path is neither read nor required; MME, local consistency and MOM run on the est cloud
   bool evaluate_without_gt_ = false;
 };
@@ -224,6 +226,13 @@ inline Param loadParametersFromYAML(const std::string &yaml_file_path) {
         throw std::runtime_error("mom_min_family must be an integer >= 1, not " + config["mom_min_family"].as<std::string>());
       param.mom_min_family_ = (int64_t)mf;
     }
+    if (config["mom_region_size"]) {
+      param.mom_region_size_ = config["mom_region_size"].as<double>();
+      if (!(std::isfinite(param.mom_region_size_) && param.mom_region_size_ >= 0.0))
+        throw std::runtime_error("mom_region_size must be finite and >= 0 (0 = off), not " + config["mom_region_size"].as<std::string>());
+      if (param.mom_region_size_ > 0.0 && !param.evaluate_mom_)
+        throw std::runtime_error("mom_region_size needs evaluate_mom: true (it breaks the MOM call down by region)");
+    }
     return param;
   } catch (const std::exception &e) {
     std::cerr << "Error loading parameters: " << e.what() << std::endl;
@@ -258,6 +267,7 @@ inline void dumpParam(const Param &p, std::ostream &os) {
      << "\nsurface_normals_knn=" << p.surface_normals_knn_ << "\nevaluate_consistency=" << p.evaluate_consistency_
      << "\nconsistency_region_size=" << p.consistency_region_size_ << "\nevaluate_mom=" << p.evaluate_mom_
      << "\nmom_angle_deg=" << p.mom_angle_deg_ << "\nmom_planarity=" << p.mom_planarity_ << "\nmom_min_family=" << p.mom_min_family_
+     << "\nmom_region_size=" << p.mom_region_size_
      << "\nevaluate_without_gt=" << p.evaluate_without_gt_ << "\n";
 }
 
@@ -941,14 +951,16 @@ inline int MapEvalB200::localConsistency() {
 inline int MapEvalB200::mom() {
   const double r = param_.nn_radius_;
   const me_mom_params p{param_.mom_angle_deg_, param_.mom_planarity_, param_.mom_min_family_};
+  const double s = param_.mom_region_size_;
   struct Run {
     int which, m;
     const char *name;
     me_mom_result res;
+    std::vector<me_mom_region_row> rows;
   };
   std::vector<Run> runs;
-  runs.push_back(Run{ME_CLOUD_EST, 10, "est", me_mom_result{}});
-  if (gt_mme()) runs.push_back(Run{ME_CLOUD_GT, 5, "gt", me_mom_result{}});
+  runs.push_back(Run{ME_CLOUD_EST, 10, "est", me_mom_result{}, {}});
+  if (gt_mme()) runs.push_back(Run{ME_CLOUD_GT, 5, "gt", me_mom_result{}, {}});
   for (Run &run : runs) {
     std::vector<double *> ptr(gpus_.size(), nullptr);
     std::vector<int32_t> n(gpus_.size(), 0), done(gpus_.size(), 0);
@@ -962,7 +974,24 @@ inline int MapEvalB200::mom() {
       if (!gpus_.allreduce_device(ptr, (size_t)n[0], ncclSum)) return fail("all-reduce of the MOM block");
       if (gpus_.for_each([&](int g, me_ctx *c) { return me_mom_step(c, &done[g]); }) != ME_OK) return fail("me_mom_step");
     }
-    if (me_mom_end(ctx_, &run.res) != ME_OK) return fail("me_mom_end");
+    if (s <= 0.0) {
+      if (me_mom_end(ctx_, &run.res) != ME_OK) return fail("me_mom_end");
+      continue;
+    }
+    // per region: every GPU ends its MOM call and writes its points into the block, ONE grouped SUM all-reduce
+    std::vector<int64_t> n_regions(gpus_.size(), 0), len(gpus_.size(), 0);
+    std::vector<me_mom_result> res(gpus_.size());
+    if (gpus_.for_each([&](int g, me_ctx *c) {
+          int rc = me_mom_end(c, &res[g]);
+          if (rc == ME_OK) rc = me_mom_region_begin(c, s, p.min_family, &n_regions[g]);
+          if (rc == ME_OK) rc = me_mom_region_block(c, &ptr[g], &len[g]);
+          return rc != ME_OK ? rc : me_synchronize(c);
+        }) != ME_OK)
+      return fail("me_mom_region_begin");
+    run.res = res[0];
+    if (!gpus_.allreduce_device(ptr, (size_t)len[0], ncclSum)) return fail("all-reduce of the MOM region block");
+    run.rows.resize((size_t)n_regions[0]);
+    if (me_mom_region_end(ctx_, run.rows.data(), n_regions[0]) != ME_OK) return fail("me_mom_region_end");
   }
   const std::string path = results_subfolder + "map_mom.txt";
   std::ofstream f(path);
@@ -991,6 +1020,47 @@ inline int MapEvalB200::mom() {
     std::cout << (i ? "," : "") << " " << runs[i].name << " MOM " << runs[i].res.mom << " m^2 ("
               << status[std::min(3, std::max(0, (int)runs[i].res.status))] << ")";
   std::cout << "; saved to " << path << std::endl;
+  if (s <= 0.0) return 0;
+
+  const std::string rpath = results_subfolder + "map_mom_regions.txt";
+  std::ofstream rf(rpath);
+  if (!rf.is_open()) {
+    std::cerr << "ERROR: cannot write " << rpath << std::endl;
+    return -1;
+  }
+  rf << std::setprecision(17) << "# mutually orthogonal metric per region floor(x / s): the MOM call's axes and families, per "
+        "region and family the count, mean and exact median plane variance (m^2) of its members, mom = the sum of the medians "
+        "(NaN unless every family has min_family members); s = " << s << ", min_family " << p.min_family
+     << (param_.evaluate_without_gt_ ? "; est as loaded\n" : "; est in the ground truth's frame\n");
+  rf << "cloud min_x min_y min_z max_x max_y max_z n_points n_planar n_1 mean_1 median_1 n_2 mean_2 median_2 n_3 mean_3 median_3 "
+        "mom status\n" << std::fixed << std::setprecision(15);
+  for (const Run &run : runs)
+    for (const me_mom_region_row &x : run.rows) {
+      rf << run.name;
+      for (int a = 0; a < 3; ++a) rf << " " << (double)x.index[a] * s;
+      for (int a = 0; a < 3; ++a) rf << " " << (double)(x.index[a] + 1) * s;
+      rf << " " << x.n_points << " " << x.n_planar;
+      for (int j = 0; j < 3; ++j) rf << " " << x.n[j] << " " << x.mean[j] << " " << x.median[j];
+      rf << " " << x.mom << " " << (x.status >= 0 && x.status < 4 ? status[x.status] : "?") << "\n";
+    }
+  for (const Run &run : runs) {
+    size_t ok = 0, best = 0;
+    int best_j = -1;
+    for (size_t r = 0; r < run.rows.size(); ++r) {
+      const me_mom_region_row &x = run.rows[r];
+      ok += x.status == ME_MOM_OK;
+      for (int j = 0; j < 3; ++j)
+        if (x.n[j] > 0 && (best_j < 0 || x.median[j] > run.rows[best].median[best_j])) { best = r; best_j = j; }
+    }
+    std::cout << "INFO: MOM per region: " << run.name << " " << run.rows.size() << " regions of " << s << " m, " << ok << " OK";
+    if (best_j >= 0) {
+      const me_mom_region_row &x = run.rows[best];
+      std::cout << "; largest family median " << x.median[best_j] << " m^2 (family " << best_j + 1 << ") in [" << (double)x.index[0] * s
+                << ", " << (double)(x.index[0] + 1) * s << "] x [" << (double)x.index[1] * s << ", " << (double)(x.index[1] + 1) * s
+                << "] x [" << (double)x.index[2] * s << ", " << (double)(x.index[2] + 1) * s << "]";
+    }
+    std::cout << "; saved to " << rpath << std::endl;
+  }
   return 0;
 }
 

@@ -729,6 +729,38 @@ ME_API int  me_mom(me_ctx *ctx, int which, double radius, int32_t min_neighbors,
 ME_API int  me_mom_axes(const int64_t *hist, int32_t cells_per_edge, double angle_deg, double *axes, int32_t *status);  /* host only */
 ME_API int  me_get_mom_points(me_ctx *ctx, int which, double *v, double *lambda2, double *normal, int8_t *family);
 
+/* ---- the mutually orthogonal metric per region: where a plane family is thick ---------------------------------------------
+ * A breakdown of the last finished MOM call (me_mom_end) by region, without a new sweep (DESIGN §3.17): that call's cloud,
+ * axes, families and per-point v, valid while no cloud changed since its me_mom_begin.  A point's region is floor(x / s) per
+ * axis, the occupied list of me_consistency_begin (est ++ gt, est alone while the gt cloud is empty) with its limits and
+ * messages; at equal s the rows are the rows of me_consistency_end, in the same order.  Per region: n_points (the cloud's
+ * points), n_planar (its planar points, with a family or not), and per family j of the whole map: n_j, mean_j = sum v / n_j
+ * and median_j = numpy's quantile(v, 0.5, method="linear") of the members in the region, exact (NaN where n_j = 0);
+ * mom = (median_1 + median_2) + median_3.  status: the whole-map status when it is ME_MOM_NO_PLANAR or ME_MOM_NO_SECOND_AXIS
+ * (then n_j = 0 and NaN values); else ME_MOM_SMALL_FAMILY when some n_j < min_family (mom NaN, the per-family fields filled);
+ * else ME_MOM_OK.  The axes are the whole map's: a region whose surfaces do not lie along them has empty families.
+ * The loop (every rank the same calls): me_mom_region_begin checks and writes this rank's points into the block, *n_regions =
+ * the rows me_mom_region_end will fill; me_mom_region_block hands out the block (*n = 2 n_points fp64 values [v | code], code
+ * 0 for a point not planar or not swept by this rank, family + 1, or 4 for a planar point without a family; the same length
+ * on every rank), which the caller SUM-reduces in place (after me_synchronize); me_mom_region_end sorts the members of the
+ * reduced block by (region, family, v) and fills rows[0 .. n_regions - 1] (capacity >= n_regions).  Every rank computes the
+ * same bits from the reduced block.  Refused: no finished me_mom_end, a cloud changed since that call's me_mom_begin, s not
+ * finite or <= 0, min_family < 1, the region list's limits, an open registration or drift loop, world > 1 with ME_LAYOUT_SLAB
+ * requested, calls out of order, and a cloud changed between begin and end.  The MOM call's result and me_get_mom_points are
+ * left as they were.  me_mom_regions: the whole loop at world 1, rows allocated by the library (me_free). */
+typedef struct {
+  int64_t index[3];                             /* (ix, iy, iz) */
+  int64_t n_points, n_planar;
+  int64_t n[3];
+  double  mean[3], median[3];
+  double  mom;
+  int32_t status, reserved;                     /* status: me_mom_status */
+} me_mom_region_row;
+ME_API int  me_mom_region_begin(me_ctx *ctx, double region_size, int64_t min_family, int64_t *n_regions);
+ME_API int  me_mom_region_block(me_ctx *ctx, double **device_block, int64_t *n);
+ME_API int  me_mom_region_end(me_ctx *ctx, me_mom_region_row *rows, int64_t capacity);
+ME_API int  me_mom_regions(me_ctx *ctx, double region_size, int64_t min_family, me_mom_region_row **rows, int64_t *n_regions);
+
 /* replaces: ComputeMeanMapEntropyUsingNormalTBB / ...UsingNormal (min_neighbors 10, map_eval.cpp:1608-1737, 1538-1606),
  * ComputeMeanMapEntropy (min_neighbors 5, :1438-1535), ComputeEntropy (:1433-1436) and the min/max side effect of
  * ColorPointCloudByMME (:697-701).  entropies_host (nullable) receives N fp64, zeros where invalid.
