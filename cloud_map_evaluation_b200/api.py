@@ -342,6 +342,22 @@ class MapEvalB200:
             msg = self._L.me_last_error(self._ctx)
             raise MapEvalError(rc, msg.decode() if msg else "")
 
+    def _block(self, fn, *count_types, args=()):
+        """(device pointer, counts...) of a device block: fn(ctx, *args, &ptr, &count...) with one count of each ctypes type"""
+        ptr = C.POINTER(C.c_double)()
+        counts = [t(0) for t in count_types]
+        self._check(fn(self._ctx, *args, C.byref(ptr), *(C.byref(c) for c in counts)))
+        return (C.cast(ptr, C.c_void_p).value, *(c.value for c in counts))
+
+    def _take_rows(self, ptr, n, dtype):
+        """a numpy copy of n library-allocated rows of dtype at ptr; the rows are freed (me_free) in every case"""
+        try:
+            addr = C.cast(ptr, C.c_void_p).value
+            nb = n * dtype.itemsize
+            return np.frombuffer((C.c_char * nb).from_address(addr), dtype).copy() if nb else np.zeros(0, dtype)
+        finally:
+            self._L.me_free(ptr)
+
     def set_stream(self, stream_ptr):
         self._check(self._L.me_set_stream(self._ctx, C.c_void_p(int(stream_ptr)) if stream_ptr else None))
 
@@ -407,10 +423,7 @@ class MapEvalB200:
 
     def icp_block(self):
         """(device pointer, n_sum) of this rank's partial ICP sums (SUM-all-reduce in place); the first call sweeps"""
-        ptr = C.POINTER(C.c_double)()
-        ns = C.c_int32(0)
-        self._check(self._L.me_icp_block(self._ctx, C.byref(ptr), C.byref(ns)))
-        return C.cast(ptr, C.c_void_p).value, ns.value
+        return self._block(self._L.me_icp_block, C.c_int32)
 
     def icp_step(self):
         """reads the reduced block, updates T, moves and sweeps again; True when the loop is over"""
@@ -559,10 +572,7 @@ class MapEvalB200:
     def curve_accum_device(self, tau):
         """(device pointer, n) of this rank's SUM-reducible curve block at the levels tau (me_nn_curve_accum_device)"""
         t, tp = _curve_levels(tau)
-        ptr = C.POINTER(C.c_double)()
-        n = C.c_int32(0)
-        self._check(self._L.me_nn_curve_accum_device(self._ctx, tp, t.size, C.byref(ptr), C.byref(n)))
-        return C.cast(ptr, C.c_void_p).value, n.value
+        return self._block(self._L.me_nn_curve_accum_device, C.c_int32, args=(tp, t.size))
 
     def distance_quantiles(self, p, population=A.ME_DIST_KEPT):
         """Exact quantiles at the probabilities p (1..ME_QUANTILE_MAX_PROBS values in [0, 1]) of the distances of the last NN
@@ -582,10 +592,7 @@ class MapEvalB200:
 
     def quantile_block(self):
         """(device pointer, n) of the running pass's SUM-reducible block (all-reduce it in place after synchronize())"""
-        ptr = C.POINTER(C.c_double)()
-        n = C.c_int32(0)
-        self._check(self._L.me_nn_quantile_block(self._ctx, C.byref(ptr), C.byref(n)))
-        return C.cast(ptr, C.c_void_p).value, n.value
+        return self._block(self._L.me_nn_quantile_block, C.c_int32)
 
     def quantile_step(self):
         """reads the reduced block and runs the next pass; True after the last one"""
@@ -606,13 +613,7 @@ class MapEvalB200:
         rows = C.POINTER(A.me_region_row)()
         n = C.c_int64(0)
         self._check(self._L.me_nn_regions(self._ctx, float(region_size), C.byref(rows), C.byref(n)))
-        try:
-            nb = n.value * _REGION_ROW_DT.itemsize
-            a = np.frombuffer((C.c_char * nb).from_address(C.addressof(rows.contents)), _REGION_ROW_DT) if nb else \
-                np.zeros(0, _REGION_ROW_DT)
-            return region_dict(a.copy())
-        finally:
-            self._L.me_free(rows)
+        return region_dict(self._take_rows(rows, n.value, _REGION_ROW_DT))
 
     def region_begin(self, region_size):
         """me_nn_region_begin: lists the occupied regions and folds this rank's records; returns the region count"""
@@ -623,10 +624,7 @@ class MapEvalB200:
     def region_block(self):
         """(device pointer, n_sum, n_max) of the block: SUM-reduce its first n_sum values and MAX-reduce the next n_max in place
         (after synchronize())"""
-        ptr = C.POINTER(C.c_double)()
-        n_sum, n_max = C.c_int32(0), C.c_int32(0)
-        self._check(self._L.me_nn_region_block(self._ctx, C.byref(ptr), C.byref(n_sum), C.byref(n_max)))
-        return C.cast(ptr, C.c_void_p).value, n_sum.value, n_max.value
+        return self._block(self._L.me_nn_region_block, C.c_int32, C.c_int32)
 
     def region_end(self, n_regions):
         """the rows from the reduced block, as region_errors"""
@@ -658,10 +656,7 @@ class MapEvalB200:
     def surface_block(self):
         """(device pointer, n_sum, n_max) of the block; the first call folds this rank's records.  SUM-reduce the first n_sum
         values and MAX-reduce the next n_max in place (after synchronize())"""
-        ptr = C.POINTER(C.c_double)()
-        n_sum, n_max = C.c_int32(0), C.c_int32(0)
-        self._check(self._L.me_nn_surface_block(self._ctx, C.byref(ptr), C.byref(n_sum), C.byref(n_max)))
-        return C.cast(ptr, C.c_void_p).value, n_sum.value, n_max.value
+        return self._block(self._L.me_nn_surface_block, C.c_int32, C.c_int32)
 
     def surface_end(self):
         """the result from the reduced block, as surface_metrics"""
@@ -680,13 +675,7 @@ class MapEvalB200:
         n = C.c_int64(0)
         self._check(self._L.me_drift(self._ctx, float(region_size), float(max_correspondence_distance), int(max_iteration),
                                      float(relative_fitness), float(relative_rmse), C.byref(rows), C.byref(n)))
-        try:
-            nb = n.value * _DRIFT_ROW_DT.itemsize
-            a = np.frombuffer((C.c_char * nb).from_address(C.addressof(rows.contents)), _DRIFT_ROW_DT) if nb else \
-                np.zeros(0, _DRIFT_ROW_DT)
-            return drift_dict(a.copy())
-        finally:
-            self._L.me_free(rows)
+        return drift_dict(self._take_rows(rows, n.value, _DRIFT_ROW_DT))
 
     def drift_begin(self, region_size, max_correspondence_distance, max_iteration=30, relative_fitness=1e-6,
                     relative_rmse=1e-6):
@@ -700,10 +689,7 @@ class MapEvalB200:
     def drift_block(self):
         """(device pointer, n_sum) of the block, ME_ICP_BLOCK_P2P values per region: SUM-reduce it in place (after
         synchronize())"""
-        ptr = C.POINTER(C.c_double)()
-        n_sum = C.c_int32(0)
-        self._check(self._L.me_drift_block(self._ctx, C.byref(ptr), C.byref(n_sum)))
-        return C.cast(ptr, C.c_void_p).value, n_sum.value
+        return self._block(self._L.me_drift_block, C.c_int32)
 
     def drift_step(self):
         """reads the reduced block, updates every running region, moves and sweeps again; True when every region is done"""
@@ -728,14 +714,7 @@ class MapEvalB200:
         whole = A.me_consistency_result()
         self._check(self._L.me_consistency(self._ctx, int(which), float(radius), int(min_neighbors), float(region_size),
                                            C.byref(rows), C.byref(n), C.byref(whole)))
-        try:
-            nb = n.value * _CONS_ROW_DT.itemsize
-            a = np.frombuffer((C.c_char * nb).from_address(rows.value), _CONS_ROW_DT).copy() if nb else \
-                np.zeros(0, _CONS_ROW_DT)
-            return consistency_dict(a, whole)
-        finally:
-            if rows.value:
-                self._L.me_free(rows)
+        return consistency_dict(self._take_rows(rows, n.value, _CONS_ROW_DT), whole)
 
     def consistency_begin(self, which, radius, min_neighbors=10, region_size=0.0):
         """me_consistency_begin: sweeps this rank's query range and folds it by region; returns the row count (0 at
@@ -748,10 +727,7 @@ class MapEvalB200:
     def consistency_block(self):
         """(device pointer, n_sum, n_max) of the block: SUM-reduce its first n_sum values and MAX-reduce the next n_max in
         place (after synchronize())"""
-        ptr = C.POINTER(C.c_double)()
-        n_sum, n_max = C.c_int32(0), C.c_int32(0)
-        self._check(self._L.me_consistency_block(self._ctx, C.byref(ptr), C.byref(n_sum), C.byref(n_max)))
-        return C.cast(ptr, C.c_void_p).value, n_sum.value, n_max.value
+        return self._block(self._L.me_consistency_block, C.c_int32, C.c_int32)
 
     def consistency_end(self, n_regions):
         """the rows and the whole-map result from the reduced block, as local_consistency"""
@@ -788,10 +764,7 @@ class MapEvalB200:
 
     def mom_block(self):
         """(device pointer, n) of the running pass's block: SUM-reduce it in place (after synchronize())"""
-        ptr = C.POINTER(C.c_double)()
-        n = C.c_int32(0)
-        self._check(self._L.me_mom_block(self._ctx, C.byref(ptr), C.byref(n)))
-        return C.cast(ptr, C.c_void_p).value, n.value
+        return self._block(self._L.me_mom_block, C.c_int32)
 
     def mom_step(self):
         """me_mom_step: reads the reduced block, runs the next pass; True after the last"""
@@ -826,14 +799,7 @@ class MapEvalB200:
         n = C.c_int64(0)
         self._check(self._L.me_mom_regions(self._ctx, float(region_size), self._mom_min_family(min_family), C.byref(rows),
                                            C.byref(n)))
-        try:
-            nb = n.value * _MOM_REGION_ROW_DT.itemsize
-            a = np.frombuffer((C.c_char * nb).from_address(rows.value), _MOM_REGION_ROW_DT).copy() if nb else \
-                np.zeros(0, _MOM_REGION_ROW_DT)
-            return mom_region_dict(a, region_size)
-        finally:
-            if rows.value:
-                self._L.me_free(rows)
+        return mom_region_dict(self._take_rows(rows, n.value, _MOM_REGION_ROW_DT), region_size)
 
     def _mom_min_family(self, min_family):
         if min_family is not None:
@@ -851,10 +817,7 @@ class MapEvalB200:
 
     def mom_region_block(self):
         """(device pointer, n) of the block [v | code], 2 n_points fp64 values: SUM-reduce it in place (after synchronize())"""
-        ptr = C.POINTER(C.c_double)()
-        n = C.c_int64(0)
-        self._check(self._L.me_mom_region_block(self._ctx, C.byref(ptr), C.byref(n)))
-        return C.cast(ptr, C.c_void_p).value, n.value
+        return self._block(self._L.me_mom_region_block, C.c_int64)
 
     def mom_region_end(self, n_regions):
         """the rows from the reduced block, as mom_regions"""
@@ -934,10 +897,7 @@ class MapEvalB200:
 
     def accum_block(self):
         """(device pointer, n_sum, n_max) of the fp64 accumulator block"""
-        ptr = C.POINTER(C.c_double)()
-        ns, nm = C.c_int32(0), C.c_int32(0)
-        self._check(self._L.me_accum_block(self._ctx, C.byref(ptr), C.byref(ns), C.byref(nm)))
-        return C.cast(ptr, C.c_void_p).value, ns.value, nm.value
+        return self._block(self._L.me_accum_block, C.c_int32, C.c_int32)
 
     def accum_fetch(self, want_mme=(True, False)):
         e, g = A.me_nn_accum(), A.me_nn_accum()
@@ -963,10 +923,7 @@ class MapEvalB200:
 
     def voxel_w_table(self):
         """(device pointer, n) of the W table over the estimated cloud's voxels (-1 = no pair)"""
-        ptr = C.POINTER(C.c_double)()
-        n = C.c_int64(0)
-        self._check(self._L.me_voxel_w_table(self._ctx, C.byref(ptr), C.byref(n)))
-        return C.cast(ptr, C.c_void_p).value, n.value
+        return self._block(self._L.me_voxel_w_table, C.c_int64)
 
     def voxel_finish_accum_device(self, scs_radius=5):
         self._check(self._L.me_voxel_finish_accum_device(self._ctx, int(scs_radius)))

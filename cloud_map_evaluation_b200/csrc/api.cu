@@ -663,6 +663,28 @@ static void decode_block(const double *h, me_nn_accum *est_to_gt, me_nn_accum *g
   }
 }
 
+// the tail of a one-shot call that hands the caller library-allocated rows (me_free): max(n, min_rows) rows (NULL when that
+// is 0), filled by end(rows) and freed when it fails.  close() leaves the context as a failed call must when the allocation
+// fails.
+template <class Row, class End, class Close>
+static int one_shot_rows(me_ctx *ctx, int64_t n, int64_t min_rows, const char *nomem, End end, Close close, Row **rows,
+                         int64_t *n_regions) {
+  Row *r = nullptr;
+  const int64_t cap = std::max(n, min_rows);
+  if (cap > 0 && !(r = (Row *)std::malloc((size_t)cap * sizeof(Row)))) {
+    close();
+    return fail(ctx, ME_ERR_NOMEM, nomem);
+  }
+  const int rc = end(r);
+  if (rc != ME_OK) {
+    std::free(r);
+    return rc;
+  }
+  *rows = r;
+  *n_regions = n;
+  return ME_OK;
+}
+
 extern "C" {
 
 __global__ void block_init_kernel(double *blk) {
@@ -1015,16 +1037,8 @@ int me_nn_regions(me_ctx *ctx, double region_size, me_region_row **rows, int64_t
     return fail(ctx, ME_ERR_INVALID, "me_nn_regions needs world == 1; use me_nn_region_begin / _block + all-reduce / _end");
   int64_t n = 0;
   ME_TRY(me_nn_region_begin(ctx, region_size, &n));
-  me_region_row *r = (me_region_row *)std::malloc((size_t)std::max<int64_t>(n, 1) * sizeof(me_region_row));
-  if (!r) return fail(ctx, ME_ERR_NOMEM, "me_nn_regions: host allocation of the rows failed");
-  const int rc = me_nn_region_end(ctx, r, n);
-  if (rc != ME_OK) {
-    std::free(r);
-    return rc;
-  }
-  *rows = r;
-  *n_regions = n;
-  return ME_OK;
+  return one_shot_rows(ctx, n, 1, "me_nn_regions: host allocation of the rows failed",
+                       [&](me_region_row *r) { return me_nn_region_end(ctx, r, n); }, [] {}, rows, n_regions);
 }
 
 int me_surface_finalize(const me_nn_params *p, const double *host_block, int64_t n_est, int64_t n_gt, me_surface_result *out) {
@@ -1170,22 +1184,9 @@ int me_consistency(me_ctx *ctx, int which, double radius, int32_t min_neighbors,
     return fail(ctx, ME_ERR_INVALID, "me_consistency needs world == 1; use me_consistency_begin / _block + all-reduce / _end");
   int64_t n = 0;
   ME_TRY(me_consistency_begin(ctx, which, radius, min_neighbors, region_size, &n));
-  me_consistency_row *r = nullptr;
-  if (n > 0) {
-    r = (me_consistency_row *)std::malloc((size_t)n * sizeof(me_consistency_row));
-    if (!r) {
-      ctx->consistency.open = false;
-      return fail(ctx, ME_ERR_NOMEM, "me_consistency: host allocation of the rows failed");
-    }
-  }
-  const int rc = me_consistency_end(ctx, r, n, whole);
-  if (rc != ME_OK) {
-    std::free(r);
-    return rc;
-  }
-  *rows = r;
-  *n_regions = n;
-  return ME_OK;
+  return one_shot_rows(ctx, n, 0, "me_consistency: host allocation of the rows failed",
+                       [&](me_consistency_row *r) { return me_consistency_end(ctx, r, n, whole); },
+                       [&] { ctx->consistency.open = false; }, rows, n_regions);
 }
 
 int me_get_consistency_points(me_ctx *ctx, int which, double *entropy, double *plane_variance) {
@@ -1277,19 +1278,9 @@ int me_mom_regions(me_ctx *ctx, double region_size, int64_t min_family, me_mom_r
     return fail(ctx, ME_ERR_INVALID, "me_mom_regions needs world == 1; use me_mom_region_begin / _block + all-reduce / _end");
   int64_t n = 0;
   ME_TRY(me_mom_region_begin(ctx, region_size, min_family, &n));
-  me_mom_region_row *r = (me_mom_region_row *)std::malloc((size_t)std::max<int64_t>(n, 1) * sizeof(me_mom_region_row));
-  if (!r) {
-    ctx->mom_region.open = false;
-    return fail(ctx, ME_ERR_NOMEM, "me_mom_regions: host allocation of the rows failed");
-  }
-  const int rc = me_mom_region_end(ctx, r, n);
-  if (rc != ME_OK) {
-    std::free(r);
-    return rc;
-  }
-  *rows = r;
-  *n_regions = n;
-  return ME_OK;
+  return one_shot_rows(ctx, n, 1, "me_mom_regions: host allocation of the rows failed",
+                       [&](me_mom_region_row *r) { return me_mom_region_end(ctx, r, n); },
+                       [&] { ctx->mom_region.open = false; }, rows, n_regions);
 }
 
 int me_drift_begin(me_ctx *ctx, double region_size, double max_correspondence_distance, int32_t max_iteration,
@@ -1338,20 +1329,9 @@ int me_drift(me_ctx *ctx, double region_size, double max_correspondence_distance
   ME_TRY(me_drift_begin(ctx, region_size, max_correspondence_distance, max_iteration, relative_fitness, relative_rmse, &n));
   int32_t done = 0;
   while (!done) ME_TRY(me_drift_step(ctx, &done));
-  me_drift_row *r = (me_drift_row *)std::malloc((size_t)std::max<int64_t>(n, 1) * sizeof(me_drift_row));
-  if (!r) {
-    drift_close(ctx, true);
-    ctx->cloud_gen++;
-    return fail(ctx, ME_ERR_NOMEM, "me_drift: host allocation of the rows failed");
-  }
-  const int rc = me_drift_end(ctx, r, n);
-  if (rc != ME_OK) {
-    std::free(r);
-    return rc;
-  }
-  *rows = r;
-  *n_regions = n;
-  return ME_OK;
+  return one_shot_rows(ctx, n, 1, "me_drift: host allocation of the rows failed",
+                       [&](me_drift_row *r) { return me_drift_end(ctx, r, n); },
+                       [&] { drift_close(ctx, true); ctx->cloud_gen++; }, rows, n_regions);
 }
 
 int me_eval_nn(me_ctx *ctx, const me_nn_params *p, me_nn_result *out) {

@@ -23,46 +23,75 @@ class _DeviceBlock:
         self.__cuda_array_interface__ = {"shape": (n,), "typestr": "<f8", "data": (int(ptr), False), "version": 2}
 
 
+def _world(group):
+    """(rank, world) of this process in the group; (0, 1) without torch.distributed"""
+    import torch.distributed as dist
+    if not dist.is_initialized():
+        return 0, 1
+    return dist.get_rank(group), dist.get_world_size(group)
+
+
+def _reduce(ctx, ptr, n_sum, n_max, device, group=None, sync=True):
+    """All-reduce a device block the context owns, in place: SUM over its first n_sum values (counts ride as fp64, exact),
+    MAX over the next n_max; on one rank there is nothing to reduce.  sync: the collectives wait for the context's stream
+    and torch's stream is synchronised after them; without it the caller orders both on one stream.  Returns the block as
+    a tensor (None when it is empty)."""
+    import torch
+    import torch.distributed as dist
+    if n_sum + n_max == 0:
+        return None
+    t = torch.as_tensor(_DeviceBlock(ptr, n_sum + n_max), device=device)
+    if _world(group)[1] == 1:
+        return t
+    if sync:
+        ctx.synchronize()
+    if n_sum > 0:
+        dist.all_reduce(t[:n_sum], group=group)
+    if n_max > 0:
+        dist.all_reduce(t[n_sum:], op=dist.ReduceOp.MAX, group=group)
+    if sync:
+        torch.cuda.current_stream(device).synchronize()
+    return t
+
+
+def _gather_normals(ctx, slice_fn, device, group=None):
+    """The all-gather of the working normals: for each cloud whose slices are pending (this rank filled rows
+    [rank * slice, (rank + 1) * slice) of the world * slice * 3 fp64 buffer), ONE in-place all-gather"""
+    import torch
+    import torch.distributed as dist
+    rank, world = _world(group)
+    for which in (A.ME_CLOUD_EST, A.ME_CLOUD_GT):
+        ptr, s, pending = slice_fn(which)
+        if pending:
+            ctx.synchronize()
+            buf = torch.as_tensor(_DeviceBlock(ptr, world * s * 3), device=device)
+            dist.all_gather_into_tensor(buf, buf[rank * s * 3:(rank + 1) * s * 3], group=group)
+            torch.cuda.current_stream(device).synchronize()
+
+
 def allreduce_block(ctx, device, group=None):
     """All-reduce the context's device-resident accumulator block in place: ONE SUM all-reduce over the sum-reducible
     values (counts ride as fp64, exact) and one MAX all-reduce over the entropy extrema — NCCL over NVLink / NVSwitch, no
-    host round trip; the caller fetches the block afterwards (MapEvalB200.accum_fetch)."""
-    import torch
-    import torch.distributed as dist
-    ptr, n_sum, n_max = ctx.accum_block()
-    t = torch.as_tensor(_DeviceBlock(ptr, n_sum + n_max), device=device)
-    dist.all_reduce(t[:n_sum], group=group)
-    dist.all_reduce(t[n_sum:], op=dist.ReduceOp.MAX, group=group)
+    host round trip (order the context's and torch's work on one stream); the caller fetches the block afterwards
+    (MapEvalB200.accum_fetch)."""
+    _reduce(ctx, *ctx.accum_block(), device, group, sync=False)
 
 
 def allreduce_curve(ctx, tau, device, group=None):
     """The accuracy curve block of every rank at the levels tau (MapEvalB200.curve_accum_device), SUM-all-reduced in place
     on the device (counts ride as fp64, exact), returned as a host numpy array for api.curve_finalize, which every rank
     then runs with its reduced NN accumulators."""
-    import torch
-    import torch.distributed as dist
     ptr, n = ctx.curve_accum_device(tau)
     ctx.synchronize()
-    t = torch.as_tensor(_DeviceBlock(ptr, n), device=device)
-    if dist.is_initialized() and dist.get_world_size(group) > 1:
-        dist.all_reduce(t, group=group)
-    return t.cpu().numpy().copy()
+    return _reduce(ctx, ptr, n, 0, device, group, sync=False).cpu().numpy().copy()
 
 
 def regions_distributed(ctx, region_size, device, group=None):
     """AC / COM / CD / F1 / IoU per region over every rank of the job (MapEvalB200.region_errors for world > 1): every rank
     lists the same occupied regions and folds its own records, then ONE in-place SUM all-reduce of the block's sums (counts
     ride as fp64, exact) and ONE MAX all-reduce of its maxima.  Every rank returns the same table."""
-    import torch
-    import torch.distributed as dist
     n = ctx.region_begin(region_size)
-    if dist.is_initialized() and dist.get_world_size(group) > 1:
-        ptr, n_sum, n_max = ctx.region_block()
-        ctx.synchronize()
-        t = torch.as_tensor(_DeviceBlock(ptr, n_sum + n_max), device=device)
-        dist.all_reduce(t[:n_sum], group=group)
-        dist.all_reduce(t[n_sum:], op=dist.ReduceOp.MAX, group=group)
-        torch.cuda.current_stream(device).synchronize()
+    _reduce(ctx, *ctx.region_block(), device, group)
     return ctx.region_end(n)
 
 
@@ -71,25 +100,9 @@ def surface_distributed(ctx, device, knn=0, group=None):
     every rank estimates its caller-index slice of a cloud's missing working normals, ONE in-place all-gather per such cloud,
     then every rank folds its own records, ONE in-place SUM all-reduce of the block's sums (counts ride as fp64, exact) and
     ONE MAX all-reduce of its maxima.  Every rank returns the same result."""
-    import torch
-    import torch.distributed as dist
-    world = dist.get_world_size(group) if dist.is_initialized() else 1
-    rank = dist.get_rank(group) if dist.is_initialized() else 0
     ctx.surface_begin(knn)
-    for which in (A.ME_CLOUD_EST, A.ME_CLOUD_GT):
-        ptr, s, pending = ctx.surface_normals_slice(which)
-        if pending:
-            ctx.synchronize()
-            buf = torch.as_tensor(_DeviceBlock(ptr, world * s * 3), device=device)
-            dist.all_gather_into_tensor(buf, buf[rank * s * 3:(rank + 1) * s * 3], group=group)
-            torch.cuda.current_stream(device).synchronize()
-    ptr, n_sum, n_max = ctx.surface_block()
-    if world > 1:
-        ctx.synchronize()
-        t = torch.as_tensor(_DeviceBlock(ptr, n_sum + n_max), device=device)
-        dist.all_reduce(t[:n_sum], group=group)
-        dist.all_reduce(t[n_sum:], op=dist.ReduceOp.MAX, group=group)
-        torch.cuda.current_stream(device).synchronize()
+    _gather_normals(ctx, ctx.surface_normals_slice, device, group)
+    _reduce(ctx, *ctx.surface_block(), device, group)
     return ctx.surface_end()
 
 
@@ -97,16 +110,8 @@ def consistency_distributed(ctx, device, which, radius, min_neighbors=10, region
     """Local map consistency over every rank of the job (MapEvalB200.local_consistency for world > 1): every rank sweeps its
     query range of the replicated cloud and folds it by region, then ONE in-place SUM all-reduce of the block's sums (counts
     ride as fp64, exact) and ONE MAX all-reduce of its maxima.  Every rank returns the same result."""
-    import torch
-    import torch.distributed as dist
     n = ctx.consistency_begin(which, radius, min_neighbors, region_size)
-    if dist.is_initialized() and dist.get_world_size(group) > 1:
-        ptr, n_sum, n_max = ctx.consistency_block()
-        ctx.synchronize()
-        t = torch.as_tensor(_DeviceBlock(ptr, n_sum + n_max), device=device)
-        dist.all_reduce(t[:n_sum], group=group)
-        dist.all_reduce(t[n_sum:], op=dist.ReduceOp.MAX, group=group)
-        torch.cuda.current_stream(device).synchronize()
+    _reduce(ctx, *ctx.consistency_block(), device, group)
     return ctx.consistency_end(n)
 
 
@@ -115,17 +120,10 @@ def mom_distributed(ctx, device, which, radius, min_neighbors=10, angle_deg=10.0
     query range of the replicated cloud, then ONE in-place SUM all-reduce per pass: the direction histogram, the family
     fold with the medians' first digit, then the selection's later digits (counts ride as fp64, exact).  Every rank
     returns the same result."""
-    import torch
-    import torch.distributed as dist
-    world = dist.get_world_size(group) if dist.is_initialized() else 1
     ctx.mom_begin(which, radius, min_neighbors, angle_deg, planarity, min_family)
     done = False
     while not done:
-        if world > 1:
-            ptr, n = ctx.mom_block()
-            ctx.synchronize()
-            dist.all_reduce(torch.as_tensor(_DeviceBlock(ptr, n), device=device), group=group)
-            torch.cuda.current_stream(device).synchronize()
+        _reduce(ctx, *ctx.mom_block(), 0, device, group)
         done = ctx.mom_step()
     return ctx.mom_end()
 
@@ -134,14 +132,8 @@ def mom_regions_distributed(ctx, device, region_size, min_family=None, group=Non
     """The last finished MOM call per region over every rank of the job (MapEvalB200.mom_regions for world > 1): every rank
     writes the points it swept into the block [v | code], ONE in-place SUM all-reduce gathers them exactly (x + 0 = x), and
     every rank runs the same segmented selection on the same bits, so every rank returns the same rows."""
-    import torch
-    import torch.distributed as dist
     n = ctx.mom_region_begin(region_size, min_family)
-    if dist.is_initialized() and dist.get_world_size(group) > 1:
-        ptr, m = ctx.mom_region_block()
-        ctx.synchronize()
-        dist.all_reduce(torch.as_tensor(_DeviceBlock(ptr, m), device=device), group=group)
-        torch.cuda.current_stream(device).synchronize()
+    _reduce(ctx, *ctx.mom_region_block(), 0, device, group)
     return ctx.mom_region_end(n)
 
 
@@ -149,17 +141,10 @@ def quantiles_distributed(ctx, device, p, population=A.ME_DIST_KEPT, group=None)
     """Exact distance quantiles of the last NN evaluation over every rank of the job (MapEvalB200.distance_quantiles for
     world > 1): the selection loop with ONE in-place SUM all-reduce of the pass's integer counts (as fp64, exact) per pass.
     Every rank reads the same reduced counts, so every rank returns the same result."""
-    import torch
-    import torch.distributed as dist
-    world = dist.get_world_size(group) if dist.is_initialized() else 1
     ctx.quantile_begin(p, population)
     done = False
     while not done:
-        if world > 1:
-            ptr, n = ctx.quantile_block()
-            ctx.synchronize()
-            dist.all_reduce(torch.as_tensor(_DeviceBlock(ptr, n), device=device), group=group)
-            torch.cuda.current_stream(device).synchronize()
+        _reduce(ctx, *ctx.quantile_block(), 0, device, group)
         done = ctx.quantile_step()
     return ctx.quantile_end()
 
@@ -171,34 +156,13 @@ def icp_distributed(ctx, device, max_correspondence_distance, T_init=None, max_i
     cloud, then ONE SUM all-reduce of the 17 / 29-value block per iteration; every rank applies the same update to the same
     reduced doubles, so T is identical everywhere.  Returns (T 4x4, me_icp_result) like performICPRegistration; the
     estimated cloud held by ctx is the original transformed by T."""
-    import torch
-    import torch.distributed as dist
-    world = dist.get_world_size(group) if dist.is_initialized() else 1
-    rank = dist.get_rank(group) if dist.is_initialized() else 0
-    assert (rank, world) == (ctx.rank, ctx.world), "the context's shard must be this process's rank in the group"
-
-    def _torch_waits_for_ctx():
-        ctx.synchronize()
-
-    def _ctx_waits_for_torch():
-        torch.cuda.current_stream(device).synchronize()
-
+    assert _world(group) == (ctx.rank, ctx.world), "the context's shard must be this process's rank in the group"
     ctx.icp_begin(max_correspondence_distance, T_init, max_iteration, relative_fitness, relative_rmse, method)
-    for which in (A.ME_CLOUD_EST, A.ME_CLOUD_GT):
-        ptr, s, pending = ctx.icp_normals_slice(which)
-        if pending:
-            _torch_waits_for_ctx()
-            buf = torch.as_tensor(_DeviceBlock(ptr, world * s * 3), device=device)
-            dist.all_gather_into_tensor(buf, buf[rank * s * 3:(rank + 1) * s * 3], group=group)
-            _ctx_waits_for_torch()
-    done = False
+    _gather_normals(ctx, ctx.icp_normals_slice, device, group)
     ptr, n_sum = ctx.icp_block()
-    blk = torch.as_tensor(_DeviceBlock(ptr, n_sum), device=device)
+    done = False
     while not done:
-        if world > 1:
-            _torch_waits_for_ctx()
-            dist.all_reduce(blk, group=group)
-            _ctx_waits_for_torch()
+        _reduce(ctx, ptr, n_sum, 0, device, group)
         done = ctx.icp_step()
     return ctx.icp_end()
 
@@ -209,18 +173,11 @@ def drift_distributed(ctx, device, region_size, max_correspondence_distance, max
     every rank lists the same regions and folds the pairs of its query range, then ONE in-place SUM all-reduce of the
     17-value block per region per iteration; every rank applies the same updates to the same reduced doubles, so every rank
     returns the same rows."""
-    import torch
-    import torch.distributed as dist
-    world = dist.get_world_size(group) if dist.is_initialized() else 1
     n = ctx.drift_begin(region_size, max_correspondence_distance, max_iteration, relative_fitness, relative_rmse)
     ptr, n_sum = ctx.drift_block()
-    blk = torch.as_tensor(_DeviceBlock(ptr, n_sum), device=device) if world > 1 and n_sum > 0 else None
     done = False
     while not done:
-        if blk is not None:
-            ctx.synchronize()
-            dist.all_reduce(blk, group=group)
-            torch.cuda.current_stream(device).synchronize()
+        _reduce(ctx, ptr, n_sum, 0, device, group)
         done = ctx.drift_step()
     return ctx.drift_end(n)
 
@@ -229,8 +186,5 @@ def allreduce_voxel_w(ctx, device, group=None):
     """Slab layout, between MapEvalB200.voxel_begin and voxel_finish_accum_device: MAX-all-reduce of the W table over the
     estimated cloud's voxels in place (-1 = no pair; every voxel has one owner), so that the SCS sweep of every rank sees
     the W of the neighbouring ranks' voxels."""
-    import torch
-    import torch.distributed as dist
     ptr, n = ctx.voxel_w_table()
-    if n > 0:
-        dist.all_reduce(torch.as_tensor(_DeviceBlock(ptr, n), device=device), op=dist.ReduceOp.MAX, group=group)
+    _reduce(ctx, ptr, 0, n, device, group, sync=False)

@@ -78,16 +78,34 @@ class GpuGroup {
     return ME_OK;
   }
 
-  // collectives on buffers the contexts own (the accumulator and ICP blocks, the normal slices), in place on the devices.  The caller has
-  // waited for the contexts' streams (me_synchronize); on return the result is complete on every device.
-  bool allreduce_device(const std::vector<double *> &ptr, size_t len, ncclRedOp_t op) {
-    const int n = size();
-    if (n == 1 || len == 0) return true;
-    ncclGroupStart();
-    for (int r = 0; r < n; ++r) ncclAllReduce(ptr[r], ptr[r], len, ncclDouble, op, comm_[r], stream_[r]);
-    if (ncclGroupEnd() != ncclSuccess) { err_ = "ncclAllReduce failed"; return false; }
-    return sync_streams();
+  // fn(ctx, &x) on every GPU and rank 0's x into *out: the done flag of a loop's step or the result of its end, which every
+  // rank computes from the same reduced blocks
+  template <class T> int each(int (*fn)(me_ctx *, T *), T *out) {
+    return for_each([&](int r, me_ctx *c) {
+      T x{};
+      const int rc = fn(c, &x);
+      if (r == 0) *out = x;
+      return rc;
+    });
   }
+
+  // one reduction of a block the contexts own: f(rank, ctx, &ptr, &n_sum, &n_max) fills it on every GPU (n_max stays 0 for a
+  // block without a MAX part; N is the count type of the block's C call), me_synchronize, then ONE grouped SUM all-reduce of
+  // its first n_sum values and a MAX all-reduce of the next n_max, in place.  On return the block is reduced on every device.
+  template <class N = int32_t, class F> bool reduce_block(const F &f) {
+    const int n = size();
+    std::vector<double *> ptr(n, nullptr), ptr_max(n, nullptr);
+    std::vector<N> n_sum(n, 0), n_max(n, 0);
+    if (for_each([&](int r, me_ctx *c) {
+          const int rc = f(r, c, &ptr[r], &n_sum[r], &n_max[r]);
+          if (rc != ME_OK) return rc;
+          ptr_max[r] = ptr[r] + n_sum[r];
+          return me_synchronize(c);
+        }) != ME_OK)
+      return false;
+    return allreduce_device(ptr, (size_t)n_sum[0], ncclSum) && allreduce_device(ptr_max, (size_t)n_max[0], ncclMax);
+  }
+
   // rank r contributes ptr[r] + r * per_rank (per_rank doubles); every ptr[r] holds all n slices afterwards
   bool allgather_device(const std::vector<double *> &ptr, size_t per_rank) {
     const int n = size();
@@ -98,36 +116,38 @@ class GpuGroup {
     return sync_streams();
   }
 
-  // the accuracy curve blocks the contexts hold (me_nn_curve_accum_device, after me_synchronize): ONE grouped SUM all-reduce
-  // in place, then rank 0's reduced block into `host` (its size = the block's length)
-  bool reduce_curve(const std::vector<double *> &ptr, std::vector<double> &host) {
-    if (!allreduce_device(ptr, host.size(), ncclSum)) return false;
+  // the accuracy curve at the K levels tau (me_nn_curve_accum_device on every GPU): ONE grouped SUM all-reduce of the blocks,
+  // then rank 0's reduced block into `host`
+  bool reduce_curve(const double *tau, int32_t K, std::vector<double> &host) {
+    double *blk0 = nullptr;
+    if (!reduce_block([&](int r, me_ctx *c, double **ptr, int32_t *n, int32_t *) {
+          const int rc = me_nn_curve_accum_device(c, tau, K, ptr, n);
+          if (r == 0 && rc == ME_OK) {
+            blk0 = *ptr;
+            host.resize((size_t)*n);
+          }
+          return rc;
+        }))
+      return false;
     if (cudaSetDevice(dev_[0]) != cudaSuccess ||
-        cudaMemcpy(host.data(), ptr[0], host.size() * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess) {
+        cudaMemcpy(host.data(), blk0, host.size() * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess) {
       err_ = "copying the accuracy curve block back failed";
       return false;
     }
     return true;
   }
 
-  // one metric stage over every GPU: on each, me_accum_reset, the stage's *_device sweep(s) `sweep`, me_synchronize; then ONE
-  // grouped SUM all-reduce of the accumulator block's n_sum values and a MAX all-reduce of its n_max values, in place; then
-  // rank 0's reduced block into the structs (any may be NULL).  The reset keeps values of earlier stages out of the sums.
+  // one metric stage over every GPU: on each, me_accum_reset and the stage's *_device sweep(s) `sweep`, then the accumulator
+  // block reduced (reduce_block) and rank 0's reduced block into the structs (any may be NULL).  The reset keeps values of
+  // earlier stages out of the sums.
   bool reduce_accum(const std::function<int(me_ctx *)> &sweep, me_nn_accum *e2g, me_nn_accum *g2e, me_mme_accum *mme_est,
                     me_mme_accum *mme_gt) {
-    const int n = size();
-    std::vector<double *> blk(n, nullptr), blk_max(n, nullptr);
-    std::vector<int32_t> n_sum(n, 0), n_max(n, 0);
-    if (for_each([&](int r, me_ctx *c) {
+    if (!reduce_block([&](int, me_ctx *c, double **ptr, int32_t *n_sum, int32_t *n_max) {
           int rc = me_accum_reset(c);
           if (rc == ME_OK) rc = sweep(c);
-          if (rc == ME_OK) rc = me_synchronize(c);
-          if (rc == ME_OK) rc = me_accum_block(c, &blk[r], &n_sum[r], &n_max[r]);
-          blk_max[r] = blk[r] + n_sum[r];
-          return rc;
-        }) != ME_OK)
+          return rc != ME_OK ? rc : me_accum_block(c, ptr, n_sum, n_max);
+        }))
       return false;
-    if (!allreduce_device(blk, (size_t)n_sum[0], ncclSum) || !allreduce_device(blk_max, (size_t)n_max[0], ncclMax)) return false;
     if (me_accum_fetch(ctx_[0], e2g, g2e, mme_est, mme_gt) != ME_OK) { err_ = me_last_error(ctx_[0]); return false; }
     return true;
   }
@@ -140,6 +160,16 @@ class GpuGroup {
   }
 
  private:
+  // collectives on buffers the contexts own, in place on the devices.  The caller has waited for the contexts' streams
+  // (me_synchronize); on return the result is complete on every device.
+  bool allreduce_device(const std::vector<double *> &ptr, size_t len, ncclRedOp_t op) {
+    const int n = size();
+    if (n == 1 || len == 0) return true;
+    ncclGroupStart();
+    for (int r = 0; r < n; ++r) ncclAllReduce(ptr[r], ptr[r], len, ncclDouble, op, comm_[r], stream_[r]);
+    if (ncclGroupEnd() != ncclSuccess) { err_ = "ncclAllReduce failed"; return false; }
+    return sync_streams();
+  }
   bool sync_streams() {
     for (int r = 0; r < size(); ++r) {
       cudaSetDevice(dev_[r]);

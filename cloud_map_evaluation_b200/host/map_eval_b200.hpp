@@ -746,15 +746,8 @@ inline int MapEvalB200::accuracyCurve(const me_nn_params &p, const me_nn_accum &
   const int K = param_.accuracy_curve_steps_;
   std::vector<double> tau(K);
   for (int k = 1; k <= K; ++k) tau[k - 1] = (param_.accuracy_curve_max_ * (double)k) / (double)K;
-  std::vector<double *> ptr(gpus_.size(), nullptr);
-  std::vector<int32_t> len(gpus_.size(), 0);
-  if (gpus_.for_each([&](int r, me_ctx *c) {
-        const int rc = me_nn_curve_accum_device(c, tau.data(), K, &ptr[r], &len[r]);
-        return rc != ME_OK ? rc : me_synchronize(c);
-      }) != ME_OK)
-    return fail("me_nn_curve_accum_device");
-  std::vector<double> blk((size_t)len[0]);
-  if (!gpus_.reduce_curve(ptr, blk)) return fail("all-reduce of the accuracy curve");
+  std::vector<double> blk;
+  if (!gpus_.reduce_curve(tau.data(), K, blk)) return fail("me_nn_curve_accum_device / all-reduce of the accuracy curve");
   std::vector<me_curve_row> rows(K);
   if (me_nn_curve_finalize(&p, &e2g, &g2e, blk.data(), tau.data(), K, n_est_, n_gt_, rows.data()) != ME_OK)
     return fail("me_nn_curve_finalize");
@@ -785,25 +778,12 @@ inline int MapEvalB200::distanceQuantiles() {
   for (int pop : {ME_DIST_KEPT, ME_DIST_NN}) {
     if (gpus_.for_each([&](int, me_ctx *c) { return me_nn_quantile_begin(c, pop, pr.data(), K); }) != ME_OK)
       return fail("me_nn_quantile_begin");
-    for (bool done = false; !done;) {
-      std::vector<double *> ptr(gpus_.size(), nullptr);
-      std::vector<int32_t> len(gpus_.size(), 0), flag(gpus_.size(), 0);
-      if (gpus_.for_each([&](int r, me_ctx *c) {
-            const int rc = me_nn_quantile_block(c, &ptr[r], &len[r]);
-            return rc != ME_OK ? rc : me_synchronize(c);
-          }) != ME_OK)
-        return fail("me_nn_quantile_block");
-      if (!gpus_.allreduce_device(ptr, (size_t)len[0], ncclSum)) return fail("all-reduce of the distance quantile counts");
-      if (gpus_.for_each([&](int r, me_ctx *c) { return me_nn_quantile_step(c, &flag[r]); }) != ME_OK) return fail("me_nn_quantile_step");
-      done = flag[0] != 0;
+    for (int32_t done = 0; !done;) {
+      if (!gpus_.reduce_block([](int, me_ctx *c, double **ptr, int32_t *n, int32_t *) { return me_nn_quantile_block(c, ptr, n); }))
+        return fail("me_nn_quantile_block / all-reduce of the distance quantile counts");
+      if (gpus_.each(me_nn_quantile_step, &done) != ME_OK) return fail("me_nn_quantile_step");
     }
-    if (gpus_.for_each([&](int r, me_ctx *c) {
-          me_quantile_result mine;
-          const int rc = me_nn_quantile_end(c, &mine);
-          if (r == 0) res[pop] = mine;
-          return rc;
-        }) != ME_OK)
-      return fail("me_nn_quantile_end");
+    if (gpus_.each(me_nn_quantile_end, &res[pop]) != ME_OK) return fail("me_nn_quantile_end");
   }
   const std::string path = results_subfolder + "distance_quantiles.txt";
   std::ofstream f(path);
@@ -833,17 +813,11 @@ inline int MapEvalB200::distanceQuantiles() {
 inline int MapEvalB200::regionErrors() {
   const double s = param_.region_size_;
   std::vector<int64_t> n(gpus_.size(), 0);
-  std::vector<double *> ptr(gpus_.size(), nullptr), ptr_max(gpus_.size(), nullptr);
-  std::vector<int32_t> n_sum(gpus_.size(), 0), n_max(gpus_.size(), 0);
-  if (gpus_.for_each([&](int r, me_ctx *c) {
-        int rc = me_nn_region_begin(c, s, &n[r]);
-        if (rc == ME_OK) rc = me_nn_region_block(c, &ptr[r], &n_sum[r], &n_max[r]);
-        ptr_max[r] = ptr[r] + n_sum[r];
-        return rc != ME_OK ? rc : me_synchronize(c);
-      }) != ME_OK)
-    return fail("me_nn_region_begin");
-  if (!gpus_.allreduce_device(ptr, (size_t)n_sum[0], ncclSum) || !gpus_.allreduce_device(ptr_max, (size_t)n_max[0], ncclMax))
-    return fail("all-reduce of the region block");
+  if (!gpus_.reduce_block([&](int r, me_ctx *c, double **ptr, int32_t *n_sum, int32_t *n_max) {
+        const int rc = me_nn_region_begin(c, s, &n[r]);
+        return rc != ME_OK ? rc : me_nn_region_block(c, ptr, n_sum, n_max);
+      }))
+    return fail("me_nn_region_begin / all-reduce of the region block");
   std::vector<me_region_row> rows((size_t)n[0]);
   if (me_nn_region_end(ctx_, rows.data(), n[0]) != ME_OK) return fail("me_nn_region_end");
   const std::string path = results_subfolder + "region_errors.txt";
@@ -896,17 +870,11 @@ inline int MapEvalB200::localConsistency() {
   if (gt_mme()) runs.push_back(Run{ME_CLOUD_GT, 5, "gt", me_consistency_result{}, {}});
   for (Run &run : runs) {
     std::vector<int64_t> n(gpus_.size(), 0);
-    std::vector<double *> ptr(gpus_.size(), nullptr), ptr_max(gpus_.size(), nullptr);
-    std::vector<int32_t> n_sum(gpus_.size(), 0), n_max(gpus_.size(), 0);
-    if (gpus_.for_each([&](int g, me_ctx *c) {
-          int rc = me_consistency_begin(c, run.which, r, run.m, s, &n[g]);
-          if (rc == ME_OK) rc = me_consistency_block(c, &ptr[g], &n_sum[g], &n_max[g]);
-          ptr_max[g] = ptr[g] + n_sum[g];
-          return rc != ME_OK ? rc : me_synchronize(c);
-        }) != ME_OK)
-      return fail("me_consistency_begin");
-    if (!gpus_.allreduce_device(ptr, (size_t)n_sum[0], ncclSum) || !gpus_.allreduce_device(ptr_max, (size_t)n_max[0], ncclMax))
-      return fail("all-reduce of the consistency block");
+    if (!gpus_.reduce_block([&](int g, me_ctx *c, double **ptr, int32_t *n_sum, int32_t *n_max) {
+          const int rc = me_consistency_begin(c, run.which, r, run.m, s, &n[g]);
+          return rc != ME_OK ? rc : me_consistency_block(c, ptr, n_sum, n_max);
+        }))
+      return fail("me_consistency_begin / all-reduce of the consistency block");
     run.rows.resize((size_t)n[0]);
     if (me_consistency_end(ctx_, run.rows.data(), n[0], &run.whole) != ME_OK) return fail("me_consistency_end");
   }
@@ -962,34 +930,21 @@ inline int MapEvalB200::mom() {
   runs.push_back(Run{ME_CLOUD_EST, 10, "est", me_mom_result{}, {}});
   if (gt_mme()) runs.push_back(Run{ME_CLOUD_GT, 5, "gt", me_mom_result{}, {}});
   for (Run &run : runs) {
-    std::vector<double *> ptr(gpus_.size(), nullptr);
-    std::vector<int32_t> n(gpus_.size(), 0), done(gpus_.size(), 0);
     if (gpus_.for_each([&](int, me_ctx *c) { return me_mom_begin(c, run.which, r, run.m, &p); }) != ME_OK) return fail("me_mom_begin");
-    while (!done[0]) {
-      if (gpus_.for_each([&](int g, me_ctx *c) {
-            const int rc = me_mom_block(c, &ptr[g], &n[g]);
-            return rc != ME_OK ? rc : me_synchronize(c);
-          }) != ME_OK)
-        return fail("me_mom_block");
-      if (!gpus_.allreduce_device(ptr, (size_t)n[0], ncclSum)) return fail("all-reduce of the MOM block");
-      if (gpus_.for_each([&](int g, me_ctx *c) { return me_mom_step(c, &done[g]); }) != ME_OK) return fail("me_mom_step");
+    for (int32_t done = 0; !done;) {
+      if (!gpus_.reduce_block([](int, me_ctx *c, double **ptr, int32_t *n, int32_t *) { return me_mom_block(c, ptr, n); }))
+        return fail("me_mom_block / all-reduce of the MOM block");
+      if (gpus_.each(me_mom_step, &done) != ME_OK) return fail("me_mom_step");
     }
-    if (s <= 0.0) {
-      if (me_mom_end(ctx_, &run.res) != ME_OK) return fail("me_mom_end");
-      continue;
-    }
-    // per region: every GPU ends its MOM call and writes its points into the block, ONE grouped SUM all-reduce
-    std::vector<int64_t> n_regions(gpus_.size(), 0), len(gpus_.size(), 0);
-    std::vector<me_mom_result> res(gpus_.size());
-    if (gpus_.for_each([&](int g, me_ctx *c) {
-          int rc = me_mom_end(c, &res[g]);
-          if (rc == ME_OK) rc = me_mom_region_begin(c, s, p.min_family, &n_regions[g]);
-          if (rc == ME_OK) rc = me_mom_region_block(c, &ptr[g], &len[g]);
-          return rc != ME_OK ? rc : me_synchronize(c);
-        }) != ME_OK)
-      return fail("me_mom_region_begin");
-    run.res = res[0];
-    if (!gpus_.allreduce_device(ptr, (size_t)len[0], ncclSum)) return fail("all-reduce of the MOM region block");
+    if (gpus_.each(me_mom_end, &run.res) != ME_OK) return fail("me_mom_end");
+    if (s <= 0.0) continue;
+    // per region: every GPU writes its points into the block, ONE grouped SUM all-reduce
+    std::vector<int64_t> n_regions(gpus_.size(), 0);
+    if (!gpus_.reduce_block<int64_t>([&](int g, me_ctx *c, double **ptr, int64_t *n, int64_t *) {
+          const int rc = me_mom_region_begin(c, s, p.min_family, &n_regions[g]);
+          return rc != ME_OK ? rc : me_mom_region_block(c, ptr, n);
+        }))
+      return fail("me_mom_region_begin / all-reduce of the MOM region block");
     run.rows.resize((size_t)n_regions[0]);
     if (me_mom_region_end(ctx_, run.rows.data(), n_regions[0]) != ME_OK) return fail("me_mom_region_end");
   }
@@ -1128,24 +1083,12 @@ inline int MapEvalB200::surfaceMetrics() {
       return fail("me_nn_surface_normals_slice");
     if (pend[0] && !gpus_.allgather_device(nrm, (size_t)s[0] * 3)) return fail("all-gather of the working normals");
   }
-  std::vector<double *> ptr(G, nullptr), ptr_max(G, nullptr);
-  std::vector<int32_t> n_sum(G, 0), n_max(G, 0);
-  if (gpus_.for_each([&](int r, me_ctx *c) {
-        const int rc = me_nn_surface_block(c, &ptr[r], &n_sum[r], &n_max[r]);
-        ptr_max[r] = ptr[r] + n_sum[r];
-        return rc != ME_OK ? rc : me_synchronize(c);
-      }) != ME_OK)
-    return fail("me_nn_surface_block");
-  if (!gpus_.allreduce_device(ptr, (size_t)n_sum[0], ncclSum) || !gpus_.allreduce_device(ptr_max, (size_t)n_max[0], ncclMax))
-    return fail("all-reduce of the surface block");
+  if (!gpus_.reduce_block([](int, me_ctx *c, double **ptr, int32_t *n_sum, int32_t *n_max) {
+        return me_nn_surface_block(c, ptr, n_sum, n_max);
+      }))
+    return fail("me_nn_surface_block / all-reduce of the surface block");
   me_surface_result res;
-  if (gpus_.for_each([&](int r, me_ctx *c) {
-        me_surface_result mine;
-        const int rc = me_nn_surface_end(c, &mine);
-        if (r == 0) res = mine;
-        return rc;
-      }) != ME_OK)
-    return fail("me_nn_surface_end");
+  if (gpus_.each(me_nn_surface_end, &res) != ME_OK) return fail("me_nn_surface_end");
   const std::string path = results_subfolder + "surface_metrics.txt";
   std::ofstream f(path);
   if (!f.is_open()) {
@@ -1189,21 +1132,12 @@ inline int MapEvalB200::regionDrift() {
   const double s = param_.drift_region_size_;
   const int G = gpus_.size();
   std::vector<int64_t> n(G, 0);
-  std::vector<double *> ptr(G, nullptr);
-  std::vector<int32_t> n_sum(G, 0), done(G, 0);
-  if (gpus_.for_each([&](int r, me_ctx *c) {
-        int rc = me_drift_begin(c, s, param_.icp_max_distance_, 30, 1e-6, 1e-6, &n[r]);
-        if (rc == ME_OK) rc = me_drift_block(c, &ptr[r], &n_sum[r]);
-        return rc != ME_OK ? rc : me_synchronize(c);
-      }) != ME_OK)
+  if (gpus_.for_each([&](int r, me_ctx *c) { return me_drift_begin(c, s, param_.icp_max_distance_, 30, 1e-6, 1e-6, &n[r]); }) != ME_OK)
     return fail("me_drift_begin");
-  while (!done[0]) {
-    if (!gpus_.allreduce_device(ptr, (size_t)n_sum[0], ncclSum)) return fail("all-reduce of the drift block");
-    if (gpus_.for_each([&](int r, me_ctx *c) {
-          const int rc = me_drift_step(c, &done[r]);
-          return rc != ME_OK ? rc : me_synchronize(c);
-        }) != ME_OK)
-      return fail("me_drift_step");
+  for (int32_t done = 0; !done;) {
+    if (!gpus_.reduce_block([](int, me_ctx *c, double **ptr, int32_t *n_sum, int32_t *) { return me_drift_block(c, ptr, n_sum); }))
+      return fail("me_drift_block / all-reduce of the drift block");
+    if (gpus_.each(me_drift_step, &done) != ME_OK) return fail("me_drift_step");
   }
   std::vector<std::vector<me_drift_row>> rows(G, std::vector<me_drift_row>((size_t)std::max<int64_t>(n[0], 1)));
   if (gpus_.for_each([&](int r, me_ctx *c) { return me_drift_end(c, rows[r].data(), n[0]); }) != ME_OK) return fail("me_drift_end");
@@ -1288,8 +1222,7 @@ inline int MapEvalB200::performRegistration() {
     const int n = gpus_.size();
     std::vector<double *> ptr(n, nullptr);
     std::vector<int64_t> slice(n, 0);
-    std::vector<int32_t> pending(n, 0), n_sum(n, 0), done(n, 0);
-    std::vector<me_icp_result> res(n);
+    std::vector<int32_t> pending(n, 0);
     if (gpus_.for_each([&](int, me_ctx *c) {
           return me_icp_begin(c, param_.evaluation_method_, param_.icp_max_distance_, 30, 1e-6, 1e-6, param_.initial_matrix_);
         }) != ME_OK)
@@ -1302,21 +1235,12 @@ inline int MapEvalB200::performRegistration() {
         return fail("me_icp_normals_slice");
       if (pending[0] && !gpus_.allgather_device(ptr, (size_t)slice[0] * 3)) return fail("all-gather of the normals");
     }
-    if (gpus_.for_each([&](int r, me_ctx *c) {
-          const int rc = me_icp_block(c, &ptr[r], &n_sum[r]);
-          return rc != ME_OK ? rc : me_synchronize(c);
-        }) != ME_OK)
-      return fail("me_icp_block");
-    while (!done[0]) {
-      if (!gpus_.allreduce_device(ptr, (size_t)n_sum[0], ncclSum)) return fail("all-reduce of the ICP block");
-      if (gpus_.for_each([&](int r, me_ctx *c) {
-            const int rc = me_icp_step(c, &done[r]);
-            return rc != ME_OK ? rc : me_synchronize(c);
-          }) != ME_OK)
-        return fail("me_icp_step");
+    for (int32_t done = 0; !done;) {      // the first me_icp_block sweeps
+      if (!gpus_.reduce_block([](int, me_ctx *c, double **blk, int32_t *n_sum, int32_t *) { return me_icp_block(c, blk, n_sum); }))
+        return fail("me_icp_block / all-reduce of the ICP block");
+      if (gpus_.each(me_icp_step, &done) != ME_OK) return fail("me_icp_step");
     }
-    if (gpus_.for_each([&](int r, me_ctx *c) { return me_icp_end(c, &res[r]); }) != ME_OK) return fail("me_icp_end");
-    reg = res[0];
+    if (gpus_.each(me_icp_end, &reg) != ME_OK) return fail("me_icp_end");
   }
   t4 = tic_toc.toc();
   std::cout << "INFO: ICP registration time: " << (t4 - t3) / 1000.0 << " [s]" << std::endl;
