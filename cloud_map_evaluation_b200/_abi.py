@@ -272,6 +272,19 @@ class me_awd_result(C.Structure):
                 ("n_old", C.c_int64), ("n_new", C.c_int64)]
 
 
+ME_W2_ROW_COLS = 26
+ME_W2_BLOCK = 8
+# the columns of a me_eval_w2 row (sigma as xx xy xz yy yz zz)
+W2_ROW_COLUMNS = ("vmin_x", "vmin_y", "vmin_z", "n_gt", "n_est", "mu_est_x", "mu_est_y", "mu_est_z", "mu_gt_x", "mu_gt_y",
+                  "mu_gt_z", "sig_est_xx", "sig_est_xy", "sig_est_xz", "sig_est_yy", "sig_est_yz", "sig_est_zz", "sig_gt_xx",
+                  "sig_gt_xy", "sig_gt_xz", "sig_gt_yy", "sig_gt_yz", "sig_gt_zz", "offset", "shape", "w2")
+
+
+class me_w2_result(C.Structure):
+    _fields_ = [("aw2", C.c_double), ("mean_offset", C.c_double), ("mean_shape", C.c_double), ("scs", C.c_double),
+                ("n_pairs", C.c_int64), ("n_scs", C.c_int64), ("n_voxels_est", C.c_int64), ("n_voxels_gt", C.c_int64)]
+
+
 class me_icp_result(C.Structure):
     _fields_ = [("transformation", C.c_double * 16), ("fitness", C.c_double), ("inlier_rmse", C.c_double),
                 ("n_corr", C.c_int64), ("iterations", C.c_int32), ("converged", C.c_int32)]

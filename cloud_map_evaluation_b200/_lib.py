@@ -17,7 +17,8 @@ SYMBOLS = (
     "me_set_cloud", "me_set_cloud_device", "me_transform", "me_voxel_downsample", "me_get_cloud", "me_icp_point_to_point", "me_icp",
     "me_set_normals", "me_estimate_normals", "me_get_normals", "me_build_grid", "me_eval_nn_accum", "me_nn_finalize",
     "me_eval_nn", "me_get_nn", "me_eval_mme_accum", "me_mme_finalize", "me_eval_mme", "me_get_entropies",
-    "me_eval_awd", "me_awd_from_rows", "me_free", "me_get_stage_times", "me_launch_count",
+    "me_eval_awd", "me_awd_from_rows", "me_free",
+    "me_eval_w2", "me_w2_from_rows", "me_w2_begin", "me_w2_w_table", "me_w2_finish_accum_device", "me_w2_block", "me_w2_fetch", "me_get_stage_times", "me_launch_count",
     "me_accum_reset", "me_eval_nn_accum_device", "me_eval_mme_accum_device", "me_accum_block", "me_accum_fetch",
     "me_set_layout", "me_layout_active", "me_voxel_begin", "me_voxel_w_table", "me_voxel_finish_accum_device", "me_accum_fetch_awd",
     "me_plan_slab_cut", "me_plan_lattice", "me_kernel_trace",
@@ -117,6 +118,13 @@ def load():
     L.me_voxel_w_table.argtypes = [ctx, C.POINTER(dp), C.POINTER(C.c_int64)]
     L.me_voxel_finish_accum_device.argtypes = [ctx, C.c_int32]
     L.me_accum_fetch_awd.argtypes = [ctx, C.POINTER(A.me_awd_result)]
+    L.me_eval_w2.argtypes = [ctx, C.c_double, C.c_int32, C.c_int32, C.POINTER(A.me_w2_result), C.POINTER(C.c_int64), C.POINTER(dp)]
+    L.me_w2_from_rows.argtypes = [ctx, dp, C.c_int64, C.c_double, C.c_int32, dp, C.POINTER(A.me_w2_result)]
+    L.me_w2_begin.argtypes = [ctx, C.c_double, C.c_int32]
+    L.me_w2_w_table.argtypes = [ctx, C.POINTER(dp), C.POINTER(C.c_int64)]
+    L.me_w2_finish_accum_device.argtypes = [ctx, C.c_int32]
+    L.me_w2_block.argtypes = [ctx, C.POINTER(dp), C.POINTER(C.c_int32)]
+    L.me_w2_fetch.argtypes = [ctx, C.POINTER(A.me_w2_result)]
     L.me_free.argtypes = [C.c_void_p]
     L.me_free.restype = None
     L.me_get_stage_times.argtypes = [ctx, dp]

@@ -885,6 +885,50 @@ class MapEvalB200:
                                              w.ctypes.data_as(dp), C.byref(out)))
         return out, w
 
+    # -- the Gaussian 2-Wasserstein distance per voxel (DESIGN §3.18) -------------------------------------------------
+    def voxel_w2(self, voxel_size, min_points=100, scs_radius=5, want_rows=False):
+        """AW2, the mean offset and shape terms, SCS over W2 and the counts (me_w2_result); with want_rows also the
+        (n_pairs, 26) rows, columns _abi.W2_ROW_COLUMNS.  Replicated layout (dist.w2_distributed shards it)."""
+        out = A.me_w2_result()
+        n_rows = C.c_int64(0)
+        rows_p = C.POINTER(C.c_double)()
+        self._check(self._L.me_eval_w2(self._ctx, float(voxel_size), int(min_points), int(scs_radius), C.byref(out),
+                                       C.byref(n_rows), C.byref(rows_p) if want_rows else None))
+        if not want_rows:
+            return out
+        rows = self._take_rows(rows_p, n_rows.value * A.ME_W2_ROW_COLS, np.dtype(np.float64))
+        return out, rows.reshape(-1, A.ME_W2_ROW_COLS)
+
+    def w2_from_rows(self, rows, voxel_size, scs_radius=5):
+        """(me_w2_result, (n, 3) offset / shape / W2 per row) of given Gaussians in the 26-column layout of voxel_w2's rows"""
+        rows = np.ascontiguousarray(rows, dtype=np.float64)
+        assert rows.ndim == 2 and rows.shape[1] == A.ME_W2_ROW_COLS
+        out = A.me_w2_result()
+        w = np.empty((rows.shape[0], 3), np.float64)
+        dp = C.POINTER(C.c_double)
+        self._check(self._L.me_w2_from_rows(self._ctx, rows.ctypes.data_as(dp), rows.shape[0], float(voxel_size), int(scs_radius),
+                                            w.ctypes.data_as(dp), C.byref(out)))
+        return out, w
+
+    def w2_begin(self, voxel_size, min_points=100):
+        self._check(self._L.me_w2_begin(self._ctx, float(voxel_size), int(min_points)))
+
+    def w2_w_table(self):
+        """(device pointer, n) of the W2 table over the estimated cloud's voxels (-1 = no pair on a slab layout)"""
+        return self._block(self._L.me_w2_w_table, C.c_int64)
+
+    def w2_finish_accum_device(self, scs_radius=5):
+        self._check(self._L.me_w2_finish_accum_device(self._ctx, int(scs_radius)))
+
+    def w2_block(self):
+        """(device pointer, n) of the stage's block: SUM-reduce all n values in place"""
+        return self._block(self._L.me_w2_block, C.c_int32)
+
+    def w2_fetch(self):
+        out = A.me_w2_result()
+        self._check(self._L.me_w2_fetch(self._ctx, C.byref(out)))
+        return out
+
     # -- device-resident accumulators (multi-GPU passes without host round trips) ---------------------------------
     def accum_reset(self):
         self._check(self._L.me_accum_reset(self._ctx))

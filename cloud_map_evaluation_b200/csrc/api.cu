@@ -252,6 +252,7 @@ void me_destroy(me_ctx *ctx) {
   stage_pool_free(ctx);
   if (ctx->d_scratch) cudaFree(ctx->d_scratch);
   if (ctx->d_block) cudaFree(ctx->d_block);
+  if (ctx->d_w2) cudaFree(ctx->d_w2);
   if (ctx->d_trace) cudaFree(ctx->d_trace);
   if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
   if (ctx->d_work) cudaFree(ctx->d_work);
@@ -1395,6 +1396,48 @@ int me_eval_awd(me_ctx *ctx, double voxel_size, int32_t min_points, int32_t scs_
   ME_ENTER(ctx);
   if (!out) return fail(ctx, ME_ERR_INVALID, "null result");
   return run_awd(ctx, voxel_size, min_points, scs_radius, out, n_rows, rows27);
+}
+
+int me_eval_w2(me_ctx *ctx, double voxel_size, int32_t min_points, int32_t scs_radius, me_w2_result *out, int64_t *n_rows,
+               double **rows) {
+  ME_ENTER(ctx);
+  if (!out) return fail(ctx, ME_ERR_INVALID, "null result");
+  return run_w2(ctx, voxel_size, min_points, scs_radius, out, n_rows, rows);
+}
+
+int me_w2_from_rows(me_ctx *ctx, const double *rows, int64_t n_rows, double voxel_size, int32_t scs_radius, double *w_out,
+                    me_w2_result *out) {
+  ME_ENTER(ctx);
+  if (!out) return fail(ctx, ME_ERR_INVALID, "null result");
+  return run_w2_rows(ctx, rows, n_rows, voxel_size, scs_radius, w_out, out);
+}
+
+int me_w2_begin(me_ctx *ctx, double voxel_size, int32_t min_points) {
+  ME_ENTER(ctx);
+  return w2_begin(ctx, voxel_size, min_points);
+}
+
+int me_w2_w_table(me_ctx *ctx, double **device_w, int64_t *n) {
+  ME_ENTER(ctx);
+  if (!device_w || !n) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return w2_w_table(ctx, device_w, n);
+}
+
+int me_w2_finish_accum_device(me_ctx *ctx, int32_t scs_radius) {
+  ME_ENTER(ctx);
+  return w2_finish_block(ctx, scs_radius);
+}
+
+int me_w2_block(me_ctx *ctx, double **device_block, int32_t *n) {
+  ME_ENTER(ctx);
+  if (!device_block || !n) return fail(ctx, ME_ERR_INVALID, "null argument");
+  return w2_block(ctx, device_block, n);
+}
+
+int me_w2_fetch(me_ctx *ctx, me_w2_result *out) {
+  ME_ENTER(ctx);
+  if (!out) return fail(ctx, ME_ERR_INVALID, "null result");
+  return w2_fetch(ctx, out);
 }
 
 int me_awd_from_rows(me_ctx *ctx, const double *rows27, int64_t n_rows, double voxel_size, int32_t scs_radius, double *w_out,

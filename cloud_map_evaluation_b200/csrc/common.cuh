@@ -466,6 +466,9 @@ struct me_ctx {
   bool vox_open = false;
   long long vox_nvox = 0;
   size_t vox_o_w = 0, vox_o_pairs = 0;
+  // the W2 stage (me_w2_begin .. me_w2_fetch) keeps its tables in the same work buffer, so at most one of the two is open
+  bool w2_open = false, w2_finished = false;
+  void *d_w2 = nullptr;             // its accumulators and block (voxel.cu W2Dev), allocated on first use
   // lattice spec shared by both clouds, so that their cells coincide (same v, m; integer index offsets)
   double spec_v = 0.0;
   int spec_m = 0;
@@ -707,6 +710,15 @@ void slab_cut(const unsigned long long *planes_y, int n_planes_y, const unsigned
 int voxel_begin(me_ctx *ctx, double voxel_size, int min_points);
 int voxel_w_table(me_ctx *ctx, double **d_w, int64_t *n);
 int voxel_finish_block(me_ctx *ctx, int scs_radius);
+// the Gaussian 2-Wasserstein stage (voxel.cu; ME_W2_BLOCK values in me_ctx::d_w2)
+int run_w2(me_ctx *ctx, double voxel_size, int min_points, int scs_radius, me_w2_result *out, int64_t *n_rows, double **rows);
+int run_w2_rows(me_ctx *ctx, const double *rows, int64_t n_rows, double voxel_size, int scs_radius, double *w_out,
+                me_w2_result *out);
+int w2_begin(me_ctx *ctx, double voxel_size, int min_points);
+int w2_w_table(me_ctx *ctx, double **d_w, int64_t *n);
+int w2_finish_block(me_ctx *ctx, int scs_radius);
+int w2_block(me_ctx *ctx, double **d_block, int32_t *n);
+int w2_fetch(me_ctx *ctx, me_w2_result *out);
 int transform_cloud(me_ctx *ctx, int which, const double T[16]);
 int run_icp(me_ctx *ctx, int method, double max_dist, int max_iter, double rel_fitness, double rel_rmse, const double T_init[16],
             me_icp_result *out);

@@ -14,6 +14,7 @@
 // (mu = c + S1/n, M2 = S2 - S1 S1^T / n), which equals the Welford result to rounding.
 #include "common.cuh"
 #include "eig3.cuh"
+#include "svd3.cuh"
 #include <algorithm>
 #include <cstring>
 #include <cstdlib>
@@ -344,8 +345,21 @@ static Owned voxel_owned(const Cloud &c) {
   return o;
 }
 
-static int voxel_begin_impl(me_ctx *ctx, double voxel_size, int min_points, bool want_rows, double **d_rows_out) {
+// The part of the stage both voxel metrics (AWD and W2) share: lattices aligned with the voxel size and the work layout
+// cnt_e | cnt_g | mom_e | mom_g | w_vox | pair_list | rows (row_cols fp64 per pair when want_rows).  Both stages keep their
+// tables in this one work buffer, so laying it out closes whichever of them was open.
+struct VoxelTables {
+  Lattice Le, Lg;
+  bool slab;
+  int32_t *cnt_e, *cnt_g;
+  double *mom_e, *mom_g, *w_vox, *rows;
+  uint32_t *pair_list;
+  size_t o_w, o_pairs;
+};
+
+static int voxel_layout(me_ctx *ctx, double voxel_size, int min_points, int row_cols, bool want_rows, VoxelTables &t) {
   ctx->vox_open = false;
+  ctx->w2_open = false;
   if (!(voxel_size > 0)) return fail(ctx, ME_ERR_INVALID, "vmd_voxel_size must be > 0");
   if (ctx->cloud[0].n <= 0 || ctx->cloud[1].n <= 0) return fail(ctx, ME_ERR_EMPTY, "both clouds must be set");
   // the lattices must be aligned with this voxel size; rebuild them if they are not
@@ -363,7 +377,6 @@ static int voxel_begin_impl(me_ctx *ctx, double voxel_size, int min_points, bool
   if (slab && want_rows)
     return fail(ctx, ME_ERR_INVALID, "the per-voxel rows are not available on a slab layout (every rank holds its own voxels only)");
 
-  // work layout: cnt_e | cnt_g | mom_e | mom_g | w_vox | pair_list | rows27
   auto align = [](size_t x) { return (x + 255) & ~(size_t)255; };
   size_t o_cnt_e = 0;
   size_t o_cnt_g = o_cnt_e + align((size_t)Le.nvoxels * sizeof(int32_t));
@@ -374,52 +387,66 @@ static int voxel_begin_impl(me_ctx *ctx, double voxel_size, int min_points, bool
   size_t o_rows = o_pairs + align((size_t)Le.nvoxels * sizeof(uint32_t));
   // a voxel pair needs >= min_points points in each cloud, which bounds the number of rows
   long long max_pairs = std::min<long long>(Le.nvoxels, std::min(E.n, G.n) / std::max(1, min_points) + 1);
-  size_t total = o_rows + (want_rows ? align((size_t)max_pairs * 27 * sizeof(double)) : 0);
+  size_t total = o_rows + (want_rows ? align((size_t)max_pairs * row_cols * sizeof(double)) : 0);
   ME_TRY(ensure_work(ctx, total));
   char *base = (char *)ctx->d_work;
-  int32_t *cnt_e = (int32_t *)(base + o_cnt_e), *cnt_g = (int32_t *)(base + o_cnt_g);
-  double *mom_e = (double *)(base + o_mom_e), *mom_g = (double *)(base + o_mom_g);
-  double *w_vox = (double *)(base + o_w);
-  uint32_t *pair_list = (uint32_t *)(base + o_pairs);
-  double *d_rows = want_rows ? (double *)(base + o_rows) : nullptr;
-  if (d_rows_out) *d_rows_out = d_rows;
+  t.Le = Le; t.Lg = Lg; t.slab = slab;
+  t.cnt_e = (int32_t *)(base + o_cnt_e); t.cnt_g = (int32_t *)(base + o_cnt_g);
+  t.mom_e = (double *)(base + o_mom_e); t.mom_g = (double *)(base + o_mom_g);
+  t.w_vox = (double *)(base + o_w);
+  t.pair_list = (uint32_t *)(base + o_pairs);
+  t.rows = want_rows ? (double *)(base + o_rows) : nullptr;
+  t.o_w = o_w; t.o_pairs = o_pairs;
+  return ME_OK;
+}
 
+// the per-voxel moments of both clouds into the tables; occ[0], occ[1]: the occupied voxels of est and gt (zeroed by the caller)
+static int voxel_moments(me_ctx *ctx, const VoxelTables &t, unsigned long long *occ) {
+  Cloud &E = ctx->cloud[ME_CLOUD_EST], &G = ctx->cloud[ME_CLOUD_GT];
+  const Lattice &Le = t.Le, &Lg = t.Lg;
+  StageTimer timer(ctx, 6);
+  int blocks_e = (int)std::min<long long>((Le.nvoxels * 16 + kThreads - 1) / kThreads, (long long)ctx->sm_count * 8);
+  const int pb_e = (int)std::min<long long>((E.n + kThreads - 1) / kThreads, (long long)ctx->sm_count * 16);
+  const int pb_g = (int)std::min<long long>((G.n + kThreads - 1) / kThreads, (long long)ctx->sm_count * 16);
+  if (Le.sparse) {
+    ME_CUDA(ctx, cudaMemsetAsync(t.cnt_e, 0, (size_t)Le.nvoxels * sizeof(int32_t), ctx->stream));
+    voxel_precount_kernel<<<pb_e, kThreads, 0, ctx->stream>>>(E.d_sorted, E.d_rel, E.ns, index_of(E), Le, t.cnt_e);
+    ME_LAUNCH_CHECK(ctx);
+  }
+  if (Lg.sparse) {
+    ME_CUDA(ctx, cudaMemsetAsync(t.cnt_g, 0, (size_t)Lg.nvoxels * sizeof(int32_t), ctx->stream));
+    voxel_precount_kernel<<<pb_g, kThreads, 0, ctx->stream>>>(G.d_sorted, G.d_rel, G.ns, index_of(G), Lg, t.cnt_g);
+    ME_LAUNCH_CHECK(ctx);
+  }
+  voxel_moments_kernel<<<std::max(1, blocks_e), kThreads, 0, ctx->stream>>>(E.d_sorted, index_of(E), Le, Le.sparse, voxel_owned(E), t.cnt_e, t.mom_e, occ);
+  ME_LAUNCH_CHECK(ctx);
+  int blocks_g = (int)std::min<long long>((Lg.nvoxels * 16 + kThreads - 1) / kThreads, (long long)ctx->sm_count * 8);
+  voxel_moments_kernel<<<std::max(1, blocks_g), kThreads, 0, ctx->stream>>>(G.d_sorted, index_of(G), Lg, Lg.sparse, voxel_owned(G), t.cnt_g, t.mom_g, occ + 1);
+  ME_LAUNCH_CHECK(ctx);
+  return ME_OK;
+}
+
+static int voxel_begin_impl(me_ctx *ctx, double voxel_size, int min_points, bool want_rows, double **d_rows_out) {
+  VoxelTables t;
+  ME_TRY(voxel_layout(ctx, voxel_size, min_points, 27, want_rows, t));
+  if (d_rows_out) *d_rows_out = t.rows;
   AwdAcc *acc = (AwdAcc *)ctx->d_scratch;
   unsigned long long *occ = (unsigned long long *)((char *)ctx->d_scratch + 256);
   zero_awd_acc_kernel<<<1, 1, 0, ctx->stream>>>(acc, occ);
   ME_LAUNCH_CHECK(ctx);
-  {
-    StageTimer timer(ctx, 6);
-    int blocks_e = (int)std::min<long long>((Le.nvoxels * 16 + kThreads - 1) / kThreads, (long long)ctx->sm_count * 8);
-    const int pb_e = (int)std::min<long long>((E.n + kThreads - 1) / kThreads, (long long)ctx->sm_count * 16);
-    const int pb_g = (int)std::min<long long>((G.n + kThreads - 1) / kThreads, (long long)ctx->sm_count * 16);
-    if (Le.sparse) {
-      ME_CUDA(ctx, cudaMemsetAsync(cnt_e, 0, (size_t)Le.nvoxels * sizeof(int32_t), ctx->stream));
-      voxel_precount_kernel<<<pb_e, kThreads, 0, ctx->stream>>>(E.d_sorted, E.d_rel, E.ns, index_of(E), Le, cnt_e);
-      ME_LAUNCH_CHECK(ctx);
-    }
-    if (Lg.sparse) {
-      ME_CUDA(ctx, cudaMemsetAsync(cnt_g, 0, (size_t)Lg.nvoxels * sizeof(int32_t), ctx->stream));
-      voxel_precount_kernel<<<pb_g, kThreads, 0, ctx->stream>>>(G.d_sorted, G.d_rel, G.ns, index_of(G), Lg, cnt_g);
-      ME_LAUNCH_CHECK(ctx);
-    }
-    voxel_moments_kernel<<<std::max(1, blocks_e), kThreads, 0, ctx->stream>>>(E.d_sorted, index_of(E), Le, Le.sparse, voxel_owned(E), cnt_e, mom_e, occ);
-    ME_LAUNCH_CHECK(ctx);
-    int blocks_g = (int)std::min<long long>((Lg.nvoxels * 16 + kThreads - 1) / kThreads, (long long)ctx->sm_count * 8);
-    voxel_moments_kernel<<<std::max(1, blocks_g), kThreads, 0, ctx->stream>>>(G.d_sorted, index_of(G), Lg, Lg.sparse, voxel_owned(G), cnt_g, mom_g, occ + 1);
-    ME_LAUNCH_CHECK(ctx);
-  }
+  ME_TRY(voxel_moments(ctx, t, occ));
   {
     StageTimer timer(ctx, 7);
+    const Lattice Le = t.Le;
     int blocks = (int)std::min<long long>((Le.nvoxels + kThreads - 1) / kThreads, (long long)ctx->sm_count * 8);
-    awd_kernel<<<std::max(1, blocks), kThreads, 0, ctx->stream>>>(Le, Lg, cnt_e, mom_e, cnt_g, mom_g, min_points, slab ? -1.0 : (double)NAN,
-                                                                 w_vox, pair_list, d_rows, acc);
+    awd_kernel<<<std::max(1, blocks), kThreads, 0, ctx->stream>>>(t.Le, t.Lg, t.cnt_e, t.mom_e, t.cnt_g, t.mom_g, min_points,
+                                                                 t.slab ? -1.0 : (double)NAN, t.w_vox, t.pair_list, t.rows, acc);
     ME_LAUNCH_CHECK(ctx);
   }
   ctx->vox_open = true;
-  ctx->vox_nvox = Le.nvoxels;
-  ctx->vox_o_w = o_w;
-  ctx->vox_o_pairs = o_pairs;
+  ctx->vox_nvox = t.Le.nvoxels;
+  ctx->vox_o_w = t.o_w;
+  ctx->vox_o_pairs = t.o_pairs;
   return ME_OK;
 }
 
@@ -543,6 +570,7 @@ int run_awd_rows(me_ctx *ctx, const double *rows27, int64_t n_rows, double voxel
   std::memset(out, 0, sizeof(*out));
   if (n_rows <= 0 || !rows27 || !(voxel_size > 0)) return fail(ctx, ME_ERR_INVALID, "bad arguments");
   if (scs_radius < 0 || scs_radius > 64) return fail(ctx, ME_ERR_INVALID, "scs_radius out of range");
+  ctx->w2_open = false;      // the W2 stage's tables share the work buffer
   // voxel keys = vmin / v (columns 0-2), dense index inside their bounding box
   std::vector<long long> key(3 * (size_t)n_rows), vox((size_t)n_rows);
   long long lo[3] = {LLONG_MAX, LLONG_MAX, LLONG_MAX}, hi[3] = {LLONG_MIN, LLONG_MIN, LLONG_MIN};
@@ -593,6 +621,365 @@ int run_awd_rows(me_ctx *ctx, const double *rows27, int64_t n_rows, double voxel
   out->awd = h->sum_w / (double)n_rows;
   out->scs = h->sum_scs / (double)h->n_scs;
   return ME_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// The Gaussian 2-Wasserstein distance per voxel pair (DESIGN §3.18): mu, Sigma = M2 / (n - 1), offset o = |mu_est - mu_gt|,
+// shape b = Bures(Sigma_gt, Sigma_est), W2 = sqrt(o^2 + b^2).  b^2 = tr Sigma_gt + tr Sigma_est - 2 tr((A Sigma_est A)^1/2)
+// (A = Sigma_gt^1/2, B = Sigma_est^1/2) subtracts nearly equal numbers; it is also min over orthogonal U of |A - B U|_F^2,
+// reached at U = P Q^T for the SVD B A = P S Q^T, and that residual is a sum of squares in which nothing cancels.
+// ---------------------------------------------------------------------------------------------------------------
+struct W2Acc {            // scs_kernel reads and updates the AwdAcc in front (n_active / n_new stay 0)
+  AwdAcc a;
+  double sum_offset, sum_shape;
+};
+struct W2Dev {            // me_ctx::d_w2
+  W2Acc acc;
+  unsigned long long occ[2];
+  double blk[ME_W2_BLOCK];
+};
+
+// Sigma^1/2 of a symmetric 3x3 (row-major), eigenvalues clamped at 0
+__device__ void sqrt_psd(const double *sig, double *r) {
+  double w[3], v[9];
+  eig3_jacobi(sig, w, v);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) w[k] = sqrt(fmax(w[k], 0.0));
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) r[i * 3 + j] = v[i * 3] * w[0] * v[j * 3] + v[i * 3 + 1] * w[1] * v[j * 3 + 1] + v[i * 3 + 2] * w[2] * v[j * 3 + 2];
+}
+
+// offset and shape terms of (mu_g, Sigma_g) against (mu_e, Sigma_e); symmetric in the two up to rounding
+__device__ void w2_terms(const double *mu_g, const double *sig_g, const double *mu_e, const double *sig_e, double &o, double &b) {
+  const double d0 = mu_e[0] - mu_g[0], d1 = mu_e[1] - mu_g[1], d2 = mu_e[2] - mu_g[2];
+  o = sqrt(d0 * d0 + d1 * d1 + d2 * d2);
+  double A[9], B[9], M[9], P[9], s[3], Q[9], R[9];
+  sqrt_psd(sig_g, A);
+  sqrt_psd(sig_e, B);
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) M[i * 3 + j] = B[i * 3] * A[j] + B[i * 3 + 1] * A[3 + j] + B[i * 3 + 2] * A[6 + j];
+  svd3(M, P, s, Q);
+  if (!(s[0] > 0.0)) {
+    // B A = 0: tr(A B U) = 0 for every U, so U = I reaches the minimum
+#pragma unroll
+    for (int i = 0; i < 9; ++i) R[i] = (i % 4 == 0) ? 1.0 : 0.0;
+  } else {
+    if (!(s[1] > 0.0)) {
+      // rank 1: svd3 leaves P's second column 0; any unit vector orthogonal to the first serves (s_2 = s_3 = 0)
+      const double ax = fabs(P[0]), ay = fabs(P[3]), az = fabs(P[6]);
+      const int k = (ax <= ay && ax <= az) ? 0 : (ay <= az ? 1 : 2);
+      double e[3] = {0.0, 0.0, 0.0};
+      e[k] = 1.0;
+      const double pk = P[k * 3];
+      double n2 = 0.0;
+#pragma unroll
+      for (int i = 0; i < 3; ++i) { P[i * 3 + 1] = e[i] - pk * P[i * 3]; n2 += P[i * 3 + 1] * P[i * 3 + 1]; }
+      const double inv = 1.0 / sqrt(n2);
+#pragma unroll
+      for (int i = 0; i < 3; ++i) P[i * 3 + 1] *= inv;
+    }
+    // the third column: orthogonal to the first two, with the sign for which P S Q^T = B A, i.e. p3 . (B A q3) >= 0 (when
+    // s_3 = 0 both signs give the same residual)
+    P[2] = P[3] * P[7] - P[6] * P[4]; P[5] = P[6] * P[1] - P[0] * P[7]; P[8] = P[0] * P[4] - P[3] * P[1];
+    double dot = 0.0;
+#pragma unroll
+    for (int i = 0; i < 3; ++i) dot += P[i * 3 + 2] * (M[i * 3] * Q[2] + M[i * 3 + 1] * Q[5] + M[i * 3 + 2] * Q[8]);
+    if (dot < 0.0) { P[2] = -P[2]; P[5] = -P[5]; P[8] = -P[8]; }
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+      for (int j = 0; j < 3; ++j) R[i * 3 + j] = P[i * 3] * Q[j * 3] + P[i * 3 + 1] * Q[j * 3 + 1] + P[i * 3 + 2] * Q[j * 3 + 2];
+  }
+  double ss = 0.0;
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      const double r = A[i * 3 + j] - (B[i * 3] * R[j] + B[i * 3 + 1] * R[3 + j] + B[i * 3 + 2] * R[6 + j]);
+      ss += r * r;
+    }
+  b = sqrt(ss);
+}
+
+// mu and the unbiased covariance M2 / (n - 1) (xx xy xz yy yz zz) of a voxel from its moments about the centre c
+__device__ void unbiased_gaussian(const double *mom, int n, double cx, double cy, double cz, double *mu, double *sig6) {
+  const double nd = (double)n, nm1 = (double)(n - 1);
+  mu[0] = cx + mom[0] / nd; mu[1] = cy + mom[1] / nd; mu[2] = cz + mom[2] / nd;
+  sig6[0] = (mom[3] - mom[0] * mom[0] / nd) / nm1; sig6[1] = (mom[4] - mom[0] * mom[1] / nd) / nm1;
+  sig6[2] = (mom[5] - mom[0] * mom[2] / nd) / nm1; sig6[3] = (mom[6] - mom[1] * mom[1] / nd) / nm1;
+  sig6[4] = (mom[7] - mom[1] * mom[2] / nd) / nm1; sig6[5] = (mom[8] - mom[2] * mom[2] / nd) / nm1;
+}
+
+__device__ inline void sym9(const double *t, double *s) {
+  s[0] = t[0]; s[1] = t[1]; s[2] = t[2]; s[3] = t[1]; s[4] = t[3]; s[5] = t[4]; s[6] = t[2]; s[7] = t[4]; s[8] = t[5];
+}
+
+// one pair's terms into the accumulators and, when asked, its row (ME_W2_ROW_COLS columns)
+__device__ double w2_pair(const double *mu_e, const double *sig6_e, const double *mu_g, const double *sig6_g, W2Acc *acc,
+                          double *row) {
+  double se[9], sg[9], o, b;
+  sym9(sig6_e, se);
+  sym9(sig6_g, sg);
+  w2_terms(mu_g, sg, mu_e, se, o, b);
+  const double w = sqrt(o * o + b * b);
+  atomicAdd(&acc->a.sum_w, w);
+  atomicAdd(&acc->sum_offset, o);
+  atomicAdd(&acc->sum_shape, b);
+  if (row) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) { row[5 + k] = mu_e[k]; row[8 + k] = mu_g[k]; }
+#pragma unroll
+    for (int k = 0; k < 6; ++k) { row[11 + k] = sig6_e[k]; row[17 + k] = sig6_g[k]; }
+    row[23] = o; row[24] = b; row[25] = w;
+  }
+  return w;
+}
+
+// pairing as awd_kernel: one thread per est voxel
+__global__ void __launch_bounds__(kThreads)
+w2_kernel(Lattice Le, Lattice Lg, const int32_t *__restrict__ cnt_e, const double *__restrict__ mom_e,
+          const int32_t *__restrict__ cnt_g, const double *__restrict__ mom_g, int min_points, double missing,
+          double *__restrict__ w_out, uint32_t *__restrict__ pair_list, double *__restrict__ rows, W2Acc *__restrict__ acc) {
+  for (long long vox = blockIdx.x * (long long)blockDim.x + threadIdx.x; vox < Le.nvoxels;
+       vox += (long long)gridDim.x * blockDim.x) {
+    double w = missing;      // NaN, or -1 when the table is MAX-all-reduced across ranks (slab layout)
+    const int ne = cnt_e[vox];
+    if (ne >= min_points) {
+      const int vx = (int)(vox % Le.nvox[0]);
+      const int vy = (int)((vox / Le.nvox[0]) % Le.nvox[1]);
+      const int vz = (int)(vox / ((long long)Le.nvox[0] * Le.nvox[1]));
+      const long long kx = (long long)Le.k_lo[0] + vx, ky = (long long)Le.k_lo[1] + vy, kz = (long long)Le.k_lo[2] + vz;
+      const long long gx = kx - Lg.k_lo[0], gy = ky - Lg.k_lo[1], gz = kz - Lg.k_lo[2];
+      int ng = 0;
+      long long gvox = -1;
+      if (gx >= 0 && gx < Lg.nvox[0] && gy >= 0 && gy < Lg.nvox[1] && gz >= 0 && gz < Lg.nvox[2]) {
+        gvox = (gz * Lg.nvox[1] + gy) * (long long)Lg.nvox[0] + gx;
+        ng = cnt_g[gvox];
+      }
+      if (ng >= min_points) {
+        const double cx = ((double)kx + 0.5) * Le.v, cy = ((double)ky + 0.5) * Le.v, cz = ((double)kz + 0.5) * Le.v;
+        double mu_e[3], sig_e[6], mu_g[3], sig_g[6];
+        unbiased_gaussian(mom_e + vox * 9, ne, cx, cy, cz, mu_e, sig_e);
+        unbiased_gaussian(mom_g + gvox * 9, ng, cx, cy, cz, mu_g, sig_g);
+        const unsigned long long slot = atomicAdd(&acc->a.n_pairs, 1ull);
+        pair_list[slot] = (uint32_t)vox;
+        double *r = rows ? rows + slot * ME_W2_ROW_COLS : nullptr;
+        if (r) {
+          r[0] = (double)kx * Le.v; r[1] = (double)ky * Le.v; r[2] = (double)kz * Le.v;
+          r[3] = (double)ng; r[4] = (double)ne;
+        }
+        w = w2_pair(mu_e, sig_e, mu_g, sig_g, acc, r);
+      }
+    }
+    w_out[vox] = w;
+  }
+}
+
+// the eight SUM-reducible values of the stage -> its block
+__global__ void pack_w2_kernel(W2Dev *d) {
+  if (threadIdx.x != 0) return;
+  const W2Acc &a = d->acc;
+  double *blk = d->blk;
+  blk[0] = (double)a.a.n_pairs; blk[1] = (double)a.a.n_scs; blk[2] = (double)d->occ[0]; blk[3] = (double)d->occ[1];
+  blk[4] = a.a.sum_w; blk[5] = a.a.sum_scs; blk[6] = a.sum_offset; blk[7] = a.sum_shape;
+}
+
+static int w2_state(me_ctx *ctx, W2Dev **d) {
+  if (!ctx->d_w2) {
+    const cudaError_t e = cudaMalloc(&ctx->d_w2, sizeof(W2Dev));
+    if (e != cudaSuccess) {
+      ctx->d_w2 = nullptr;
+      cudaGetLastError();
+      return fail(ctx, ME_ERR_NOMEM, std::string("cudaMalloc of the W2 accumulators: ") + cudaGetErrorString(e));
+    }
+  }
+  *d = (W2Dev *)ctx->d_w2;
+  ME_CUDA(ctx, cudaMemsetAsync(*d, 0, sizeof(W2Dev), ctx->stream));
+  return ME_OK;
+}
+
+static int w2_begin_impl(me_ctx *ctx, double voxel_size, int min_points, bool want_rows, double **d_rows_out) {
+  ctx->w2_finished = false;
+  if (min_points < 2) return fail(ctx, ME_ERR_INVALID, "W2: min_points must be >= 2 (the unbiased covariance divides by n - 1)");
+  VoxelTables t;
+  ME_TRY(voxel_layout(ctx, voxel_size, min_points, ME_W2_ROW_COLS, want_rows, t));
+  if (d_rows_out) *d_rows_out = t.rows;
+  W2Dev *d = nullptr;
+  ME_TRY(w2_state(ctx, &d));
+  ME_TRY(voxel_moments(ctx, t, d->occ));
+  int blocks = (int)std::min<long long>((t.Le.nvoxels + kThreads - 1) / kThreads, (long long)ctx->sm_count * 8);
+  w2_kernel<<<std::max(1, blocks), kThreads, 0, ctx->stream>>>(t.Le, t.Lg, t.cnt_e, t.mom_e, t.cnt_g, t.mom_g, min_points,
+                                                              t.slab ? -1.0 : (double)NAN, t.w_vox, t.pair_list, t.rows, &d->acc);
+  ME_LAUNCH_CHECK(ctx);
+  ctx->w2_open = true;
+  ctx->vox_nvox = t.Le.nvoxels;
+  ctx->vox_o_w = t.o_w;
+  ctx->vox_o_pairs = t.o_pairs;
+  return ME_OK;
+}
+
+static int launch_scs(me_ctx *ctx, const Lattice &L, const double *w_vox, const uint32_t *pair_list, int scs_radius, AwdAcc *acc) {
+  if (scs_radius == 5) scs_kernel<5><<<ctx->sm_count * 4, kThreads, 0, ctx->stream>>>(L, w_vox, pair_list, scs_radius, acc);
+  else scs_kernel<0><<<ctx->sm_count * 4, kThreads, 0, ctx->stream>>>(L, w_vox, pair_list, scs_radius, acc);
+  ME_LAUNCH_CHECK(ctx);
+  trace_scs(ctx, scs_radius);
+  return ME_OK;
+}
+
+int w2_begin(me_ctx *ctx, double voxel_size, int min_points) { return w2_begin_impl(ctx, voxel_size, min_points, false, nullptr); }
+
+int w2_w_table(me_ctx *ctx, double **d_w, int64_t *n) {
+  if (!ctx->w2_open) return fail(ctx, ME_ERR_INVALID, "me_w2_w_table before me_w2_begin");
+  *d_w = (double *)((char *)ctx->d_work + ctx->vox_o_w);
+  *n = (int64_t)ctx->vox_nvox;
+  return ME_OK;
+}
+
+int w2_finish_block(me_ctx *ctx, int scs_radius) {
+  if (!ctx->w2_open) return fail(ctx, ME_ERR_INVALID, "me_w2_finish_accum_device before me_w2_begin");
+  if (scs_radius < 0 || scs_radius > 64) return fail(ctx, ME_ERR_INVALID, "scs_radius out of range");
+  ctx->w2_open = false;
+  W2Dev *d = (W2Dev *)ctx->d_w2;
+  ME_TRY(launch_scs(ctx, ctx->cloud[ME_CLOUD_EST].lat, (const double *)((char *)ctx->d_work + ctx->vox_o_w),
+                    (const uint32_t *)((char *)ctx->d_work + ctx->vox_o_pairs), scs_radius, &d->acc.a));
+  pack_w2_kernel<<<1, 32, 0, ctx->stream>>>(d);
+  ME_LAUNCH_CHECK(ctx);
+  ctx->w2_finished = true;
+  return ME_OK;
+}
+
+int w2_block(me_ctx *ctx, double **d_block, int32_t *n) {
+  if (!ctx->w2_finished) return fail(ctx, ME_ERR_INVALID, "me_w2_block before me_w2_finish_accum_device");
+  *d_block = ((W2Dev *)ctx->d_w2)->blk;
+  *n = ME_W2_BLOCK;
+  return ME_OK;
+}
+
+static void w2_result(const double v[ME_W2_BLOCK], me_w2_result *out) {
+  auto i64 = [](double x) { return (int64_t)std::llround(x); };
+  std::memset(out, 0, sizeof(*out));
+  out->n_pairs = i64(v[0]); out->n_scs = i64(v[1]);
+  out->n_voxels_est = i64(v[2]); out->n_voxels_gt = i64(v[3]);
+  out->aw2 = v[4] / (double)out->n_pairs;           // 0/0 -> NaN
+  out->scs = v[5] / (double)out->n_scs;
+  out->mean_offset = v[6] / (double)out->n_pairs;
+  out->mean_shape = v[7] / (double)out->n_pairs;
+}
+
+int w2_fetch(me_ctx *ctx, me_w2_result *out) {
+  std::memset(out, 0, sizeof(*out));
+  if (!ctx->w2_finished) return fail(ctx, ME_ERR_INVALID, "me_w2_fetch before me_w2_finish_accum_device");
+  double *h = (double *)ctx->h_pinned;
+  ME_CUDA(ctx, cudaMemcpyAsync(h, ((W2Dev *)ctx->d_w2)->blk, ME_W2_BLOCK * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  ME_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  w2_result(h, out);
+  return ME_OK;
+}
+
+int run_w2(me_ctx *ctx, double voxel_size, int min_points, int scs_radius, me_w2_result *out, int64_t *n_rows, double **rows) {
+  std::memset(out, 0, sizeof(*out));
+  if (n_rows) *n_rows = 0;
+  if (rows) *rows = nullptr;
+  if (scs_radius < 0 || scs_radius > 64) return fail(ctx, ME_ERR_INVALID, "scs_radius out of range");
+  double *d_rows = nullptr;
+  ME_TRY(w2_begin_impl(ctx, voxel_size, min_points, rows != nullptr, &d_rows));
+  if (ctx->cloud[ME_CLOUD_EST].slab || ctx->cloud[ME_CLOUD_GT].slab) {
+    ctx->w2_open = false;
+    return fail(ctx, ME_ERR_INVALID, "slab layout: run the W2 stage as me_w2_begin / all-reduce of me_w2_w_table / "
+                                     "me_w2_finish_accum_device / all-reduce of me_w2_block / me_w2_fetch");
+  }
+  ME_TRY(w2_finish_block(ctx, scs_radius));
+  ME_TRY(w2_fetch(ctx, out));
+  if (n_rows) *n_rows = out->n_pairs;
+  if (rows) {
+    const size_t row_bytes = ME_W2_ROW_COLS * sizeof(double);
+    double *hr = (double *)std::malloc((size_t)std::max<int64_t>(out->n_pairs, 1) * row_bytes);
+    if (!hr) return fail(ctx, ME_ERR_NOMEM, "malloc(W2 rows) failed");
+    if (out->n_pairs > 0) {
+      const cudaError_t e = cudaMemcpyAsync(hr, d_rows, (size_t)out->n_pairs * row_bytes, cudaMemcpyDeviceToHost, ctx->stream);
+      if (e != cudaSuccess || cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
+        std::free(hr);
+        return fail(ctx, ME_ERR_CUDA, std::string("copying the W2 rows: ") + cudaGetErrorString(cudaGetLastError()));
+      }
+    }
+    *rows = hr;
+  }
+  return ME_OK;
+}
+
+// W2 and SCS on GIVEN Gaussians (ME_W2_ROW_COLS rows): the counterpart of awd_rows_kernel
+__global__ void __launch_bounds__(kThreads)
+w2_rows_kernel(const double *__restrict__ rows, long long n, const long long *__restrict__ vox_of_row, double *__restrict__ w_rows,
+               double *__restrict__ w_vox, uint32_t *__restrict__ pair_list, W2Acc *__restrict__ acc) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const double *r = rows + i * ME_W2_ROW_COLS;
+    double se[9], sg[9], o, b;
+    sym9(r + 11, se);
+    sym9(r + 17, sg);
+    w2_terms(r + 8, sg, r + 5, se, o, b);
+    const double w = sqrt(o * o + b * b);
+    w_rows[3 * i] = o; w_rows[3 * i + 1] = b; w_rows[3 * i + 2] = w;
+    w_vox[vox_of_row[i]] = w;
+    pair_list[i] = (uint32_t)vox_of_row[i];
+    atomicAdd(&acc->a.sum_w, w);
+    atomicAdd(&acc->sum_offset, o);
+    atomicAdd(&acc->sum_shape, b);
+    if (i == 0) acc->a.n_pairs = (unsigned long long)n;
+  }
+}
+
+int run_w2_rows(me_ctx *ctx, const double *rows, int64_t n_rows, double voxel_size, int scs_radius, double *w_out,
+                me_w2_result *out) {
+  std::memset(out, 0, sizeof(*out));
+  if (n_rows <= 0 || !rows || !(voxel_size > 0)) return fail(ctx, ME_ERR_INVALID, "bad arguments");
+  if (scs_radius < 0 || scs_radius > 64) return fail(ctx, ME_ERR_INVALID, "scs_radius out of range");
+  ctx->vox_open = false;      // the work buffer is reused below
+  ctx->w2_open = false;
+  ctx->w2_finished = false;
+  std::vector<long long> key(3 * (size_t)n_rows), vox((size_t)n_rows);
+  long long lo[3] = {LLONG_MAX, LLONG_MAX, LLONG_MAX}, hi[3] = {LLONG_MIN, LLONG_MIN, LLONG_MIN};
+  for (int64_t i = 0; i < n_rows; ++i)
+    for (int a = 0; a < 3; ++a) {
+      const long long k = llround(rows[i * ME_W2_ROW_COLS + a] / voxel_size);
+      key[3 * i + a] = k; lo[a] = std::min(lo[a], k); hi[a] = std::max(hi[a], k);
+    }
+  Lattice L;
+  std::memset(&L, 0, sizeof(L));
+  long long nvox = 1;
+  for (int a = 0; a < 3; ++a) {
+    if (hi[a] - lo[a] + 1 > 4096) return fail(ctx, ME_ERR_RANGE, "voxel keys span too large a box");
+    L.nvox[a] = (int)(hi[a] - lo[a] + 1); nvox *= L.nvox[a];
+  }
+  L.nvoxels = nvox; L.v = voxel_size;
+  for (int64_t i = 0; i < n_rows; ++i)
+    vox[i] = ((key[3 * i + 2] - lo[2]) * L.nvox[1] + (key[3 * i + 1] - lo[1])) * L.nvox[0] + (key[3 * i] - lo[0]);
+  auto align = [](size_t x) { return (x + 255) & ~(size_t)255; };
+  const size_t o_rows = 0, o_vox = o_rows + align((size_t)n_rows * ME_W2_ROW_COLS * 8), o_w = o_vox + align((size_t)n_rows * 8),
+               o_wv = o_w + align((size_t)n_rows * 3 * 8), o_pl = o_wv + align((size_t)nvox * 8), total = o_pl + align((size_t)n_rows * 4);
+  ME_TRY(ensure_work(ctx, total));
+  char *base = (char *)ctx->d_work;
+  double *d_rows = (double *)(base + o_rows), *d_w = (double *)(base + o_w), *d_wv = (double *)(base + o_wv);
+  long long *d_vox = (long long *)(base + o_vox);
+  uint32_t *d_pl = (uint32_t *)(base + o_pl);
+  W2Dev *d = nullptr;
+  ME_TRY(w2_state(ctx, &d));
+  ME_CUDA(ctx, cudaMemcpyAsync(d_rows, rows, (size_t)n_rows * ME_W2_ROW_COLS * 8, cudaMemcpyHostToDevice, ctx->stream));
+  ME_CUDA(ctx, cudaMemcpyAsync(d_vox, vox.data(), (size_t)n_rows * 8, cudaMemcpyHostToDevice, ctx->stream));
+  fill_nan_kernel<<<ctx->sm_count * 4, kThreads, 0, ctx->stream>>>(d_wv, nvox);
+  ME_LAUNCH_CHECK(ctx);
+  w2_rows_kernel<<<std::max(1, (int)std::min<long long>((n_rows + kThreads - 1) / kThreads, ctx->sm_count * 8)), kThreads, 0, ctx->stream>>>(
+      d_rows, n_rows, d_vox, d_w, d_wv, d_pl, &d->acc);
+  ME_LAUNCH_CHECK(ctx);
+  ME_TRY(launch_scs(ctx, L, d_wv, d_pl, scs_radius, &d->acc.a));
+  pack_w2_kernel<<<1, 32, 0, ctx->stream>>>(d);
+  ME_LAUNCH_CHECK(ctx);
+  ctx->w2_finished = true;
+  if (w_out) ME_CUDA(ctx, cudaMemcpyAsync(w_out, d_w, (size_t)n_rows * 3 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  return w2_fetch(ctx, out);
 }
 
 }  // namespace me

@@ -188,3 +188,20 @@ def allreduce_voxel_w(ctx, device, group=None):
     the W of the neighbouring ranks' voxels."""
     ptr, n = ctx.voxel_w_table()
     _reduce(ctx, ptr, 0, n, device, group, sync=False)
+
+
+def w2_distributed(ctx, device, voxel_size, min_points=100, scs_radius=5, group=None):
+    """The Gaussian 2-Wasserstein stage over every rank of the job (MapEvalB200.voxel_w2 for world > 1).  On a replicated
+    layout every rank computes the whole stage, with no collective.  On a slab layout every rank computes the voxels it
+    owns, then ONE in-place MAX all-reduce of the W2 table (-1 = no pair; every voxel has one owner), the SCS sweep over
+    its pairs, and ONE in-place SUM all-reduce of the stage's block (counts ride as fp64, exact).  Every rank returns the
+    same result."""
+    ctx.w2_begin(voxel_size, min_points)
+    if ctx.layout_active()["layout"] != A.ME_LAYOUT_SLAB:
+        ctx.w2_finish_accum_device(scs_radius)
+        return ctx.w2_fetch()
+    ptr, n = ctx.w2_w_table()
+    _reduce(ctx, ptr, 0, n, device, group)
+    ctx.w2_finish_accum_device(scs_radius)
+    _reduce(ctx, *ctx.w2_block(), 0, device, group)
+    return ctx.w2_fetch()

@@ -118,6 +118,10 @@ struct Param {   // map_eval.h:60-116
   double mom_region_size_ = 0.0;
   // the estimate alone: gt_map_path is neither read nor required; MME, local consistency and MOM run on the est cloud
   bool evaluate_without_gt_ = false;
+  // the Gaussian 2-Wasserstein distance per voxel at vmd_voxel_size (me_eval_w2, after calculateVMD): offset and shape terms,
+  // their means and SCS over W2, written to map_w2.txt and voxel_w2.txt; pairs need w2_min_points (>= 2) in each cloud
+  bool evaluate_w2_ = false;
+  int w2_min_points_ = 100;
 };
 
 // map_eval_main.cpp:120-208
@@ -233,6 +237,13 @@ inline Param loadParametersFromYAML(const std::string &yaml_file_path) {
       if (param.mom_region_size_ > 0.0 && !param.evaluate_mom_)
         throw std::runtime_error("mom_region_size needs evaluate_mom: true (it breaks the MOM call down by region)");
     }
+    if (config["evaluate_w2"]) param.evaluate_w2_ = config["evaluate_w2"].as<bool>();
+    if (config["w2_min_points"]) {
+      const double mp = config["w2_min_points"].as<double>();
+      if (!(mp >= 2.0 && mp <= 2147483647.0 && mp == std::floor(mp)))
+        throw std::runtime_error("w2_min_points must be an integer >= 2, not " + config["w2_min_points"].as<std::string>());
+      param.w2_min_points_ = (int)mp;
+    }
     return param;
   } catch (const std::exception &e) {
     std::cerr << "Error loading parameters: " << e.what() << std::endl;
@@ -267,7 +278,7 @@ inline void dumpParam(const Param &p, std::ostream &os) {
      << "\nsurface_normals_knn=" << p.surface_normals_knn_ << "\nevaluate_consistency=" << p.evaluate_consistency_
      << "\nconsistency_region_size=" << p.consistency_region_size_ << "\nevaluate_mom=" << p.evaluate_mom_
      << "\nmom_angle_deg=" << p.mom_angle_deg_ << "\nmom_planarity=" << p.mom_planarity_ << "\nmom_min_family=" << p.mom_min_family_
-     << "\nmom_region_size=" << p.mom_region_size_
+     << "\nmom_region_size=" << p.mom_region_size_ << "\nevaluate_w2=" << p.evaluate_w2_ << "\nw2_min_points=" << p.w2_min_points_
      << "\nevaluate_without_gt=" << p.evaluate_without_gt_ << "\n";
 }
 
@@ -348,7 +359,8 @@ class MapEvalB200 {
                         : !p.distance_quantiles_.empty() ? "distance_quantiles"
                         : p.region_size_ > 0.0 ? "region_size"
                         : p.drift_region_size_ > 0.0 ? "drift_region_size"
-                        : p.surface_metrics_ ? "surface_metrics" : nullptr;
+                        : p.surface_metrics_ ? "surface_metrics"
+                        : p.evaluate_w2_ ? "evaluate_w2" : nullptr;
       if (key) {
         *why = std::string(key) + " needs a ground truth; evaluate_without_gt evaluates the estimate alone";
         return false;
@@ -432,6 +444,7 @@ class MapEvalB200 {
   int surfaceMetrics();
   int localConsistency();
   int mom();
+  int voxelW2();
   int processWithoutGt();
   bool gt_mme() const { return param_.evaluate_gt_mme_ && !param_.evaluate_without_gt_; }
   int regionDrift();
@@ -542,6 +555,8 @@ inline int MapEvalB200::process() {
   }
   if (calculateVMD() != 0) return -1;
   if (param_.enable_debug) std::cout << "INFO: VMD calculation completed." << std::endl;
+  // on the lattices calculateVMD left aligned with vmd_voxel_size
+  if (param_.evaluate_w2_ && voxelW2() != 0) return -1;
   // after every consumer of the pass's NN records (the sweep may lay a cloud out again), with the estimate in its final frame
   if (param_.evaluate_consistency_ && localConsistency() != 0) return -1;
   if (param_.evaluate_mom_ && mom() != 0) return -1;
@@ -1324,6 +1339,49 @@ inline int MapEvalB200::calculateVMD() {
   scs_overall = awd_.scs;
   t_scs = ticToc.toc();
   std::cout << "INFO: Spatial Consistency Score (SCS): " << scs_overall << std::endl;
+  return 0;
+}
+
+// the Gaussian 2-Wasserstein distance per voxel (me_eval_w2 on GPU 0, as calculateVMD) -> map_w2.txt and voxel_w2.txt next to
+// map_results.txt
+inline int MapEvalB200::voxelW2() {
+  const double v = param_.vmd_voxel_size_;
+  me_w2_result res{};
+  int64_t n_rows = 0;
+  double *rows = nullptr;
+  if (me_eval_w2(ctx_, v, param_.w2_min_points_, 5, &res, &n_rows, &rows) != ME_OK) return fail("me_eval_w2");
+  std::vector<double> table(rows, rows + (size_t)n_rows * ME_W2_ROW_COLS);
+  me_free(rows);
+  const std::string path = results_subfolder + "map_w2.txt", rpath = results_subfolder + "voxel_w2.txt";
+  std::ofstream f(path);
+  if (!f.is_open()) {
+    std::cerr << "ERROR: cannot write " << path << std::endl;
+    return -1;
+  }
+  f << std::setprecision(17) << "# Gaussian 2-Wasserstein distance per voxel floor(x / v): W2 = sqrt(offset^2 + shape^2), offset = "
+       "|mu_est - mu_gt|, shape = Bures(Sigma_gt, Sigma_est), Sigma = M2 / (n - 1) (m); scs over W2 with radius 5; v = " << v
+    << ", min_points " << param_.w2_min_points_ << "; est in the ground truth's frame\n";
+  f << "aw2 mean_offset mean_shape scs n_pairs n_scs n_voxels_est n_voxels_gt\n" << std::fixed << std::setprecision(15)
+    << res.aw2 << " " << res.mean_offset << " " << res.mean_shape << " " << res.scs << " " << res.n_pairs << " " << res.n_scs << " "
+    << res.n_voxels_est << " " << res.n_voxels_gt << "\n";
+  std::ofstream rf(rpath);
+  if (!rf.is_open()) {
+    std::cerr << "ERROR: cannot write " << rpath << std::endl;
+    return -1;
+  }
+  rf << std::setprecision(17) << "# one row per voxel pair of map_w2.txt (sigma as xx xy xz yy yz zz, m^2); v = " << v << "\n";
+  rf << "min_x min_y min_z n_gt n_est mu_est_x mu_est_y mu_est_z mu_gt_x mu_gt_y mu_gt_z sig_est_xx sig_est_xy sig_est_xz "
+        "sig_est_yy sig_est_yz sig_est_zz sig_gt_xx sig_gt_xy sig_gt_xz sig_gt_yy sig_gt_yz sig_gt_zz offset shape w2\n";
+  for (int64_t r = 0; r < n_rows; ++r) {
+    const double *x = table.data() + r * ME_W2_ROW_COLS;
+    for (int c = 0; c < ME_W2_ROW_COLS; ++c) {
+      if (c == 3 || c == 4) rf << (long long)x[c];
+      else rf << x[c];
+      rf << (c + 1 == ME_W2_ROW_COLS ? "\n" : " ");
+    }
+  }
+  std::cout << "INFO: Gaussian 2-Wasserstein: AW2 " << res.aw2 << " m (offset " << res.mean_offset << ", shape " << res.mean_shape
+            << "), SCS " << res.scs << ", " << res.n_pairs << " pairs; saved to " << path << " and " << rpath << std::endl;
   return 0;
 }
 

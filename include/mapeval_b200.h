@@ -814,6 +814,46 @@ ME_API int  me_awd_from_rows(me_ctx *ctx, const double *rows27, int64_t n_rows, 
                       double *w_out, me_awd_result *out);
 ME_API void me_free(void *p);
 
+/* ---- the Gaussian 2-Wasserstein distance per voxel (no reference counterpart; DESIGN §3.18) -----------------------------
+ * Voxels floor(x / v) as for AWD; a voxel is paired when it is occupied in both clouds with >= min_points (>= 2) points in
+ * each.  Per pair: mu = the mean of the voxel's points, Sigma = M2 / (n - 1) (unbiased, no clamp), offset o = |mu_est -
+ * mu_gt|, shape b = Bures(Sigma_gt, Sigma_est) with b^2 = tr Sigma_gt + tr Sigma_est - 2 tr((Sigma_gt^1/2 Sigma_est
+ * Sigma_gt^1/2)^1/2), W2 = sqrt(o^2 + b^2), symmetric in the two clouds.  b is taken as the residual |A - B P Q^T|_F of the
+ * square roots A = Sigma_gt^1/2, B = Sigma_est^1/2 and the SVD B A = P S Q^T, in which nothing cancels: on an exact copy of
+ * the ground truth it is at the rounding of the moments, where the trace formula leaves ~sqrt(u tr Sigma).  SCS is the
+ * AWD stage's rule over W2.  Everything runs in fp64. */
+#define ME_W2_ROW_COLS 26     /* vmin[3] n_gt n_est mu_est[3] mu_gt[3] sigma_est[6] sigma_gt[6] offset shape w2;
+                                 sigma as xx xy xz yy yz zz */
+#define ME_W2_BLOCK 8         /* the SUM-reducible block: n_pairs n_scs n_voxels_est n_voxels_gt sum_w2 sum_scs
+                                 sum_offset sum_shape */
+typedef struct {
+  double  aw2;                       /* mean of W2 over the pairs (NaN without pairs)                                  */
+  double  mean_offset, mean_shape;   /* means of o and b over the pairs                                                */
+  double  scs;                       /* SCS over W2: population std / mean of the paired neighbours' W2, mean over the
+                                        voxels that have any (NaN if none)                                             */
+  int64_t n_pairs, n_scs;
+  int64_t n_voxels_est, n_voxels_gt; /* occupied voxels of each cloud                                                  */
+} me_w2_result;
+/* One call on a replicated layout.  rows (nullable): library-allocated n_rows x ME_W2_ROW_COLS, one row per pair, release
+ * with me_free.  min_points < 2 or voxel_size <= 0: ME_ERR_INVALID; more than 2^31 voxels: ME_ERR_RANGE. */
+ME_API int  me_eval_w2(me_ctx *ctx, double voxel_size, int32_t min_points, int32_t scs_radius, me_w2_result *out,
+                       int64_t *n_rows, double **rows);
+/* W2 and SCS on GIVEN Gaussians: rows = n_rows x ME_W2_ROW_COLS (vmin, mu and sigma are read; n, offset, shape and w2 are
+ * not).  w_out (nullable): n_rows x 3 = offset, shape, w2 per row.  The counterpart of me_awd_from_rows. */
+ME_API int  me_w2_from_rows(me_ctx *ctx, const double *rows, int64_t n_rows, double voxel_size, int32_t scs_radius,
+                            double *w_out, me_w2_result *out);
+/* The stage in halves, for either layout (the pattern of me_voxel_begin): me_w2_begin computes the Gaussians and W2 of the
+ * voxels this rank owns; me_w2_w_table hands out the DEVICE W2 table over the estimated cloud's voxels (no pair: NaN, or
+ * -1 on an active slab layout, where the caller MAX-all-reduces it in place); me_w2_finish_accum_device runs SCS over this rank's
+ * pairs and fills the stage's block; me_w2_block hands it out (*n = ME_W2_BLOCK fp64 values, SUM-reduce them all);
+ * me_w2_fetch decodes it.  The stage shares the voxel stage's work buffer: a me_voxel_begin closes an open W2 stage and
+ * the other way round. */
+ME_API int  me_w2_begin(me_ctx *ctx, double voxel_size, int32_t min_points);
+ME_API int  me_w2_w_table(me_ctx *ctx, double **device_w, int64_t *n);
+ME_API int  me_w2_finish_accum_device(me_ctx *ctx, int32_t scs_radius);
+ME_API int  me_w2_block(me_ctx *ctx, double **device_block, int32_t *n);
+ME_API int  me_w2_fetch(me_ctx *ctx, me_w2_result *out);
+
 /* timing of the last call of each stage in milliseconds (CUDA events on the context's stream):
  * [0] grid est [1] grid gt [2] nn est->gt [3] nn gt->est [4] mme est [5] mme gt [6] voxel moments [7] awd [8] scs */
 #define ME_N_STAGE_TIMES 9
